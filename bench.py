@@ -1,7 +1,8 @@
-"""bench.py -- train-step throughput of the B200-native MIDIModel (BASELINE.json configs[1]).
+"""bench.py -- train-step throughput of the CUDA-native MIDIModel on one H100 (BASELINE.json configs[1]).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference|reference-gpu]
                     [--api fused|dropin] [--model tv2o-medium|tv2o-large|...] [--events S] [--batch B]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
            --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -14,8 +15,8 @@ Default workload = BASELINE.json configs[1]: tv2o-medium, B=8, S=2048.  Metric: 
   value : device-timed (CUDA events, max over ranks), batches already resident in HBM
   e2e   : same step through the public API with the batch in pinned HOST memory: H2D copy of the
           batch and D2H read of the loss inside the timed region, every step
-  roofline     : aggregate of all tcgen05 GEMM launches of the timed steps (CUDA events around each
-                 launch on the launching stream): algorithmic FLOPs / measured time vs measured bf16 peak
+  roofline     : aggregate of all tensor-core GEMM launches of the timed steps (CUDA events around each
+                 launch on the launching stream): algorithmic FLOPs / measured time vs the bf16 peak
   hbm_kernels  : the memory-bound kernels of the step (norm / RoPE / SwiGLU / CE / AdamW / sampler) timed alone on
                  bench-shape tensors: algorithmic bytes / time vs the measured copy bandwidth
   generate     : BASELINE's second metric, events/s of the KV-cached generate loop, with its HBM roofline
@@ -29,8 +30,13 @@ Arms:
   --impl reference          the reference's CPU path (oracle port; the reference is pure Python and cannot travel).
   --impl reference-gpu      the reference's own GPU path on the same box: HF LlamaModel eager bf16 + torch SDPA +
                             F.cross_entropy + torch fused AdamW (midi_model.py:102-150, train.py:121-138,168-188) --
-                            cuBLAS / ATen kernels only, nothing of this repo's engine.  The comparator the sm_100a
-                            kernels have to beat (BASELINE.md section 4).
+                            cuBLAS / ATen kernels only, nothing of this repo's engine.  The comparator the native
+                            kernels have to beat.
+
+--steps K / --warmup W: timed and warm-up steps of the measured arm, used exactly as given (every arm).
+--dump-outputs DIR (native arm): after the timed steps, what the last timed step computed -- the loss, and a fixed,
+seeded sample of the parameter gradients and of the updated parameters -- is written as DIR/<name>.npy (float32).
+Weights and batches are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -64,7 +70,8 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data-sheet"
 
 
 def model_dims(name: str):
@@ -74,7 +81,7 @@ def model_dims(name: str):
 
 
 def train_flops_per_token(model: str, S: int) -> float:
-    """SURVEY.md Appendix C: forward 861.6 MFLOP/event for tv2o-medium at S=2048 (GEMMs + causal attention), x3."""
+    """Forward 861.6 MFLOP/event for tv2o-medium at S=2048 (GEMMs + causal attention), x3."""
     H, V = 1024, 3406
     n_o, n_i = model_dims(model)
     outer = n_o * (4 * 2 * H * H + 3 * 2 * H * 4096 + 2 * 2 * H * (S + 1) / 2)
@@ -160,8 +167,7 @@ def make_timed(world, dev, launch_counter=None):
 # CPU arm: the oracle's train step (fp32 eager PyTorch + torch AdamW), bounded sample
 # ---------------------------------------------------------------------------------------------
 def cpu_threads() -> int:
-    # eager PyTorch at B=1 does not scale past a few dozen threads (profiles/r2_cpu_thread_sweep.txt: the 128-thread GPU
-    # host is several times SLOWER with all threads than with 16): use up to 16 and report that count
+    # eager PyTorch at B=1 does not scale past a few dozen threads: use up to 16 and report that count
     return min(os.cpu_count() or 1, int(os.environ.get("B200_CPU_THREADS", "16")))
 
 
@@ -225,7 +231,7 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return 0
-    steps, warmup = max(1, min(args.steps, 6)), max(1, min(args.warmup, 2))
+    steps, warmup = args.steps, args.warmup
     v, ms, cores, sample = cpu_train_step_tokens_per_s(args.model, steps, warmup)
     line = {"impl": "reference", "metric": METRIC, "value": v, "unit": UNIT, "n_gpus": args.gpus, "steps": steps,
             "warmup": warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -309,7 +315,7 @@ def run_reference_gpu(args):
         return loss
 
     timed = make_timed(world, dev)
-    W, K = max(3, args.warmup), max(1, args.steps)
+    W, K = args.warmup, args.steps
     for i in range(W):
         step(resident[i % n_batches])
     sampler = ClockSampler(local)
@@ -360,7 +366,7 @@ def run_native(args):
 
     world, rank, local = dist_env()
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback; use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device (the native path has no CPU fallback; use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -433,7 +439,7 @@ def run_native(args):
             return loss
 
     timed = make_timed(world, dev, lambda: lib.query("b200_launch_count"))
-    W, K = max(3, args.warmup), max(1, args.steps)
+    W, K = args.warmup, args.steps
     for i in range(W):
         step(resident[i % n_batches])
     torch.cuda.synchronize()
@@ -441,7 +447,14 @@ def run_native(args):
     sampler = ClockSampler(local)
     sampler.start()
     time.sleep(0.3)
-    ms_total, launches, t0, t1 = timed(lambda i: step(resident[i % n_batches]), K)      # the timed region (`value`)
+    last = {}
+
+    def timed_step(i):
+        last["loss"] = step(resident[i % n_batches])
+
+    ms_total, launches, t0, t1 = timed(timed_step, K)      # the timed region (`value`)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, last["loss"])
     # Roofline pass: the same K steps again with CUDA events around every GEMM launch.  It runs single-stream (the
     # weight-gradient GEMMs of the timed region run on a side stream under the HBM-bound kernels, where an event pair
     # would time the co-running kernels too), so `achieved` is each GEMM's own duration inside a full step.
@@ -502,16 +515,15 @@ def run_native(args):
                    "api": api_note,
                    "global_batch": world * B_PER_GPU, "n_events": S_EVENTS, "tokens_per_event": T_TOK,
                    "parallelism": f"dp{world}", "weights": "seeded-init (torch.manual_seed(0))",
-                   "l2": "per-step working set ~20 GB >> 126 MB L2 (no explicit flush needed); 4 distinct batches cycled"},
+                   "l2": "per-step working set ~20 GB >> 50 MB L2 (no explicit flush needed); 4 distinct batches cycled"},
         "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": ms_e2e / K,
                 "h2d_bytes_per_step": int(host16[0].numel() * host16[0].element_size()), "d2h_bytes_per_step": 4,
                 "last_loss": losses[-1] if losses else None},
         "gpu_launches": int(launches),
         "clocks": clocks,
         "roofline": {"bound": "tensor", "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s",
-                     "frac": ach_tf / peak_tf if peak_tf else None, "traffic": gemm_traffic() if default_workload else None,
-                     "traffic_unit": "DRAM bytes (read+write) per GEMM launch, ncu capture of this command (profiles/*_gemm_traffic.json)",
-                     "kernel": "gemm_tcgen05_kernel (every launch of K steps, CUDA events on the launching stream; single-stream pass of the same steps)", "peak_kind": f"{pk_kind} sustained cuBLAS bf16",
+                     "frac": ach_tf / peak_tf if peak_tf else None,
+                     "kernel": "gemm_wgmma_kernel (every launch of K steps, CUDA events on the launching stream; single-stream pass of the same steps)", "peak_kind": f"{pk_kind} bf16",
                      "gemm_ms_per_step": gemm_ms / K, "gemm_share_of_step": gemm_ms / ms_prof if ms_prof else None,
                      "profile_pass_ms_per_step": ms_prof / K, "wgrad_side_stream_in_timed_region": bool(wg_stream),
                      "whole_step_model_tflops": step_tf, "whole_step_frac": step_tf / peak_tf if peak_tf else None,
@@ -519,9 +531,9 @@ def run_native(args):
         "peak_mem_gb": torch.cuda.max_memory_allocated() / 2 ** 30,
     }
     if not args.no_hbm_kernels and default_workload:
-        line["hbm_kernels"] = hbm_kernels_leg(model, dev, float(pk.get("hbm_gbs", 6586.4)), pk_kind)
+        line["hbm_kernels"] = hbm_kernels_leg(model, dev, float(pk.get("hbm_gbs", 3350.0)), pk_kind)
     if not args.no_generate and default_workload:
-        line["generate"] = generate_leg(model, dev, world, rank, float(pk.get("hbm_gbs", 6586.4)),
+        line["generate"] = generate_leg(model, dev, world, rank, float(pk.get("hbm_gbs", 3350.0)),
                                         cpu=(world == 1 and not args.no_cpu_baseline))
     if world == 1 and not args.no_cpu_baseline:
         v, ms, cores, sample = cpu_train_step_tokens_per_s(args.model, 3, 1)
@@ -534,22 +546,26 @@ def run_native(args):
     return 0
 
 
-def gemm_traffic():
-    """DRAM bytes (read + write) per GEMM launch from the committed ncu capture of this same command (newest
-    profiles/r*_gemm_traffic.json, derived from that round's launch list); None when no capture is committed."""
-    import glob
-    for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_gemm_traffic.json")), reverse=True):
-        try:
-            with open(path) as f:
-                return float(json.load(f)["dram_bytes_per_launch"])
-        except (OSError, KeyError, ValueError):
-            continue
-    return None
+def dump_outputs(out_dir: str, model, loss, sample: int = 1 << 21):
+    """Write what the last timed step computed: the loss, and the same seeded sample of `sample` indices of the flat
+    parameter-gradient and updated-parameter buffers (float32, 2 x 8 MB at the default; indices as float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    rt = model._rt()
+    flat, gflat = rt.store.flat, rt.store.gflat
+    g = torch.Generator().manual_seed(20240601)
+    n = flat.numel()
+    idx = torch.randint(0, n, (min(sample, n),), generator=g).unique().to(flat.device)   # sorted, seeded, O(sample)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss)], dtype=np.float32))
+    np.save(os.path.join(out_dir, "grads_sample.npy"), gflat[idx].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat[idx].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "sample_index.npy"), idx.cpu().numpy().astype(np.float64))
 
 
 def hbm_kernels_leg(model, dev, peak_gbs, pk_kind):
     """The memory-bound kernels of the path, each timed alone (CUDA events, 3 warm-up + 10 launches cycling through
-    input sets larger than the 126 MB L2) on the tensors it sees in the benchmark step: achieved = algorithmic bytes
+    input sets larger than the 50 MB L2) on the tensors it sees in the benchmark step: achieved = algorithmic bytes
     (every operand read once + every result written once) / time, against the measured copy bandwidth."""
     from midi_b200 import decode as dec, lib, ops
     BF = torch.bfloat16
@@ -636,7 +652,7 @@ def generate_leg(model, dev, world, rank, peak_gbs, cpu=False):
     """BASELINE.json's second metric: events/s of the KV-cached generate loop (midi_model.py:167-250) with the
     reference's default sampling (temp 1.0, top-p 0.98, top-k 20), from one BOS event; replicas only across GPUs
     (each rank generates its own rows, no collective).  EOS stopping is disabled so the event count is fixed
-    (seeded-init weights emit EOS at random).  Roofline (SURVEY.md 8d): HBM bytes one event step has to move =
+    (seeded-init weights emit EOS at random).  Roofline: HBM bytes one event step has to move =
     event-level layer weights + token-level layer weights + lm_head (the 8 token steps re-read theirs from L2) + the KV
     cache of the mean context, / measured copy bandwidth."""
     import torch.distributed as dist
@@ -701,7 +717,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-generate", action="store_true")
     ap.add_argument("--no-hbm-kernels", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (native arm)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         return run_reference(args)
     if args.impl == "reference-gpu":

@@ -1,4 +1,4 @@
-/* midi_b200.h -- C ABI of libmidi_b200.so: the sm_100a kernels behind the drop-in MIDIModel.
+/* midi_b200.h -- C ABI of libmidi_b200.so: the sm_90a (H100) kernels behind the drop-in MIDIModel.
  *
  * The reference (SkyTNT/midi-model) has no FFI: its hot path is the Python class
  * `MIDIModel` (midi_model.py:99-250) whose arithmetic is delegated to HF transformers /
@@ -83,7 +83,7 @@ int b200_swiglu_bwd(const void* gu, const void* dact, void* dgu, long long rows,
  *      epilogue, and the four gradient GEMMs (midi_b200/engine.py::StackEngine._lora_fwd/_lora_bwd). */
 int b200_scale_bf16(const void* x, void* y, long long n, float scale, cudaStream_t s);
 
-/* ---- tensor-core GEMM (tcgen05 / TMEM / TMA): every nn.Linear of hf modeling_llama.py:177-184,
+/* ---- tensor-core GEMM (wgmma / TMA): every nn.Linear of hf modeling_llama.py:177-184,
  *      238-264, 288 and lm_head (midi_model.py:135), plus their dgrad / wgrad.
  *      C[M,N] = A . B^T, fp32 accumulate, bf16 out.  a_mn_major / b_mn_major = operand stored [K, rows].
  *      R != NULL: C = bf16(bf16(acc) + R) (residual add, hf :325 / :331).
@@ -113,26 +113,22 @@ int b200_gemm_bf16_swiglu(const void* A, const void* Wgu, void* gu, void* act, i
 int b200_attn_causal_fwd(const void* q, const void* k, const void* v, void* o, float* lse /*may be NULL*/,
                          const long long* strides /*4x3: q,k,v,o*/, int batch, int n_heads, int Sq, int Sk, int head_dim,
                          float scale, cudaStream_t s);
-/*      same contract on the tcgen05 tensor cores (TMA-staged 128-key K/V tiles, S and P.V accumulators in TMEM);
- *      heads must be contiguous blocks of 64 columns (strides[.h] == 64) */
-int b200_attn_causal_fwd_tc(const void* q, const void* k, const void* v, void* o, float* lse /*may be NULL*/,
-                            const long long* strides /*4x3: q,k,v,o*/, int batch, int n_heads, int Sq, int Sk, int head_dim,
-                            float scale, cudaStream_t s);
 int b200_attn_causal_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                          float* delta /*float[batch*n_heads*Sq]*/, void* dq, void* dk, void* dv,
                          const long long* strides /*8x3: q,k,v,o,do,dq,dk,dv*/, int batch, int n_heads, int Sq, int Sk,
                          int head_dim, float scale, const void* rope_cos /*may be NULL: fuse RoPE backward into dq, dk*/,
                          const void* rope_sin, cudaStream_t s);
-/*      backward on tcgen05 (5 UMMA groups per tile pair, dQ accumulated in fp32 with red.global); training shapes only */
-size_t b200_attn_causal_bwd_tc_workspace_bytes(int batch, int n_heads, int Sq);
-int b200_attn_causal_bwd_tc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                            void* dq, void* dk, void* dv, const long long* strides /*8x3: q,k,v,o,do,dq,dk,dv*/, int batch,
-                            int n_heads, int Sq, int Sk, int head_dim, float scale, const void* rope_cos /*may be NULL*/,
-                            const void* rope_sin, void* workspace, size_t workspace_bytes, cudaStream_t s);
-/*      tuning hook, device buffer of 128 int64 (NULL = off): while set, b200_attn_causal_fwd_tc launches its instrumented
-        instantiation, which adds per-phase clock64 sums of the softmax warps into buf[group*16 + phase] (tools/attn_fwd_profile.py),
-        and the split dQ kernel writes a clock64 trace of CTA (0,0) */
-void b200_attn_debug_trace(long long* buf);
+/*      the same two contracts on the Hopper tensor cores (wgmma, TMA-staged 64 x 64 tiles, mbarrier double buffering);
+ *      heads must be contiguous blocks of 64 columns (strides[.h] == 64).  The training path uses these; the mma.sync
+ *      kernels above are the second implementation the tests compare against. */
+int b200_attn_causal_fwd_wgmma(const void* q, const void* k, const void* v, void* o, float* lse /*may be NULL*/,
+                               const long long* strides /*4x3: q,k,v,o*/, int batch, int n_heads, int Sq, int Sk,
+                               int head_dim, float scale, cudaStream_t s);
+int b200_attn_causal_bwd_wgmma(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                               float* delta /*float[batch*n_heads*Sq]*/, void* dq, void* dk, void* dv,
+                               const long long* strides /*8x3: q,k,v,o,do,dq,dk,dv*/, int batch, int n_heads, int Sq,
+                               int Sk, int head_dim, float scale, const void* rope_cos /*may be NULL*/,
+                               const void* rope_sin, cudaStream_t s);
 /*      inner stack: L <= 8 positions per event, head_dim 256, packed qkv rows [n_events*L, ld_qkv]. */
 /*      rope_cos/sin != NULL: qkv holds PRE-RoPE projections; q and k are rotated in place (fused RoPE) before use */
 int b200_attn_tiny_fwd(void* qkv, void* out, int n_events, int L, int n_heads, int head_dim, int ld_qkv, int ld_out,

@@ -1,9 +1,9 @@
-"""Build libmidi_b200.so (all CUDA kernels + the C ABI) in-tree with nvcc for sm_100a.
+"""Build libmidi_b200.so (all CUDA kernels + the C ABI) in-tree with nvcc for sm_90a (H100).
 
     python midi-model_b200/build_ext.py [--force]
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the
-repo snapshot.  Objects are rebuilt only when their source (or a header) is newer.
+nvcc cross-compiles without a GPU; the .so and the objects are build products (git-ignored).
+Objects are rebuilt only when their source (or a header) is newer.
 """
 from __future__ import annotations
 
@@ -17,8 +17,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "midi_b200", "libmidi_b200.so")
-SOURCES = ["runtime.cu", "elementwise.cu", "gemm_tcgen05.cu", "attn_flash.cu", "attn_tc05.cu", "attn_tiny.cu", "train_misc.cu", "decode.cu", "decode_persist.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+SOURCES = ["runtime.cu", "elementwise.cu", "gemm_wgmma.cu", "attn_flash.cu", "attn_wgmma.cu", "attn_tiny.cu", "train_misc.cu", "decode.cu", "decode_persist.cu"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--threads", "2"]
 
 
@@ -59,7 +60,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
         with ThreadPoolExecutor(max_workers=min(4, len(jobs))) as ex:
             list(ex.map(run, jobs))
     if jobs or force or not os.path.exists(LIB):
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs]
+        cmd = [nvcc, "-shared", *ARCH, "-o", LIB, *objs]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,6 +1,6 @@
 // Causal attention for the outer event stack (head_dim 64; hf sdpa_attention.py:92-101 called
 // from modeling_llama.py:251-289 with is_causal=True, scale = d^-1/2), FlashAttention-style:
-// online softmax in fp32, P rounded to bf16 for P.V, output rounded to bf16 (Appendix A.5).
+// online softmax in fp32, P rounded to bf16 for P.V, output rounded to bf16 (DESIGN.md 3.3).
 //   fwd      : CTA = 64 query rows x (batch, head); K/V tiles of 64 keys double-buffered by cp.async
 //   bwd dK/dV: CTA = 64 keys  x (batch, head), loops over query tiles      (no atomics, deterministic)
 //   bwd dQ   : CTA = 64 query rows x (batch, head), loops over key tiles
@@ -563,7 +563,7 @@ extern "C" int b200_attn_causal_fwd(const void* q, const void* k, const void* v,
     return B200_OK;
 }
 
-// delta[b,h,q] = rowsum(dO * O): shared by the mma.sync and the tcgen05 backward paths
+// delta[b,h,q] = rowsum(dO * O)
 int b200_attn_bwd_delta_launch(const void* o, const void* d_o, float* delta, const long long* so, const long long* sdo,
                                int batch, int n_heads, int Sq, cudaStream_t stream) {
     B200_CHECK_ARG(n_heads % 4 == 0, "attn bwd: n_heads must be a multiple of 4");

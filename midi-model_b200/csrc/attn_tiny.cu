@@ -2,7 +2,7 @@
 // L <= 8 positions with head_dim 256 (midi_model.py:116-135 -> hf sdpa, scale 1/16).  A flash
 // tile would be >= 94 % padding, so one warp owns one (event, head): each lane holds an
 // 8-wide slice of d for all L rows in registers, the L(L+1)/2 scores are reduced with warp
-// shuffles, softmax is fp32, P is rounded to bf16 before P.V (flash semantics, Appendix A.5).
+// shuffles, softmax is fp32, P is rounded to bf16 before P.V (flash semantics, DESIGN.md 3.3).
 // HBM-bound: reads the packed qkv rows once, writes the output once.
 #include "common.cuh"
 

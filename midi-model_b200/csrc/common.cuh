@@ -1,4 +1,4 @@
-// Common device/host helpers for the sm_100a kernels of the MIDIModel hot path.
+// Common device/host helpers for the sm_90a kernels of the MIDIModel hot path.
 // Everything here is plain CUDA C++ + inline PTX (no CUTLASS / no torch types).
 #pragma once
 #include <cuda.h>
@@ -57,7 +57,7 @@ int b200_num_sms();
 
 // Programmatic dependent launch (PDL).  Kernels that run right before a tensor-core GEMM execute
 // `griddepcontrol.launch_dependents` first thing: a GEMM launched with the programmatic-serialization attribute may then be
-// scheduled onto SMs as they drain and run its prologue (barrier init, TMEM allocation, tensor-map prefetch) under this
+// scheduled onto SMs as they drain and run its prologue (barrier init, tensor-map prefetch) under this
 // kernel's tail; it touches no memory before its own `griddepcontrol.wait`, which returns only once this grid has completed
 // and flushed.  Without the launch attribute on the next kernel both instructions are no-ops.
 #define B200_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")

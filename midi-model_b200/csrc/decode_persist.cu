@@ -4,15 +4,14 @@
 // dependent phases instead of a kernel boundary.  Per layer: norm+QKV | RoPE+append+attention | (combine) |
 // o_proj+residual | norm+gate/up+SwiGLU | down+residual; per token: ... | final norm+lm_head | sample.
 //
-// Why: at batch 1 a decode step moves < 0.5 GB (70 us at HBM speed) but the launch-per-phase loop needs ~210 graph nodes
-// per event at ~5.8 us each (round-1 profile: 1.22 ms / event).  Here a phase boundary costs one L2 round trip, and each
+// Why: at batch 1 a decode step moves < 0.5 GB (~150 us at H100 HBM speed) but the launch-per-phase loop needs ~210 graph nodes
+// per event, each a launch with its own fixed cost.  Here a phase boundary is a grid barrier instead, and each
 // warp issues the loads of its first weight rows of the NEXT phase before it waits at the barrier (weights do not depend
 // on the previous phase), so the HBM latency of every phase hides behind the barrier.
 //
-// Measured notes (profiles/r2_decode_*): a bare grid barrier of 148 x 512 threads costs ~2 300 cycles
-// (tools/micro/gridbar_bench.cu) and waits for the issuing SM's outstanding loads, so a phase boundary is ~1.2 us, not the
-// L2 round trip; a variant with the phases as shared non-inlined routines (smaller instruction footprint) plus bulk L2
-// prefetch of the event-level weights was 25 % SLOWER at batch 1 (argument structs in local memory, calls) and was dropped.
+// A grid barrier waits for the issuing SM's outstanding loads (tools/micro/gridbar_bench.cu measures its cost), so a
+// phase boundary costs more than one L2 round trip.  The phases stay inlined: shared non-inlined routines put their
+// argument structs in local memory.
 //
 // Arithmetic and rounding points are those of the launch-per-phase kernels in decode.cu (same per-row accumulation
 // order in the projections; attention differs only in how the context is cut into chunks).
@@ -70,8 +69,8 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
 }
 __device__ __forceinline__ uint4 ldcg16(const void* p) { return __ldcg(reinterpret_cast<const uint4*>(p)); }
 // weights: read-only for the whole launch.  Event-level weights (403 MB) are streamed once per event -> evict first, so
-// that the token-level weights (51 MB, re-read by each of the 8 token steps) stay in the 126 MB L2.
-// (L2 eviction priority through a createpolicy cache hint: the plain .L2::evict_* qualifiers need 256-bit loads on sm_100.)
+// that as much as possible of the token-level weights (51 MB, re-read by each of the 8 token steps) stays in the 50 MB L2.
+// (L2 eviction priority through a createpolicy cache hint.)
 __device__ __forceinline__ unsigned long long l2_policy(bool keep) {
     unsigned long long pol;
     if (keep) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));

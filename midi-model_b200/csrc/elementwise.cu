@@ -1,7 +1,7 @@
 // HBM-bound kernels of the MIDIModel hot path: embedding gather-sum (midi_model.py:145-146),
 // inner-input builder (midi_model.py:126-131), RMSNorm (hf modeling_llama.py:62-67), RoPE
 // (hf :124-168), SwiGLU (hf :183), and their backward passes.  All arithmetic is fp32 on
-// bf16 storage with the reference's rounding points (SURVEY.md Appendix A).  16-byte vector
+// bf16 storage with the reference's rounding points (DESIGN.md 3.3).  16-byte vector
 // accesses, one 128-thread CTA per row (rows are 2 KB at hidden=1024), grids sized in rows.
 #include "common.cuh"
 
@@ -13,7 +13,7 @@ constexpr int MAXV = 8;   // vectors of 8 bf16 per thread: hidden <= 128*8*8 = 8
 // ---------------------------------------------------------------------------
 // embedding
 // ---------------------------------------------------------------------------
-// out[m, :] = bf16( sum_t fp32(table[ids[m, t], :]) )   -- one rounding (Appendix A.1)
+// out[m, :] = bf16( sum_t fp32(table[ids[m, t], :]) )   -- one rounding (DESIGN.md 3.3)
 __global__ void embed_sum_fwd_kernel(const long long* __restrict__ ids, const bf16* __restrict__ table,
                                      bf16* __restrict__ out, int T, int H, int V) {
     const int m = blockIdx.x;
@@ -178,7 +178,7 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
     return t;
 }
 
-// y = w * bf16(x * rsqrt(mean(x^2) + eps))  -- two roundings (Appendix A.2)
+// y = w * bf16(x * rsqrt(mean(x^2) + eps))  -- two roundings (DESIGN.md 3.3)
 template <int VPT>
 __global__ void __launch_bounds__(ROW_THREADS)
 rmsnorm_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, bf16* __restrict__ y,

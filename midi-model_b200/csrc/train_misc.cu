@@ -67,8 +67,7 @@ ce_fwd_kernel(const bf16* __restrict__ logits, const long long* __restrict__ tar
 
 // Warp-per-row variant: the whole row (<= 16 vectors of 8 per lane, i.e. V <= 4096) is loaded ONCE into registers with all
 // loads in flight, max and sum-of-exponentials are then two passes over registers, reductions are shuffles (no block
-// barrier).  The CTA-per-row kernel above re-read the row and went through four __syncthreads per 6.8 KB row: 0.28 of the
-// copy bandwidth (profiles/r2_bench_1gpu_start.json).
+// barrier).  The CTA-per-row kernel above re-reads the row and goes through four __syncthreads per 6.8 KB row.
 constexpr int CEW_WARPS = 4;
 template <int VPL>
 __global__ void __launch_bounds__(CEW_WARPS * 32, 8)

@@ -1,4 +1,4 @@
-"""Host data path of the train step (train.py:31-90, 408-425), B200 side.
+"""Host data path of the train step (train.py:31-90, 408-425), GPU side.
 
 The reference dataset keeps every tokenised MIDI file as an int16 matrix `[events, max_token_seq]` (train.py:71), widens it
 to int64 on the host, pads to the longest sample of the batch with `pad_id` (`collate_fn`, train.py:82-86) and lets the

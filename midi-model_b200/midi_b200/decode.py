@@ -63,7 +63,7 @@ class PagedKV:
 
 
 def _linear(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """nn.Linear on a few rows: weight-streaming skinny GEMM for <= 16 rows, tcgen05 GEMM otherwise."""
+    """nn.Linear on a few rows: weight-streaming skinny GEMM for <= 16 rows, tensor-core GEMM otherwise."""
     M, K = x.shape
     N = w.shape[0]
     if M > 16:

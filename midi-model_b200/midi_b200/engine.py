@@ -1,14 +1,14 @@
-"""Layer-by-layer execution of the two Llama stacks of MIDIModel on the sm_100a kernels.
+"""Layer-by-layer execution of the two Llama stacks of MIDIModel on the sm_90a kernels.
 
 `ParamStore` keeps every parameter (and gradient) of the model as a view into ONE flat bf16
 buffer, in `named_parameters()` order.  Because q/k/v and gate/up projections are adjacent in
 that order, the fused `[3H, H]` QKV and `[2I, H]` gate|up weights are *views* -- the reference's
-`state_dict` keys stay the source of truth (SURVEY.md section 5, checkpoint row) and no packed
+`state_dict` keys stay the source of truth and no packed
 copies exist.  One flat gradient buffer means one all-reduce and one AdamW launch per step.
 
 `StackEngine` runs forward (saving exactly what backward needs) and an explicit backward; there
 is no autograd graph inside -- `autograd.Function`s in midi_model.py wrap whole stacks.
-Math per layer: hf modeling_llama.py:303-332; rounding points: SURVEY.md Appendix A.
+Math per layer: hf modeling_llama.py:303-332; rounding points: DESIGN.md 3.3.
 """
 from __future__ import annotations
 
@@ -24,18 +24,13 @@ import os
 
 BF16 = torch.bfloat16
 # RoPE backward is fused into the attention backward kernels (B200_FUSE_ROPE=0 -> stand-alone kernel).
-# The forward fusion into the QKV GEMM epilogue exists (ops.linear_rope, bit-identical, per-thread or TMA-staged stores)
-# but is OFF by default: four epilogue warps doing the rotation outlast the K=1024 main loop.  Measured A/B on one box
-# with the staged epilogue: +0.2 ms/step against the HBM-roofline stand-alone kernel (QKV GEMM 1213 -> 843 TFLOP/s with
-# the earlier per-thread stores).
+# The forward fusion into the QKV GEMM epilogue exists (ops.linear_rope, bit-identical) but is OFF by default
+# (B200_FUSE_ROPE_FWD=1 turns it on).
 FUSE_ROPE = os.environ.get("B200_FUSE_ROPE", "1") != "0"
 FUSE_ROPE_FWD = os.environ.get("B200_FUSE_ROPE_FWD", "0") != "0"
 # SwiGLU formed in the epilogue of the gate|up GEMM (ops.linear_swiglu, bit-identical to GEMM + stand-alone kernel): ON.
-# Round 1 measured it slower (+1.5 ms/step: four epilogue warps doing an IEEE division and two SFU ops per element outlasted
-# the K=1024 main loop).  With two epilogue warp groups (8 warps, each group its own staging box and store leader) and
-# silu through ex2.approx / rcp.approx the fused GEMM costs +1.0 ms of GEMM time per step and removes the 1.5 ms/step
-# stand-alone kernel plus its 17.6 GB of traffic: 56.4 -> 54.8 ms/step on one box (profiles/r2_epilogue_ab.txt).
-# B200_FUSE_SWIGLU=0 restores GEMM + kernel.  (The fused RoPE epilogue stays off: neutral within box noise.)
+# It removes the stand-alone kernel and its round trip of the [rows, 2I] activation through HBM.
+# B200_FUSE_SWIGLU=0 restores GEMM + kernel.
 FUSE_SWIGLU = os.environ.get("B200_FUSE_SWIGLU", "1") != "0"
 # Weight-gradient GEMMs on a second stream: dW = dY^T X is off the backward's critical path, so it can run
 # under the HBM-bound kernels that follow on the main stream (SwiGLU / RMSNorm backward leave the tensor pipe idle, and an
@@ -74,7 +69,7 @@ ALIGN = 256   # elements; AdamW's no-decay flags are per 256-element block
 
 def _require_device(n: str, p: torch.Tensor, dev) -> None:
     if p.device != dev or p.dtype != BF16 or not p.is_cuda:
-        raise lib.B200Error(f"parameter {n} is {p.dtype} on {p.device}: the B200 path needs the whole model in "
+        raise lib.B200Error(f"parameter {n} is {p.dtype} on {p.device}: the native path needs the whole model in "
                             "bfloat16 on one CUDA device (model.to('cuda', dtype=torch.bfloat16)); no fallback")
 
 

@@ -46,11 +46,9 @@ SIGNATURES = {
     "b200_gemm_bf16_rope": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp]),
     "b200_gemm_bf16_swiglu": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "b200_attn_causal_fwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp]),
-    "b200_attn_causal_fwd_tc": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp]),
+    "b200_attn_causal_fwd_wgmma": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp]),
+    "b200_attn_causal_bwd_wgmma": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200_attn_causal_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
-    "b200_attn_causal_bwd_tc_workspace_bytes": (sz, [i32, i32, i32]),
-    "b200_attn_causal_bwd_tc": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp, sz, vp]),
-    "b200_attn_debug_trace": (None, [vp]),
     "b200_attn_tiny_fwd": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200_attn_tiny_bwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200_ce_fwd": (i32, [vp, vp, vp, vp, vp, i64, i32, i32, i64, vp]),
@@ -144,4 +142,4 @@ def query(name: str, *args):
 
 def require_cuda(t: torch.Tensor, what: str = "tensor"):
     if not t.is_cuda:
-        raise B200Error(f"{what} must live on a CUDA device: the B200 path has no CPU fallback")
+        raise B200Error(f"{what} must live on a CUDA device: the native path has no CPU fallback")

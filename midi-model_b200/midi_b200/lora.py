@@ -3,7 +3,7 @@
 The reference trains LoRA through `model.add_adapter(LoraConfig(r=64, lora_alpha=128, target_modules=[q,k,v,o,gate,up,
 down]_proj, lora_dropout=0, bias="none"))` (train.py:439-449), saves `adapter_config.json` +
 `adapter_model.safetensors` (train.py:234-244) and merges them for inference (midi_model.py:109-114).  peft is not part
-of this image, and the sm_100a engine never calls a module's `forward` anyway: the HF modules are parameter containers.
+of this image, and the native engine never calls a module's `forward` anyway: the HF modules are parameter containers.
 So what has to match peft is the *container*: every targeted `nn.Linear` becomes a module with
 
     <path>.base_layer.weight                 frozen base weight (same Parameter object as before)
@@ -138,7 +138,7 @@ class LoraLinear(nn.Module):
         self.active_adapters = [adapter_name]
 
     def forward(self, *args, **kwargs):
-        raise B200Error("LoraLinear is a parameter container: MIDIModel computes through the sm_100a engine "
+        raise B200Error("LoraLinear is a parameter container: MIDIModel computes through the native engine "
                         "(forward / forward_token / training_loss), there is no PyTorch path")
 
 
@@ -152,7 +152,7 @@ def inject(model: nn.Module, cfg: LoraAdapterConfig, adapter_name: str = "defaul
     """What peft's inject_adapter_in_model does for LoRA on Linear targets: wrap every matching layer, then leave only
     the adapter weights trainable (mark_only_lora_as_trainable, bias="none").  Returns the wrapped module paths."""
     if cfg.lora_dropout != 0.0:
-        raise B200Error("lora_dropout > 0 is not supported by the sm_100a engine (train.py:447 uses 0)")
+        raise B200Error("lora_dropout > 0 is not supported by the native engine (train.py:447 uses 0)")
     if cfg.bias != "none":
         raise B200Error(f"LoRA bias mode {cfg.bias!r} is not supported (train.py:445 uses 'none')")
     if cfg.fan_in_fan_out:
@@ -246,7 +246,7 @@ def find_sites(model: nn.Module) -> Dict[str, LoraSite]:
             raise B200Error(f"{path}: LoRA on {type(mod.base_layer).__name__} is not supported (bias-free Linear only)")
         drop = mod.lora_dropout[a] if hasattr(mod, "lora_dropout") and a in mod.lora_dropout else None
         if drop is not None and not isinstance(drop, nn.Identity) and getattr(drop, "p", 0.0) > 0.0:
-            raise B200Error(f"{path}: lora_dropout > 0 is not supported by the sm_100a engine")
+            raise B200Error(f"{path}: lora_dropout > 0 is not supported by the native engine")
         use_dora = getattr(mod, "use_dora", {})
         if isinstance(use_dora, dict) and use_dora.get(a, False):
             raise B200Error(f"{path}: DoRA is not supported")

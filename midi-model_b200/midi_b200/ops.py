@@ -32,7 +32,7 @@ def _ws(key, nbytes: int, device, zero: bool = False) -> torch.Tensor:
 def _check(t: torch.Tensor, name: str):
     if not t.is_cuda or t.dtype != BF16 or not t.is_contiguous():
         raise lib.B200Error(f"{name}: expected a contiguous CUDA bfloat16 tensor, got {t.dtype} on {t.device} "
-                            f"(contiguous={t.is_contiguous()}); the B200 path has no fallback")
+                            f"(contiguous={t.is_contiguous()}); the native path has no fallback")
 
 
 # ------------------------------------------------------------------ embeddings
@@ -186,7 +186,7 @@ def _tail_bytes(M: int, N: int, K: int, block_n: int) -> int:
 def gemm(A: torch.Tensor, B: torch.Tensor, M: int, N: int, K: int, *, lda: int, ldb: int, a_mn: bool = False,
          b_mn: bool = False, out: Optional[torch.Tensor] = None, ldc: Optional[int] = None,
          residual: Optional[torch.Tensor] = None, accumulate: bool = False, allow_split: bool = False) -> torch.Tensor:
-    """C[M,N] = A . B^T on tcgen05 tensor cores (see csrc/gemm_tcgen05.cu)."""
+    """C[M,N] = A . B^T on the wgmma tensor cores (see csrc/gemm_wgmma.cu)."""
     if out is None:
         out = torch.empty((M, N), dtype=BF16, device=A.device)
     if ldc is None:
@@ -270,9 +270,9 @@ def _strides_packed(S: int, H: int, D: int, col0: int, ld: int):
 
 import os as _os
 
-# "tc" = tcgen05 / TMEM / TMA kernel (csrc/attn_tc05.cu); "mma" = mma.sync kernel (csrc/attn_flash.cu)
-ATTN_FWD_IMPL = _os.environ.get("B200_ATTN_FWD", "tc")
-ATTN_BWD_IMPL = _os.environ.get("B200_ATTN_BWD", "tc")
+# "wgmma" = Hopper tensor-core kernels (csrc/attn_wgmma.cu, the default); "mma" = mma.sync kernels (csrc/attn_flash.cu)
+ATTN_IMPL = _os.environ.get("B200_ATTN", "wgmma")
+_ATTN_SUFFIX = {"wgmma": "_wgmma", "mma": ""}
 
 
 def attn_causal_fwd(qkv: torch.Tensor, B: int, S: int, n_heads: int, D: int, want_lse: bool, impl: Optional[str] = None):
@@ -283,17 +283,14 @@ def attn_causal_fwd(qkv: torch.Tensor, B: int, S: int, n_heads: int, D: int, wan
     lse = torch.empty((B, n_heads, S), dtype=torch.float32, device=qkv.device) if want_lse else None
     st = torch.tensor([S * ld, ld, D] * 3 + [S * H, H, D], dtype=torch.int64)
     base = qkv.data_ptr()
-    fn = "b200_attn_causal_fwd_tc" if (impl or ATTN_FWD_IMPL) == "tc" else "b200_attn_causal_fwd"
-    lib.call(fn, base, base + 2 * H, base + 4 * H, out.data_ptr(), lib.ptr(lse), st.data_ptr(), B,
-             n_heads, S, S, D, 1.0 / math.sqrt(D), lib.stream())
+    lib.call("b200_attn_causal_fwd" + _ATTN_SUFFIX[impl or ATTN_IMPL], base, base + 2 * H, base + 4 * H, out.data_ptr(),
+             lib.ptr(lse), st.data_ptr(), B, n_heads, S, S, D, 1.0 / math.sqrt(D), lib.stream())
     return out, lse
 
 
 def attn_causal_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, B: int, S: int,
                     n_heads: int, D: int, rope=None, impl: Optional[str] = None) -> torch.Tensor:
     """`rope=(cos, sin)`: also apply the RoPE backward to dq, dk (gradient w.r.t. the pre-rotation projections)."""
-    if (impl or ATTN_BWD_IMPL) == "tc":
-        return _attn_causal_bwd_tc(qkv, out, dout, lse, B, S, n_heads, D, rope)
     H = n_heads * D
     ld = qkv.stride(0)
     dqkv = torch.empty_like(qkv)
@@ -302,25 +299,9 @@ def attn_causal_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, ls
     po = [S * H, H, D]
     st = torch.tensor(pk * 3 + po + po + pk * 3, dtype=torch.int64)
     b, d = qkv.data_ptr(), dqkv.data_ptr()
-    lib.call("b200_attn_causal_bwd", b, b + 2 * H, b + 4 * H, out.data_ptr(), dout.data_ptr(), lse.data_ptr(),
-             delta.data_ptr(), d, d + 2 * H, d + 4 * H, st.data_ptr(), B, n_heads, S, S, D, 1.0 / math.sqrt(D),
-             rope[0].data_ptr() if rope else None, rope[1].data_ptr() if rope else None, lib.stream())
-    return dqkv
-
-
-def _attn_causal_bwd_tc(qkv, out, dout, lse, B, S, n_heads, D, rope):
-    H = n_heads * D
-    ld = qkv.stride(0)
-    dqkv = torch.empty_like(qkv)
-    pk = [S * ld, ld, D]
-    po = [S * H, H, D]
-    st = torch.tensor(pk * 3 + po + po + pk * 3, dtype=torch.int64)
-    nbytes = lib.query("b200_attn_causal_bwd_tc_workspace_bytes", B, n_heads, S)
-    ws = _ws("attn_bwd_tc", nbytes, qkv.device)
-    b, d = qkv.data_ptr(), dqkv.data_ptr()
-    lib.call("b200_attn_causal_bwd_tc", b, b + 2 * H, b + 4 * H, out.data_ptr(), dout.data_ptr(), lse.data_ptr(), d, d + 2 * H,
-             d + 4 * H, st.data_ptr(), B, n_heads, S, S, D, 1.0 / math.sqrt(D), rope[0].data_ptr() if rope else None,
-             rope[1].data_ptr() if rope else None, ws.data_ptr(), ws.numel(), lib.stream())
+    lib.call("b200_attn_causal_bwd" + _ATTN_SUFFIX[impl or ATTN_IMPL], b, b + 2 * H, b + 4 * H, out.data_ptr(),
+             dout.data_ptr(), lse.data_ptr(), delta.data_ptr(), d, d + 2 * H, d + 4 * H, st.data_ptr(), B, n_heads, S, S, D,
+             1.0 / math.sqrt(D), rope[0].data_ptr() if rope else None, rope[1].data_ptr() if rope else None, lib.stream())
     return dqkv
 
 

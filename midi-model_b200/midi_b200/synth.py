@@ -1,4 +1,4 @@
-"""Seeded synthetic, grammar-valid MIDI-event token tensors (SURVEY.md section 8d).
+"""Seeded synthetic, grammar-valid MIDI-event token tensors.
 
 Row 0 of every sequence is `[bos, 0 x 7]`; every later row is one event drawn
 with the type mix note .85 / control_change .06 / patch_change .03 / set_tempo

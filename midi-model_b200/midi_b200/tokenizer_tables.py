@@ -10,7 +10,7 @@ deployment: this repo's `midi_model.py` placed ahead of the reference on
 `sys.path`) the drop-in uses that class unchanged, so `tokenize/detokenize`
 keep working.  When it is not (the GPU box, unit tests, the benchmark) this
 table-only stand-in provides the same attributes.  Score <-> token conversion,
-augmentation and quality filters are out of scope (SURVEY.md section 2, rows 4-5).
+augmentation and quality filters are out of scope.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Drop-in `midi_model` module: B200-native MIDIModel.
+"""Drop-in `midi_model` module: CUDA-native MIDIModel (H100, sm_90a).
 
 Place this directory ahead of the reference checkout on `sys.path`; `train.py` / `app.py` then do
 `from midi_model import MIDIModel, MIDIModelConfig, config_name_list` and get this implementation
@@ -7,7 +7,7 @@ tree and `state_dict` keys (`net.*`, `net_token.*`, `lm_head.weight` -- the HF `
 as parameter containers only, so seeded init, the four dtype-following RoPE `inv_freq` buffers and
 peft/LoRA affordances behave exactly like the reference), and the signatures / semantics of
 `forward`, `forward_token`, `sample_top_p_k`, `generate`.  What is new is everything that computes:
-all arithmetic runs in hand-written sm_100a kernels behind the C ABI in `include/midi_b200.h`
+all arithmetic runs in hand-written sm_90a kernels behind the C ABI in `include/midi_b200.h`
 (`midi_b200/lib.py`).  There is no PyTorch / CPU fallback: parameters must be bfloat16 on a CUDA
 device, otherwise the call raises.
 
@@ -264,7 +264,7 @@ class _LazyCEFn(torch.autograd.Function):
 class LazyLogits(torch.Tensor):
     """What forward_token returns in training: an ordinary dense [N, L, V] logits tensor (every op works on it as before)
     that remembers the pitched buffer behind it, so that the reference's loss expression is served by the fused
-    cross-entropy kernels instead of materialising log-softmax and dlogits copies of the 0.9 GB logits (SURVEY.md 8 f2)."""
+    cross-entropy kernels instead of materialising log-softmax and dlogits copies of the 0.9 GB logits."""
 
     @classmethod
     def __torch_function__(cls, func, types, args=(), kwargs=None):

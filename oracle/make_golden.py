@@ -1,17 +1,22 @@
-"""Generate tests/golden/*.npz from the UNMODIFIED reference -- run in the build
-container only (`/root/reference` present):  python oracle/make_golden.py
+"""Generate tests/golden/*.npz from the UNMODIFIED reference -- run where a checkout of the reference
+is present (MIDI_REFERENCE_DIR, see oracle/ref_loader.py):  python oracle/make_golden.py
 
-The reference ships no tests or golden vectors (SURVEY.md section 4), so these fixtures
+The reference ships no tests or golden vectors, so these fixtures
 are outputs of the reference itself (torch 2.11.0 / transformers 5.5.0, CPU),
 imported read-only through oracle/ref_loader.py.
 
-  tiny.npz    tiny config (4L/4h/32/64 -> inner 1L/1h/32/16), seed-0 weights
-              COMMITTED, inputs, fp32 + bf16 hidden / logits / loss, fp32 grads
+  tiny.npz    tiny config (4L/4h/32/64 -> inner 1L/1h/32/16), seed-0 weights (vocab-sized
+              tensors: first 160 rows + checksums; the tests regenerate them with the product's drop-in class, so
+              the oracle checks that use them are anchored to it by those rows and checksums), inputs,
+              fp32 + bf16 hidden / loss, logits on a fixed sample of 128 vocab columns, fp32 grads
               checksums, greedy generate ids, sample_top_p_k cases.
   medium.npz  tv2o-medium seed-0 init checksums + fp32 hidden/logits slices and
               loss on a (1,17,8) synthetic batch (weights regenerated from seed).
   app_stream.npz  events yielded by the reference's app.py generate() (app.py:27-120, executed from the reference
               file at run time, nothing copied) on the tiny model with the disable_* options, greedy and sampled.
+  ref_live.npz  what the reference itself computes for the cross-checks of tests/test_oracle.py: its tokenizer
+              tables (pickled), one more app.py generate() case, and tv2o-medium hidden states / sampled logits
+              on a (1, 9, 8) batch.
 """
 from __future__ import annotations
 
@@ -54,13 +59,19 @@ def tiny():
     tok = model.tokenizer
     out = {}
     for k, v in model.state_dict().items():
-        out["sd/" + k] = v.detach().numpy().astype(np.float32)
+        v = v.detach()
+        if v.shape[0] > 1000:          # vocab-sized: first 160 rows + checksums of the whole tensor
+            out["sdsum/" + k] = np.array([v.double().sum().item(), v.double().abs().sum().item()])
+            v = v[:160]
+        out["sd/" + k] = v.numpy().astype(np.float32)
+    cols = np.sort(np.random.default_rng(0).choice(tok.vocab_size, 128, replace=False))
+    out["logit_cols"] = cols
     batch = synth_batch(tok, 2, 13, seed=7, pad_tail=2)
     out["batch"] = batch.numpy()
     hidden, logits, loss = ref_train_loss(model, batch)
     loss.backward()
     out["fp32/hidden"] = hidden.detach().numpy()
-    out["fp32/logits"] = logits.detach().numpy()
+    out["fp32/logits"] = logits.detach().numpy()[..., cols]
     out["fp32/loss"] = np.float32(loss.item())
     for k, p in model.named_parameters():
         g = p.grad.detach()
@@ -83,7 +94,7 @@ def tiny():
     with torch.no_grad():
         hb, lb, lossb = ref_train_loss(m16, batch)
     out["bf16/hidden"] = hb.float().numpy()
-    out["bf16/logits"] = lb.float().numpy()
+    out["bf16/logits"] = lb.float().numpy()[..., cols]
     out["bf16/loss"] = np.float32(lossb.float().item())
     # KV-cached incremental forward == full forward (public forward(x, cache) API)
     from transformers import DynamicCache
@@ -187,6 +198,41 @@ def app_stream():
     np.savez_compressed(os.path.join(OUT, "app_stream.npz"), **out)
 
 
+LIVE_APP_KW = dict(batch_size=3, max_len=9, temp=0.9, top_p=0.95, top_k=10, disable_patch_change=True,
+                   disable_control_change=False, disable_channels=[0, 3])
+
+
+def ref_live():
+    import pickle
+    mm, rt = ref_loader.load()
+    out = {}
+    for ver in ("v1", "v2"):
+        t = rt.MIDITokenizer(ver)
+        attrs = {a: getattr(t, a) for a in ("vocab_size", "pad_id", "bos_id", "eos_id", "events", "event_parameters",
+                                              "event_ids", "id_events", "parameter_ids", "max_token_seq")}
+        attrs["to_dict"] = t.to_dict()
+        out["tokenizer/" + ver] = np.frombuffer(pickle.dumps(attrs), dtype=np.uint8)
+    torch.manual_seed(0)
+    cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=4, n_embd=32, n_inner=64)
+    model = mm.MIDIModel(cfg).eval()
+    gen = ref_app_generate(model, model.tokenizer)
+    out["app_live"] = np.stack(list(gen(prompt=None, generator=torch.Generator().manual_seed(21), **LIVE_APP_KW)), axis=1)
+    torch.manual_seed(1)
+    cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=16, n_embd=1024, n_inner=4096)
+    model = mm.MIDIModel(cfg).eval()
+    batch = synth_batch(model.tokenizer, 1, 9, seed=5)
+    with torch.no_grad():
+        h = model.forward(batch[:, :-1])
+        lg = model.forward_token(h.reshape(-1, 1024), batch[:, 1:].reshape(-1, 8)[:, :-1])
+    cols = np.sort(np.random.default_rng(1).choice(lg.shape[-1], 256, replace=False))
+    out["medium/batch"] = batch.numpy()
+    out["medium/hidden"] = h.numpy()
+    out["medium/logit_cols"] = cols
+    out["medium/logits"] = lg.numpy()[..., cols]
+    np.savez_compressed(os.path.join(OUT, "ref_live.npz"), **out)
+    print("ref_live.npz:", sorted(out))
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
@@ -196,3 +242,4 @@ if __name__ == "__main__":
         tiny()
         medium()
         app_stream()
+        ref_live()

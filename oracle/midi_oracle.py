@@ -9,9 +9,8 @@ Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline /
 `--impl reference` legs may import this module, and only as the checker /
 timed CPU baseline.  The product (`midi-model_b200/`) never imports it.
 
-Pinning: the reference has no tests or golden vectors of its own (SURVEY.md
-section 4), so this restatement is pinned against outputs of the reference itself,
-imported read-only in the build container with a 4-name `peft` stub
+Pinning: the reference has no tests or golden vectors of its own, so this restatement is pinned against outputs of the reference itself,
+imported read-only with a 4-name `peft` stub
 (`oracle/ref_loader.py`); the generating script is `oracle/make_golden.py` and
 the vectors live in `tests/golden/`.  `tests/test_oracle.py` re-checks them.
 
@@ -19,7 +18,7 @@ Everything operates on a flat ``state_dict`` with the reference's key names
 (`net.layers.{i}.self_attn.q_proj.weight`, ...) so that the same function can
 be fed weights from the reference, from the drop-in class or from a file.
 Computation happens in the dtype of the weights: with bf16 weights every torch
-op rounds where the reference's eager bf16 path rounds (SURVEY.md Appendix A).
+op rounds where the reference's eager bf16 path rounds (DESIGN.md 3.3).
 """
 from __future__ import annotations
 
@@ -161,7 +160,7 @@ def llama_stack(sd: Dict[str, torch.Tensor], cfg: StackCfg, x: torch.Tensor,
     h, d = cfg.n_head, cfg.head_dim
     if inv_freq is None:
         inv_freq = default_inv_freq(d, cfg.theta)
-        if x.dtype != torch.float32:          # model.to(bf16) rounds the buffer (SURVEY.md 0.6)
+        if x.dtype != torch.float32:          # model.to(bf16) rounds the buffer
             inv_freq = inv_freq.to(x.dtype)
     past = cache.seq_len() if cache is not None else 0
     pos = torch.arange(past, past + S, device=x.device)       # hf :394-397
@@ -247,7 +246,7 @@ def lora_effective_sd(sd: Dict[str, torch.Tensor], scaling: float, adapter: str 
 def sample_top_p_k(probs: torch.Tensor, p: float, k: int, generator=None, stable: bool = True) -> torch.Tensor:
     """midi_model.py:152-165.  `stable=True` breaks exact ties by ascending id
     (the reference's torch.sort is unstable; its tie order is implementation
-    defined -- SURVEY.md 0.6)."""
+    defined)."""
     probs_sort, probs_idx = torch.sort(probs, dim=-1, descending=True, stable=stable)
     probs_sum = torch.cumsum(probs_sort, dim=-1)
     mask = probs_sum - probs_sort > p

@@ -1,13 +1,13 @@
-"""Import the UNMODIFIED reference (`/root/reference`) read-only -- TEST INFRASTRUCTURE.
+"""Import the UNMODIFIED reference (a checkout of SkyTNT/midi-model named by MIDI_REFERENCE_DIR) read-only -- used by
+oracle/make_golden.py to produce the fixtures under tests/golden/.
 
-The reference fails to import in this image only because `midi_model.py:9`
+The reference fails to import without peft only because `midi_model.py:9`
 imports four `peft` names that are used solely inside `load_merge_lora`
 (`midi_model.py:109-114`).  We register a 4-name stub module and import the
 reference's own `midi_model` / `midi_tokenizer` under private module names so
 they never shadow the drop-in `midi_model` of this repo.
 
-`/root/reference` exists only in the build container; on the GPU box
-`available()` is False and callers must skip.
+Without MIDI_REFERENCE_DIR `available()` is False; the tests never need the reference (they read the fixtures).
 """
 from __future__ import annotations
 
@@ -16,11 +16,11 @@ import os
 import sys
 import types
 
-REF_DIR = os.environ.get("MIDI_REFERENCE_DIR", "/root/reference")
+REF_DIR = os.environ.get("MIDI_REFERENCE_DIR", "")
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REF_DIR, "midi_model.py"))
+    return bool(REF_DIR) and os.path.isfile(os.path.join(REF_DIR, "midi_model.py"))
 
 
 def _load(name: str, alias: str):
@@ -39,7 +39,7 @@ def load():
     if "m" in _cache:
         return _cache["m"], _cache["t"]
     if not available():
-        raise RuntimeError(f"reference not present at {REF_DIR}")
+        raise RuntimeError(f"reference not present (MIDI_REFERENCE_DIR={REF_DIR!r})")
     if "peft" not in sys.modules:
         try:
             import peft  # noqa: F401

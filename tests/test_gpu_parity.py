@@ -1,4 +1,4 @@
-"""GPU parity tests (driver: `pytest -m gpu`).  Each group compares the sm_100a kernels / the drop-in
+"""GPU parity tests (`pytest -m gpu`).  Each group compares the sm_90a kernels / the drop-in
 MIDIModel -- called through the C ABI -- with the PyTorch composite / the oracle; see gpu_checks.py."""
 import os
 import sys
@@ -7,7 +7,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-GROUP_NAMES = ["gemm_fwd", "gemm_swiglu", "gemm_dgrad", "gemm_wgrad", "elementwise", "fused_rope", "attn_flash", "attn_tc05", "attn_tiny", "loss_optim", "decode",
+GROUP_NAMES = ["gemm_fwd", "gemm_swiglu", "gemm_dgrad", "gemm_wgrad", "elementwise", "fused_rope", "attn_flash", "attn_wgmma", "attn_tiny", "loss_optim", "decode",
                "model_forward", "model_layer_tf", "model_train", "model_generate", "model_peaked_greedy", "model_large",
                "gemm_exact", "decode_paged", "lora_train", "model_vs_hf", "model_medium_long"]
 
@@ -26,7 +26,7 @@ def test_native_library_is_loaded():
 @pytest.mark.parametrize("group", GROUP_NAMES)
 def test_gpu_group(group):
     import torch
-    assert torch.cuda.is_available(), "needs a B200"
+    assert torch.cuda.is_available(), "needs an H100"
     import gpu_checks as G
     metrics = G.GROUPS[group]()
     torch.cuda.synchronize()

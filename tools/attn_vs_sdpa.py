@@ -1,7 +1,7 @@
-"""A/B of the tcgen05 attention kernels against torch's F.scaled_dot_product_attention (the reference's backend,
+"""A/B of the attention kernels against torch's F.scaled_dot_product_attention (the reference's backend,
 hf integrations/sdpa_attention.py:92-101) at the benchmark shape (8 sequences, 16 heads, 2048 events, head_dim 64,
 causal, bf16), forward and backward, plus the token-level shape (16 384 events x 8 tokens, 4 heads of 256).
-CUDA events, 3 warm-up + 20 launches.  Writes gpurun_out/attn_vs_sdpa.json.
+CUDA events, 3 warm-up + 20 launches.  Writes $MIDI_TOOLS_OUT/attn_vs_sdpa.json.
 
     python tools/attn_vs_sdpa.py
 """
@@ -10,6 +10,7 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+OUT_DIR = os.environ.get("MIDI_TOOLS_OUT", os.path.join(ROOT, "tools_out"))
 sys.path.insert(0, os.path.join(ROOT, "midi-model_b200"))
 sys.path.insert(0, ROOT)
 import torch  # noqa: E402
@@ -72,8 +73,8 @@ def main():
     res["token_bwd"] = {"ours_ms": t, "sdpa_ms": t_ref, "ratio": t_ref / t}
     for k_, v_ in res.items():
         print(k_, json.dumps(v_))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "attn_vs_sdpa.json"), "w") as f:
+    os.makedirs(OUT_DIR, exist_ok=True)
+    with open(os.path.join(OUT_DIR, "attn_vs_sdpa.json"), "w") as f:
         json.dump(res, f, indent=1)
 
 

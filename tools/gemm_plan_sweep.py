@@ -1,13 +1,14 @@
 """Sweep (block_n, splits) for the 24 GEMM shapes of one tv2o-medium train step and compare the fastest configuration with
 the one the library's cost model (b200_gemm_plan) picks.  Same timing method as tools/gemm_vs_cublas.py.
 
-    python tools/gemm_plan_sweep.py            # writes gpurun_out/gemm_plan_sweep.json
+    python tools/gemm_plan_sweep.py            # writes $MIDI_TOOLS_OUT/gemm_plan_sweep.json
 """
 import json
 import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+OUT_DIR = os.environ.get("MIDI_TOOLS_OUT", os.path.join(ROOT, "tools_out"))
 sys.path.insert(0, os.path.join(ROOT, "midi-model_b200"))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -78,8 +79,8 @@ def main():
     tot_a = sum(r["planner_ms"] * r["launches_per_step"] for r in rows)
     tot_b = sum(min(r["best_ms"], r["planner_ms"]) * r["launches_per_step"] for r in rows)
     print(f"per-step GEMM time (isolated, launch-weighted): planner {tot_a:.2f} ms, best-of-sweep {tot_b:.2f} ms")
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "gemm_plan_sweep.json"), "w") as f:
+    os.makedirs(OUT_DIR, exist_ok=True)
+    with open(os.path.join(OUT_DIR, "gemm_plan_sweep.json"), "w") as f:
         json.dump({"rows": rows, "planner_ms_per_step": tot_a, "best_ms_per_step": tot_b}, f, indent=1)
 
 

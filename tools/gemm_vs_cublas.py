@@ -1,7 +1,7 @@
-"""Per-shape A/B of the tcgen05 GEMM against cuBLAS (torch.matmul, bf16) on the 24 GEMM shapes of one tv2o-medium
+"""Per-shape A/B of the wgmma GEMM against cuBLAS (torch.matmul, bf16) on the 24 GEMM shapes of one tv2o-medium
 train step (the per-shape table of bench.py's roofline object), each timed alone: CUDA events, 3 warm-up + 20 launches,
-operands rotated through enough copies to exceed the 126 MB L2.  Prints a table and writes
-gpurun_out/gemm_vs_cublas.json.  `ratio` > 1 means this repo's kernel is faster.
+operands rotated through enough copies to exceed the 50 MB L2.  Prints a table and writes
+$MIDI_TOOLS_OUT/gemm_vs_cublas.json.  `ratio` > 1 means this repo's kernel is faster.
 
     python tools/gemm_vs_cublas.py
 """
@@ -10,6 +10,7 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+OUT_DIR = os.environ.get("MIDI_TOOLS_OUT", os.path.join(ROOT, "tools_out"))
 sys.path.insert(0, os.path.join(ROOT, "midi-model_b200"))
 sys.path.insert(0, ROOT)
 import torch  # noqa: E402
@@ -73,8 +74,8 @@ def main():
     tot_o = sum(r["ours_ms"] * r["launches_per_step"] for r in rows)
     tot_r = sum(r["cublas_ms"] * r["launches_per_step"] for r in rows)
     print(f"per-step GEMM time (launch-weighted, isolated): ours {tot_o:.2f} ms, cuBLAS {tot_r:.2f} ms, ratio {tot_r / tot_o:.3f}")
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "gemm_vs_cublas.json"), "w") as f:
+    os.makedirs(OUT_DIR, exist_ok=True)
+    with open(os.path.join(OUT_DIR, "gemm_vs_cublas.json"), "w") as f:
         json.dump({"rows": rows, "ours_ms_per_step": tot_o, "cublas_ms_per_step": tot_r}, f, indent=1)
 
 

@@ -1,5 +1,5 @@
 """One launch of every HBM-bound kernel of the train step on bench-shape tensors (after one warm-up launch each), for
-`ncu --set full -k regex:...` captures (profiles/r2_hbm_kernels_ncu.txt)."""
+`ncu --set full -k regex:...` captures (kept out of the repository)."""
 import os
 import sys
 

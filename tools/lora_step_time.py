@@ -1,7 +1,7 @@
 """LoRA step time at the benchmark shape (tv2o-medium, B=8 x 2048 events x 8 tokens): train.py --task lora
 (r = 64, lora_alpha = 128, all seven projections, frozen base; train.py:439-449) on the fused trainer
 (training_loss + fused_optimizer_step over the adapter tail), then the full-training step of the same model for comparison.
-Writes gpurun_out/lora_step_time.json after each leg.
+Writes $MIDI_TOOLS_OUT/lora_step_time.json after each leg.
 
     python tools/lora_step_time.py [steps]
 """
@@ -11,6 +11,7 @@ import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+OUT_DIR = os.environ.get("MIDI_TOOLS_OUT", os.path.join(ROOT, "tools_out"))
 for p in (os.path.join(ROOT, "midi-model_b200"), ROOT):
     sys.path.insert(0, p)
 import torch  # noqa: E402
@@ -22,11 +23,11 @@ from midi_b200.synth import synth_batch  # noqa: E402
 K = int(sys.argv[1]) if len(sys.argv) > 1 else 5
 dev = torch.device("cuda", 0)
 out = {"workload": "tv2o-medium train step, B=8, 2048 events x 8 tokens, bf16", "steps": K}
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
+os.makedirs(OUT_DIR, exist_ok=True)
 
 
 def dump():
-    with open(os.path.join(ROOT, "gpurun_out", "lora_step_time.json"), "w") as f:
+    with open(os.path.join(OUT_DIR, "lora_step_time.json"), "w") as f:
         json.dump(out, f, indent=1)
     print(json.dumps(out), flush=True)
 

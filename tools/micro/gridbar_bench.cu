@@ -1,6 +1,6 @@
 // Micro-benchmark of grid-wide barrier variants on one CTA per SM (cooperative launch): cycles per barrier, measured by
 // CTA 0, with and without a burst of weight-like global loads issued by the other warps right before the barrier.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gridbar_bench gridbar_bench.cu && ./gridbar_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gridbar_bench gridbar_bench.cu && ./gridbar_bench
 #include <cstdio>
 #include <cuda_runtime.h>
 

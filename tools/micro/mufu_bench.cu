@@ -2,7 +2,7 @@
 // MUFU.EX2 as a function of warps per sub-partition and of the instruction mix around it (the softmax inner loop issues,
 // per element, 1 FFMA (scale), 1 MUFU.EX2, 1 FADD (row sum) and 1/2 F2FP (bf16 pack)).  Also: packed half-precision
 // exponentials, and a degree-3 polynomial 2^x on the FMA pipe.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mufu_bench mufu_bench.cu && ./mufu_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mufu_bench mufu_bench.cu && ./mufu_bench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -87,19 +87,19 @@ __global__ void bench(float* out, long long* cycles, int iters, float seed) {
 template <int MODE>
 void run(const char* name, int exps_per_iter_per_thread) {
     float* out; long long* cyc;
-    cudaMalloc(&out, 148 * 1024 * sizeof(float));
-    cudaMalloc(&cyc, 148 * sizeof(long long));
+    cudaMalloc(&out, 132 * 1024 * sizeof(float));
+    cudaMalloc(&cyc, 132 * sizeof(long long));
     const int iters = 2000;
     for (int wps = 1; wps <= 4; wps *= 2) {       // warps per sub-partition
         const int threads = 128 * wps;
-        bench<MODE><<<148, threads>>>(out, cyc, 10, 0.25f);
-        bench<MODE><<<148, threads>>>(out, cyc, iters, 0.25f);
+        bench<MODE><<<132, threads>>>(out, cyc, 10, 0.25f);
+        bench<MODE><<<132, threads>>>(out, cyc, iters, 0.25f);
         cudaDeviceSynchronize();
-        long long h[148];
+        long long h[132];
         cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
         double avg = 0;
-        for (int i = 0; i < 148; i++) avg += (double)h[i];
-        avg /= 148;
+        for (int i = 0; i < 132; i++) avg += (double)h[i];
+        avg /= 132;
         // warp-level exponential instructions issued per sub-partition = wps * iters * exps_per_iter
         printf("%-44s warps/SMSP %d : %7.2f cycles per warp-exponential per SMSP  (%s)\n", name, wps,
                avg / ((double)wps * iters * exps_per_iter_per_thread), cudaGetErrorString(cudaGetLastError()));

@@ -1,5 +1,5 @@
 """Run every GPU parity group of tests/gpu_checks.py in its own subprocess (a trapped kernel cannot
-poison the other groups), print a table and write gpurun_out/checks.json.
+poison the other groups), print a table and write $MIDI_TOOLS_OUT/checks.json.
 
     python tools/run_gpu_checks.py [group ...]
 """
@@ -10,7 +10,8 @@ import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OUT = os.path.join(ROOT, "gpurun_out")
+OUT_DIR = os.environ.get("MIDI_TOOLS_OUT", os.path.join(ROOT, "tools_out"))
+OUT = OUT_DIR
 
 
 def child(group):

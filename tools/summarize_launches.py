@@ -2,7 +2,7 @@
 --clock-control none --csv ...`) of `bench.py --steps 1 --warmup 1`: one optimizer step = the launches between the last two
 adamw_kernel launches.  Writes the per-kernel table and the GEMM DRAM traffic json used by bench.py's roofline.traffic.
 
-    python tools/summarize_launches.py gpurun_out/launches.csv profiles/r2
+    python tools/summarize_launches.py $MIDI_TOOLS_OUT/launches.csv $MIDI_TOOLS_OUT/run
 """
 import csv
 import json
@@ -49,11 +49,11 @@ def main():
         if a[1] / tot < 0.001:
             continue
         out.append(f"{n[:60]:60s} {a[0]:8d} {a[1]:10.1f} {a[1] / tot:7.1%} {a[2] / 1e9:9.2f}")
-    gemm = [a for n, a in agg.items() if "gemm_tcgen05_kernel" in n]
+    gemm = [a for n, a in agg.items() if "gemm_wgmma_kernel" in n]
     g_l, g_t, g_b = sum(a[0] for a in gemm), sum(a[1] for a in gemm), sum(a[2] for a in gemm)
     out.append(f"GEMM share of the step: {g_t / 1e3:.2f} ms of {tot / 1e3:.2f} ms = {g_t / tot:.1%}; {g_l} launches, {g_b / 1e9:.1f} GB DRAM")
     open(prefix + "_launches_step_summary.txt", "w").write("\n".join(out) + "\n")
-    json.dump({"kernel": "gemm_tcgen05_kernel", "launches_per_step": g_l, "dram_bytes_per_step": g_b,
+    json.dump({"kernel": "gemm_wgmma_kernel", "launches_per_step": g_l, "dram_bytes_per_step": g_b,
                "dram_bytes_per_launch": g_b / max(g_l, 1),
                "source": f"{src} (ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none "
                          "python bench.py --steps 1 --warmup 1 --no-cpu-baseline --no-generate --no-hbm-kernels; one optimizer step)"},
