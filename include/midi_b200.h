@@ -87,7 +87,11 @@ int b200_scale_bf16(const void* x, void* y, long long n, float scale, cudaStream
  *      238-264, 288 and lm_head (midi_model.py:135), plus their dgrad / wgrad.
  *      C[M,N] = A . B^T, fp32 accumulate, bf16 out.  a_mn_major / b_mn_major = operand stored [K, rows].
  *      R != NULL: C = bf16(bf16(acc) + R) (residual add, hf :325 / :331).
- *      splits > 1 or accumulate: fp32 split-K partials in `workspace`, reduced (and added to C). */
+ *      splits > 1 or accumulate: fp32 split-K partials in `workspace`, reduced (and added to C); such a call needs
+ *      ldc == N, N % 8 == 0, no residual, and b200_gemm_workspace_bytes(M, N, splits) = max(splits, 1) * M * N * 4 bytes.
+ *      splits is clamped to the number of 64-deep k-blocks, then re-counted so that no split is empty.
+ *      Any M, N, K >= 1 is accepted (N need not be a multiple of 8: columns N..roundup8(N) of C are written as zeros,
+ *      so ldc >= roundup8(N)); lda, ldb, ldc, ldr multiples of 8, pointers 16-byte aligned. */
 size_t b200_gemm_workspace_bytes(int M, int N, int splits);
 /* optional fp32 workspace that lets b200_gemm_bf16 cut the tiles of the last partial wave along K (0: not useful) */
 size_t b200_gemm_tail_workspace_bytes(int M, int N, int K, int block_n);
@@ -109,7 +113,8 @@ int b200_gemm_bf16_swiglu(const void* A, const void* Wgu, void* gu, void* act, i
                           int ld_gu, int ld_act, cudaStream_t s);
 
 /* ---- attention (hf integrations/sdpa_attention.py:41-104 via modeling_llama.py:251-289) ----------
- *      outer stack: causal flash attention, head_dim 64; strides are element strides {batch,row,head}. */
+ *      outer stack: causal flash attention, head_dim 64; strides are element strides {batch,row,head}; Sk >= Sq, query
+ *      row q sees keys <= q + Sk - Sq.  The backward pass of these mma.sync kernels needs n_heads % 4 == 0. */
 int b200_attn_causal_fwd(const void* q, const void* k, const void* v, void* o, float* lse /*may be NULL*/,
                          const long long* strides /*4x3: q,k,v,o*/, int batch, int n_heads, int Sq, int Sk, int head_dim,
                          float scale, cudaStream_t s);

@@ -282,18 +282,21 @@ __device__ __forceinline__ void rope_bwd_acc(float acc[8][4], int r, const bf16*
 __global__ void flash_bwd_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, float* __restrict__ delta,
                                        Strides so, Strides sdo, int n_heads, int Sq) {
     const int row = blockIdx.x % Sq, b = blockIdx.x / Sq;
-    for (int i = threadIdx.x; i < n_heads * 8; i += blockDim.x) {
-        const int h = i >> 3, c = i & 7;
-        float a[8], d[8];
-        unpack8(*reinterpret_cast<const uint4*>(o + b * so.b + (long long)row * so.r + h * so.h + c * 8), a);
-        unpack8(*reinterpret_cast<const uint4*>(d_o + b * sdo.b + (long long)row * sdo.r + h * sdo.h + c * 8), d);
+    // whole warps stay in the loop (full-mask shuffles); lanes past the last head contribute nothing
+    for (int i0 = 0; i0 < n_heads * 8; i0 += blockDim.x) {
+        const int i = i0 + threadIdx.x, h = i >> 3, c = i & 7;
         float s = 0.f;
+        if (h < n_heads) {
+            float a[8], d[8];
+            unpack8(*reinterpret_cast<const uint4*>(o + b * so.b + (long long)row * so.r + h * so.h + c * 8), a);
+            unpack8(*reinterpret_cast<const uint4*>(d_o + b * sdo.b + (long long)row * sdo.r + h * sdo.h + c * 8), d);
 #pragma unroll
-        for (int j = 0; j < 8; j++) s += a[j] * d[j];
+            for (int j = 0; j < 8; j++) s += a[j] * d[j];
+        }
         s += __shfl_xor_sync(0xffffffffu, s, 1);
         s += __shfl_xor_sync(0xffffffffu, s, 2);
         s += __shfl_xor_sync(0xffffffffu, s, 4);
-        if (c == 0) delta[((long long)b * n_heads + h) * Sq + row] = s;
+        if (h < n_heads && c == 0) delta[((long long)b * n_heads + h) * Sq + row] = s;
     }
 }
 
@@ -566,7 +569,6 @@ extern "C" int b200_attn_causal_fwd(const void* q, const void* k, const void* v,
 // delta[b,h,q] = rowsum(dO * O)
 int b200_attn_bwd_delta_launch(const void* o, const void* d_o, float* delta, const long long* so, const long long* sdo,
                                int batch, int n_heads, int Sq, cudaStream_t stream) {
-    B200_CHECK_ARG(n_heads % 4 == 0, "attn bwd: n_heads must be a multiple of 4");
     Strides a{so[0], so[1], so[2]}, b{sdo[0], sdo[1], sdo[2]};
     flash_bwd_delta_kernel<<<batch * Sq, 128, 0, stream>>>((const bf16*)o, (const bf16*)d_o, delta, a, b, n_heads, Sq);
     B200_CHECK_LAUNCH("attn_bwd_delta");

@@ -444,8 +444,9 @@ int hopper::make_tmap_3d(CUtensorMap* tm, const void* ptr, uint64_t cols, uint64
 // ---------------------------------------------------------------------------
 // C ABI (declared in include/midi_b200.h)
 // ---------------------------------------------------------------------------
+// fp32 partials of a call that splits K or accumulates (accumulate with splits == 1 still needs one M x N slice)
 extern "C" size_t b200_gemm_workspace_bytes(int M, int N, int splits) {
-    return splits > 1 ? (size_t)splits * M * N * sizeof(float) : 0;
+    return (size_t)(splits > 1 ? splits : 1) * M * N * sizeof(float);
 }
 
 // Tail split.  tiles = full * sms + r: the last wave keeps only r of the sms CTAs busy for a whole tile time.  Cutting

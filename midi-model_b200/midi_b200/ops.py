@@ -194,9 +194,7 @@ def gemm(A: torch.Tensor, B: torch.Tensor, M: int, N: int, K: int, *, lda: int, 
     block_n, splits = _plan(M, N, K, bool(allow_split and residual is None and ldc == N and N % 8 == 0))
     ws_ptr, ws_bytes = None, 0
     if splits > 1 or accumulate:
-        nbytes = lib.query("b200_gemm_workspace_bytes", M, N, max(splits, 1))
-        if nbytes == 0:
-            nbytes = M * N * 4
+        nbytes = lib.query("b200_gemm_workspace_bytes", M, N, splits)
         ws = _ws("gemm", nbytes, A.device)
         ws_ptr, ws_bytes = ws.data_ptr(), ws.numel()
     elif residual is None:

@@ -11,6 +11,8 @@ int main(void) {
     if (b200_decode_desc_bytes() != sizeof(b200_decode_desc)) { printf("decode_desc size mismatch\n"); fails++; }
     /* split-K workspace: splits * M * N fp32 partials */
     if (b200_gemm_workspace_bytes(1024, 1024, 4) != (size_t)4 * 1024 * 1024 * sizeof(float)) { printf("workspace bytes\n"); fails++; }
+    /* accumulate without split-K still reduces through one fp32 slice: the query covers it */
+    if (b200_gemm_workspace_bytes(300, 520, 1) != (size_t)300 * 520 * sizeof(float)) { printf("workspace bytes, splits 1\n"); fails++; }
     /* argument validation happens before any CUDA call: an empty problem is B200_ERR_ARG with a message */
     int rc = b200_gemm_bf16(NULL, NULL, NULL, NULL, 0, 0, 0, 8, 8, 8, 0, 0, 0, 0, 128, 1, NULL, 0, NULL);
     if (rc != B200_ERR_ARG) { printf("empty gemm: rc %d\n", rc); fails++; }

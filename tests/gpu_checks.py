@@ -1418,6 +1418,341 @@ def check_lora_train():
     return out
 
 
+# ------------------------------------------------------------------------------------------ conformance groups
+# The wgmma GEMM and attention called straight through the C ABI with explicit plans, layouts and strides, scored per
+# element / per row against fp64 (tests/parity_metrics.py).  Outputs live inside NaN-filled buffers (extra rows, a wider
+# pitch) and every input's padding is NaN, so a store outside its range, a tile left unwritten or a read past an extent
+# shows up.  Metrics are aggregated per family (worst case); the worst case of each family is printed.
+def _rup8(n):
+    return (n + 7) // 8 * 8
+
+
+class _Worst:
+    """Worst value per metric over many cases, and which case it came from (NaN counts as worst)."""
+
+    def __init__(self, prefix):
+        self.prefix, self.m, self.where = prefix, {}, {}
+
+    def add(self, family, case, d):
+        for k, v in d.items():
+            key = f"{self.prefix}{family}_{k}" if family else f"{self.prefix}{k}"
+            old = self.m.get(key)
+            if old is None or math.isnan(v) or (not math.isnan(old) and v > old):
+                self.m[key], self.where[key] = float(v), case
+
+    def report(self):
+        for k in sorted(self.m):
+            print(f"  {k} = {self.m[k]:.4g}  worst at {self.where[k]}")
+        return dict(self.m)
+
+
+def _gm_operand(vals, mn_major, extra):
+    """vals [rows, K] as the kernel reads it: K-major = stored [rows, K] with NaN columns K..ld and NaN rows past rows;
+    MN-major = stored [K, rows] with NaN rows past K and NaN columns past rows."""
+    import parity_metrics as P
+    t = vals.T if mn_major else vals
+    return P.poisoned(t.contiguous(), t.shape[0] + extra, _rup8(t.shape[1]) + 8)
+
+
+def _gm_call(A, B, C, R, M, N, K, ldc, ldr, a_mn, b_mn, acc, bn, splits, ws):
+    lib.call("b200_gemm_bf16", A.data_ptr(), B.data_ptr(), C.data_ptr(), lib.ptr(R), M, N, K, A.stride(0), B.stride(0),
+             ldc, ldr, int(a_mn), int(b_mn), int(acc), bn, splits, lib.ptr(ws), 0 if ws is None else ws.numel(), lib.stream())
+
+
+def check_gemm_matrix():
+    """b200_gemm_bf16 with an explicit (block_n, splits) for every instantiation (block_n x operand layouts), each
+    epilogue, split-K with uneven slices, accumulate, the tail split and small / ragged edges, against an fp64 product of
+    the same bf16 operands rounded at the epilogue's rounding points.  No edge is rejected by argument validation or
+    tensor-map encoding (gm_edge_rejected counts them)."""
+    import parity_metrics as P
+    W = _Worst("gm_")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    layouts = [(0, 0), (0, 1), (1, 0), (1, 1)]
+    ran, rejected, min_waves = set(), 0, float("inf")
+
+    def operands(M, N, K, a_mn, b_mn, seed):
+        a, b = randn(M, K, seed=seed), randn(N, K, scale=0.05, seed=seed + 1)
+        return a, b, _gm_operand(a, a_mn, 5), _gm_operand(b, b_mn, 5), a.double() @ b.double().T
+
+    def store(fam, M, N, K, bn, a_mn, b_mn, seed, ldc=None, ws=None):
+        case = f"{M}x{N}x{K} bn{bn} a{a_mn}b{b_mn}"
+        a, b, A, B, ref = operands(M, N, K, a_mn, b_mn, seed)
+        N8 = _rup8(N)
+        ldc = ldc or N8 + 16
+        C = P.nan_buffer((M + 3, ldc), device=DEV)
+        _gm_call(A, B, C, None, M, N, K, ldc, 0, a_mn, b_mn, 0, bn, 1, ws)
+        W.add(fam, case, P.exact_metrics(C[:M, :N], ref))
+        W.add("", case, P.sentinel_report(C, (slice(0, M), slice(0, N)), (slice(0, M), slice(N, N8))))
+        ran.add((bn, a_mn, b_mn))
+        return ref
+
+    def residuals(M, N, K, bn, a_mn, b_mn, seed):
+        a, b, A, B, ref = operands(M, N, K, a_mn, b_mn, seed)
+        r = randn(M, N, seed=seed + 2)
+        acc = P.round_bf16(ref)
+        want = (acc + r.double()).to(torch.float32).to(BF)
+        # residual in its own buffer, ldr != ldc
+        ldc = N + 16
+        R = P.poisoned(r, M + 2, N + 24)
+        C = P.nan_buffer((M + 3, ldc), device=DEV)
+        _gm_call(A, B, C, R, M, N, K, ldc, R.stride(0), a_mn, b_mn, 0, bn, 1, None)
+        case = f"{M}x{N}x{K} bn{bn} a{a_mn}b{b_mn}"
+        W.add("residual", case, P.exact_metrics(C[:M, :N], acc + r.double(), want, inter=ref))
+        W.add("", case, P.sentinel_report(C, (slice(0, M), slice(0, N))))
+        # residual aliasing the output in place, in a column view of a wider buffer (engine._fold, _lora_fwd)
+        wide = P.nan_buffer((M + 3, N + 40), device=DEV)
+        wide[:M, 16:16 + N] = r
+        view = wide[:, 16:]
+        _gm_call(A, B, view, view, M, N, K, wide.stride(0), wide.stride(0), a_mn, b_mn, 0, bn, 1, None)
+        W.add("inplace", case, P.exact_metrics(wide[:M, 16:16 + N], acc + r.double(), want, inter=ref))
+        W.add("", case, P.sentinel_report(wide, (slice(0, M), slice(16, 16 + N))))
+
+    # every instantiation: one ragged shape and one multi-wave shape (more work items than SMs, ragged last wave and
+    # ragged last M / N tiles, so some persistent CTA's second item is ragged), each with every bf16 epilogue
+    for bn in (128, 256):
+        for li, (a_mn, b_mn) in enumerate(layouts):
+            for si, (M, N, K) in enumerate(((129, 136, 72), (2200, 2000, 200))):
+                seed = 1000 + 100 * si + 10 * li + bn // 128
+                if si == 1:
+                    min_waves = min(min_waves, (M + 127) // 128 * ((N + bn - 1) // bn) / sms)
+                store("store", M, N, K, bn, a_mn, b_mn, seed)
+                residuals(M, N, K, bn, a_mn, b_mn, seed)
+
+    # split-K: K = 1050 is 17 k-blocks, so 2 / 3 splits are uneven, 7 re-counts to 6 non-empty splits and 40 clamps to
+    # 17; the workspace is sized by b200_gemm_workspace_bytes alone
+    M, N, K = 300, 520, 1050
+    for bn in (128, 256):
+        for i, splits in enumerate((2, 3, 7, 40)):
+            a_mn, b_mn = layouts[(i + bn // 128) % 4]
+            a, b, A, B, ref = operands(M, N, K, a_mn, b_mn, 2000 + 10 * i + bn)
+            ws = torch.empty(lib.query("b200_gemm_workspace_bytes", M, N, splits), dtype=torch.uint8, device=DEV)
+            C = P.nan_buffer((M + 3, N), device=DEV)
+            _gm_call(A, B, C, None, M, N, K, N, 0, a_mn, b_mn, 0, bn, splits, ws)
+            case = f"splits{splits} bn{bn} a{a_mn}b{b_mn}"
+            W.add("split", case, P.exact_metrics(C[:M], ref))
+            W.add("", case, P.sentinel_report(C, (slice(0, M), slice(0, N))))
+            ran.add((bn, a_mn, b_mn))
+    # accumulate onto a non-zero C at splits 1 and 3: bf16(bf16(acc) + old)
+    for splits in (1, 3):
+        for bn, (a_mn, b_mn) in ((128, (1, 1)), (256, (0, 1))):
+            a, b, A, B, ref = operands(M, N, K, a_mn, b_mn, 2100 + splits + bn)
+            old = randn(M, N, seed=2200 + splits)
+            ws = torch.empty(lib.query("b200_gemm_workspace_bytes", M, N, splits), dtype=torch.uint8, device=DEV)
+            C = P.nan_buffer((M + 3, N), device=DEV)
+            C[:M] = old
+            _gm_call(A, B, C, None, M, N, K, N, 0, a_mn, b_mn, 1, bn, splits, ws)
+            acc = P.round_bf16(ref)
+            case = f"accumulate splits{splits} bn{bn} a{a_mn}b{b_mn}"
+            W.add("accum", case, P.exact_metrics(C[:M], acc + old.double(), (acc + old.double()).to(torch.float32).to(BF),
+                                                 inter=ref))
+            W.add("", case, P.sentinel_report(C, (slice(0, M), slice(0, N))))
+
+    # tail split of the last partial wave: shapes whose tail workspace the library itself asks for on this device are
+    # run with it and without it; ragged M, ragged N (2002: not a multiple of 8 either), both block_n
+    engaged = 0
+    for i, (M, N, K, bn, a_mn, b_mn) in enumerate(((1100, 2000, 6184, 128, 0, 0), (2200, 2002, 6184, 256, 0, 1),
+                                                   (1100, 2002, 6184, 128, 0, 1), (2200, 2000, 6184, 256, 0, 0))):
+        tb = int(lib.query("b200_gemm_tail_workspace_bytes", M, N, K, bn))
+        if tb > 0:
+            engaged += 1
+            store("tail", M, N, K, bn, a_mn, b_mn, 2300 + i, ws=torch.empty(tb, dtype=torch.uint8, device=DEV))
+        store("notail", M, N, K, bn, a_mn, b_mn, 2300 + i)
+
+    # small edges: M = 1 / 63 leave the second consumer warpgroup out of range; N = 8, N = 3406 at pitch 3408; K = 8 /
+    # 16 / 200 (below one k-block and ragged); every operand has lda > K
+    for M, N, K in ((1, 136, 200), (63, 136, 200), (129, 8, 200), (129, 3406, 200), (129, 136, 8), (129, 136, 16),
+                    (1, 8, 8), (63, 3406, 16)):
+        for bn in (128, 256):
+            for li, (a_mn, b_mn) in enumerate(layouts):
+                try:
+                    store("edge", M, N, K, bn, a_mn, b_mn, 2400 + li, ldc=3408 if N == 3406 else None)
+                except lib.B200Error as e:
+                    rejected += 1
+                    print(f"  rejected {M}x{N}x{K} bn{bn} a{a_mn}b{b_mn}: {e}")
+    out = W.report()
+    out["gm_instantiations_run"] = float(len(ran))
+    out["gm_tail_cases_engaged"] = float(engaged)
+    out["gm_edge_rejected"] = float(rejected)
+    out["gm_multiwave_waves"] = min_waves
+    return out
+
+
+def check_gemm_epilogues():
+    """Fused RoPE (head_dim 64 / 128 / 256, rope_cols < N, S = 37 so sequences straddle 128-row tiles) and fused SwiGLU
+    (K = 200, M in {1, 129}, I in {128, 384}) epilogues: bit-identical to the plain GEMM + the stand-alone kernel, and
+    within one ulp of an fp64 chain with the same rounding points.  Sentinel outputs, poisoned inputs."""
+    import parity_metrics as P
+    W = _Worst("ge_")
+    # RoPE: qkv = [q | k | v], H = 256 columns each; columns [0, 512) rotated per head, v stored as is
+    S, K, H = 37, 200, 256
+    for M in (259, 129):
+        for D in (64, 128, 256):
+            N, rope_cols = 3 * H, 2 * H
+            x, w = randn(M, K, seed=M + D), randn(N, K, scale=0.05, seed=M + D + 1)
+            A, B = P.poisoned(x, M + 5, K + 16), P.poisoned(w, N + 5, K + 24)
+            inv = O.default_inv_freq(D).to(BF).to(DEV)
+            cos, sin = ops.rope_table(inv, S)
+            ldc = N + 16
+            C = P.nan_buffer((M + 3, ldc), device=DEV)
+            lib.call("b200_gemm_bf16_rope", A.data_ptr(), B.data_ptr(), C.data_ptr(), M, N, K, A.stride(0), B.stride(0), ldc,
+                     cos.data_ptr(), sin.data_ptr(), S, D, rope_cols, lib.stream())
+            plain = torch.empty(M, N, device=DEV, dtype=BF)
+            _gm_call(A, B, plain, None, M, N, K, N, 0, 0, 0, 0, 256, 1, None)
+            ops.rope_qk_(plain, cos, sin, S, H, D)
+            case = f"M{M} D{D}"
+            W.add("", case, {f"rope_vs_unfused_mismatch_D{D}": float((C[:M, :N] != plain).sum())})
+            # fp64 chain: x = bf16(acc); o1 = bf16(bf16(x1 c) + bf16(-x2 s)), o2 = bf16(bf16(x2 c) + bf16(x1 s))
+            acc = x.double() @ w.double().T
+            xr = P.round_bf16(acc)
+            pos = torch.arange(M, device=DEV) % S
+            c, s = cos.double()[pos][:, None], sin.double()[pos][:, None]
+            q = xr[:, :rope_cols].view(M, -1, 2, D // 2)
+            x1, x2 = q[:, :, 0], q[:, :, 1]
+            o1 = P.round_bf16(x1 * c) + P.round_bf16(-x2 * s)
+            o2 = P.round_bf16(x2 * c) + P.round_bf16(x1 * s)
+            chain = torch.cat([torch.stack([o1, o2], 2).reshape(M, rope_cols), xr[:, rope_cols:]], 1)
+            mag = torch.maximum(x1.abs(), x2.abs())
+            inter = torch.cat([torch.stack([mag, mag], 2).reshape(M, rope_cols), torch.zeros_like(xr[:, rope_cols:])], 1)
+            W.add("rope", case, P.exact_metrics(C[:M, :N], chain, chain.to(torch.float32).to(BF), inter=inter))
+            W.add("", case, P.sentinel_report(C, (slice(0, M), slice(0, N))))
+    # SwiGLU: gu = [g | u] = x Wgu^T stored, act = bf16(bf16(silu(g)) u)
+    K = 200
+    for M in (1, 129):
+        for I in (128, 384):
+            x, w = randn(M, K, seed=M + I), randn(2 * I, K, scale=0.05, seed=M + I + 1)
+            A, B = P.poisoned(x, M + 5, K + 16), P.poisoned(w, 2 * I + 5, K + 24)
+            gu = P.nan_buffer((M + 3, 2 * I + 16), device=DEV)
+            act = P.nan_buffer((M + 3, I + 8), device=DEV)
+            lib.call("b200_gemm_bf16_swiglu", A.data_ptr(), B.data_ptr(), gu.data_ptr(), act.data_ptr(), M, I, K, A.stride(0),
+                     B.stride(0), gu.stride(0), act.stride(0), lib.stream())
+            plain = torch.empty(M, 2 * I, device=DEV, dtype=BF)
+            _gm_call(A, B, plain, None, M, 2 * I, K, 2 * I, 0, 0, 0, 0, 256, 1, None)
+            act_ref = ops.swiglu(plain)
+            case = f"M{M} I{I}"
+            W.add("", case, {"swiglu_gu_vs_unfused_mismatch": float((gu[:M, :2 * I] != plain).sum()),
+                             "swiglu_act_vs_unfused_mismatch": float((act[:M, :I] != act_ref).sum())})
+            acc = x.double() @ w.double().T
+            g, u = P.round_bf16(acc[:, :I]), P.round_bf16(acc[:, I:])
+            chain = P.round_bf16(g * torch.sigmoid(g)) * u
+            W.add("swiglu_gu", case, P.exact_metrics(gu[:M, :2 * I], acc))
+            W.add("swiglu_act", case, P.exact_metrics(act[:M, :I], chain))
+            W.add("", case, P.sentinel_report(gu, (slice(0, M), slice(0, 2 * I))))
+            W.add("", case, P.sentinel_report(act, (slice(0, M), slice(0, I))))
+    return W.report()
+
+
+def _attn_ref64(q, k, v, do, off, scale=0.125, o_in=None):
+    """fp64 causal attention (query q sees keys <= q + off) and its gradients; tensors (B, h, S, D).
+
+    The backward is written out (dS = P (dP - delta), delta = rowsum(dO o)) because the kernels take o as an input: with
+    o_in (the bf16 o handed to the backward) delta is formed from it, so the reference is the exact gradient of the
+    inputs the kernel gets.  Without o_in (o exact) this is fp64 autograd.  It matters where softmax saturates: there
+    dS cancels almost completely and the rounding of o alone moves dq, dk far more than any kernel error."""
+    q, k, v, do = (t.detach().double() for t in (q, k, v, do))
+    s = (q @ k.transpose(-1, -2)) * scale
+    Sq, Sk = q.shape[-2], k.shape[-2]
+    m = torch.arange(Sk, device=q.device)[None] > (torch.arange(Sq, device=q.device)[:, None] + off)
+    s = s.masked_fill(m, float("-inf"))
+    lse = torch.logsumexp(s, -1)
+    p = torch.softmax(s, -1)
+    o = p @ v
+    delta = (do * (o if o_in is None else o_in.double())).sum(-1, keepdim=True)
+    ds = p * (do @ v.transpose(-1, -2) - delta)
+    return o, lse, ds @ k * scale, ds.transpose(-1, -2) @ q * scale, p.transpose(-1, -2) @ do
+
+
+def _rope_bwd64(g, cos, sin, pos):
+    """gradient w.r.t. the pre-rotation projection: the transpose of x' = x c + rotate_half(x) s, in fp64 at `pos`."""
+    c, s = cos.double()[pos], sin.double()[pos]
+    g1, g2 = g[..., :32], g[..., 32:]
+    return torch.cat([g1 * c + g2 * s, g2 * c - g1 * s], -1)
+
+
+def check_attn_edges():
+    """Both attention implementations through the C ABI with explicit strides: separate q / k / v / dO buffers with a
+    batch pitch of S + 3 rows and a row pitch of H + 16 (all padding NaN), outputs inside NaN buffers; S from 1 to 320,
+    Sq < Sk, one head, saturated softmax.  Scored per (batch, head, row) against fp64 attention and its fp64 gradient
+    given the o each backward receives, and wgmma against mma on the same inputs.  The mma backward needs n_heads % 4 == 0, so one-head cases run its forward
+    only."""
+    import parity_metrics as P
+    W = _Worst("ae_")
+    D, scale, floor = 64, 0.125, 1e-3
+    cases = [(3, S, S, nh, 1.0) for S in (1, 2, 17, 63, 64, 65, 127, 129, 320) for nh in (1, 4)]
+    cases += [(3, Sq, Sk, 4, 1.0) for Sq, Sk in ((1, 300), (5, 70), (64, 129), (65, 200))]
+    cases += [(2, 129, 129, 4, 8.0)]
+    inv = O.default_inv_freq(D).to(BF).to(DEV)
+    for ci, (B, Sq, Sk, nh, amp) in enumerate(cases):
+        H = nh * D
+        ld = H + 16
+        off = Sk - Sq
+        case = f"B{B} Sq{Sq} Sk{Sk} h{nh}" + (f" x{amp:g}" if amp != 1.0 else "")
+
+        def buf(S, seed, a=1.0):
+            vals = randn(B, S, H, scale=a, seed=seed)
+            t = P.nan_buffer((B, S + 3, ld), device=DEV)
+            t[:, :S, :H] = vals
+            return vals.view(B, S, nh, D).transpose(1, 2), t
+
+        def st(S):
+            return [(S + 3) * ld, ld, D]
+
+        q, qb = buf(Sq, 3000 + 4 * ci, amp)
+        k, kb = buf(Sk, 3001 + 4 * ci, amp)
+        v, vb = buf(Sk, 3002 + 4 * ci)
+        do, dob = buf(Sq, 3003 + 4 * ci)
+        o64, lse64, _, _, _ = _attn_ref64(q, k, v, do, off, scale)
+        atol = 1e-3 * float(do.double().norm(dim=-1).median())   # row-norm floor on the scale of the inputs
+        cos, sin = ops.rope_table(inv, Sk)
+        rows = {}
+        for impl, sfx in (("wg", "_wgmma"), ("mma", "")):
+            ob = P.nan_buffer((B, Sq + 3, ld), device=DEV)
+            n_lse = B * nh * Sq
+            lse = torch.full((n_lse + 64,), float("nan"), device=DEV)
+            stt = torch.tensor(st(Sq) + st(Sk) + st(Sk) + st(Sq), dtype=torch.int64)
+            lib.call("b200_attn_causal_fwd" + sfx, qb.data_ptr(), kb.data_ptr(), vb.data_ptr(), ob.data_ptr(), lse.data_ptr(),
+                     stt.data_ptr(), B, nh, Sq, Sk, D, scale, lib.stream())
+            o = ob[:, :Sq, :H].view(B, Sq, nh, D).transpose(1, 2)
+            rows[(impl, "o")] = P.row_worst(o, o64, atol=atol)
+            W.add(impl, case, {"lse_abs": float((lse[:n_lse].view(B, nh, Sq).double() - lse64).abs().max())})
+            W.add("", case, P.sentinel_report(ob, (slice(None), slice(0, Sq), slice(0, H))))
+            W.add("", case, P.sentinel_report(lse, (slice(0, n_lse),)))
+            if impl == "mma" and nh % 4:
+                continue
+            # backward (plain and with the RoPE backward fused into dq / dk), from this implementation's o and lse; the
+            # fp64 reference is the gradient given that o
+            _, _, dq64, dk64, dv64 = _attn_ref64(q, k, v, do, off, scale, o_in=o)
+            dq64r = _rope_bwd64(dq64, cos, sin, torch.arange(Sq, device=DEV) + off)
+            dk64r = _rope_bwd64(dk64, cos, sin, torch.arange(Sk, device=DEV))
+            for rope in (False, True):
+                dq = P.nan_buffer((B, Sq + 3, ld), device=DEV)
+                dk = P.nan_buffer((B, Sk + 3, ld), device=DEV)
+                dv = P.nan_buffer((B, Sk + 3, ld), device=DEV)
+                delta = torch.empty(n_lse, device=DEV)
+                stb = torch.tensor(st(Sq) + st(Sk) + st(Sk) + st(Sq) + st(Sq) + st(Sq) + st(Sk) + st(Sk), dtype=torch.int64)
+                lib.call("b200_attn_causal_bwd" + sfx, qb.data_ptr(), kb.data_ptr(), vb.data_ptr(), ob.data_ptr(),
+                         dob.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                         stb.data_ptr(), B, nh, Sq, Sk, D, scale, cos.data_ptr() if rope else None,
+                         sin.data_ptr() if rope else None, lib.stream())
+                g = {n: t[:, :S, :H].view(B, S, nh, D).transpose(1, 2) for n, t, S in (("dq", dq, Sq), ("dk", dk, Sk),
+                                                                                    ("dv", dv, Sk))}
+                if rope:
+                    W.add(impl, case, {"rope_dq_row": P.row_worst(g["dq"], dq64r, atol=atol),
+                                       "rope_dk_row": P.row_worst(g["dk"], dk64r, atol=atol),
+                                       "rope_dv_mismatch": float((g["dv"] != dv_plain).sum())})
+                else:
+                    for n, ref in (("dq", dq64), ("dk", dk64), ("dv", dv64)):
+                        rows[(impl, n)] = P.row_worst(g[n], ref, atol=atol)
+                    dv_plain = g["dv"].clone()
+                for t, S in ((dq, Sq), (dk, Sk), (dv, Sk)):
+                    W.add("", case, P.sentinel_report(t, (slice(None), slice(0, S), slice(0, H))))
+        for (impl, n), val in rows.items():
+            W.add(impl, case, {f"{n}_row": val})
+            if impl == "wg" and ("mma", n) in rows:
+                # same semantics, so the wgmma worst row should stay near the mma worst row on the same inputs
+                W.add("wg_over_mma", case, {n: val / (1.5 * rows[("mma", n)] + floor)})
+    return W.report()
+
+
 GROUPS = {
     "gemm_fwd": check_gemm_fwd, "gemm_swiglu": check_gemm_swiglu, "gemm_dgrad": check_gemm_dgrad, "gemm_wgrad": check_gemm_wgrad,
     "elementwise": check_elementwise, "fused_rope": check_fused_rope, "attn_flash": check_attn_flash, "attn_wgmma": check_attn_wgmma, "attn_tiny": check_attn_tiny,
@@ -1426,10 +1761,36 @@ GROUPS = {
     "model_generate": check_model_generate, "model_peaked_greedy": check_model_peaked_greedy, "model_large": check_model_large,
     "gemm_exact": check_gemm_exact, "decode_paged": check_decode_paged, "model_vs_hf": check_model_vs_hf,
     "model_medium_long": check_model_medium_long, "lora_train": check_lora_train,
+    "gemm_matrix": check_gemm_matrix, "gemm_epilogues": check_gemm_epilogues, "attn_edges": check_attn_edges,
 }
+# groups whose every metric must have a bound in THRESH (an unmatched name would otherwise pass silently)
+STRICT_GROUPS = ("gemm_matrix", "gemm_epilogues", "attn_edges")
 
 # metric-name prefix -> upper bound (first matching prefix wins); "min:" entries are lower bounds
 THRESH = [
+    # conformance groups (gm_ gemm_matrix, ge_ gemm_epilogues, ae_ attn_edges): per-element exactness against the
+    # correctly rounded fp64 result (maxulp / err_over_tol as in gemm_exact), per-row worst relative error of attention,
+    # NaN sentinels around every output and in every input's padding
+    ("gm_sentinels_changed", 0.0), ("gm_nan_in_range", 0.0), ("gm_padcols_nonzero", 0.0), ("gm_edge_rejected", 0.0),
+    ("min:gm_instantiations_run", 8.0), ("min:gm_tail_cases_engaged", 2.0), ("min:gm_multiwave_waves", 1.01),
+    # fraction not correctly rounded, H100 80GB HBM3 at 700 W: 1.1e-4 K <= 200, 4.0e-4 split-K, 3.5e-3 at K = 6184
+    # (tail split or not); bounds about 5x.  One rounding point: <= 1 ulp.  Two (residual, accumulate, RoPE, SwiGLU
+    # act): <= 2 ulp, measured 2 (see parity_metrics.exact_metrics).  err_over_tol measured <= 0.88.
+    ("gm_store_frac", 1e-3), ("gm_residual_frac", 1e-3), ("gm_inplace_frac", 1e-3), ("gm_split_frac", 2e-3),
+    ("gm_accum_frac", 1e-3), ("gm_tail_frac", 1.5e-2), ("gm_notail_frac", 1.5e-2), ("gm_edge_frac", 1e-3),
+    *[(f"gm_{f}_maxulp", 1.0) for f in ("store", "split", "tail", "notail", "edge")],
+    *[(f"gm_{f}_maxulp", 2.0) for f in ("residual", "inplace", "accum")],
+    *[(f"gm_{f}_err_over_tol", 1.0) for f in ("store", "residual", "inplace", "split", "accum", "tail", "notail", "edge")],
+    ("ge_sentinels_changed", 0.0), ("ge_nan_in_range", 0.0), ("ge_rope_vs_unfused_mismatch", 0.0),
+    ("ge_swiglu_gu_vs_unfused_mismatch", 0.0), ("ge_swiglu_act_vs_unfused_mismatch", 0.0),
+    ("ge_rope_frac", 1e-3), ("ge_swiglu_gu_frac", 1e-3), ("ge_swiglu_act_frac", 1e-3),
+    ("ge_swiglu_gu_maxulp", 1.0), ("ge_rope_maxulp", 2.0), ("ge_swiglu_act_maxulp", 2.0),
+    *[(f"ge_{f}_err_over_tol", 1.0) for f in ("rope", "swiglu_gu", "swiglu_act")],
+    # attention, same card: worst row 3.4e-3 (o), 4.4e-3 / 4.6e-3 / 4.5e-3 (dq / dk / dv, with or without the fused
+    # RoPE backward), equal for both implementations; wgmma / (1.5 mma + 1e-3) <= 0.58; LSE 4.8e-5 (saturated softmax)
+    ("ae_sentinels_changed", 0.0), ("ae_nan_in_range", 0.0), ("ae_wg_rope_dv_mismatch", 0.0),
+    ("ae_mma_rope_dv_mismatch", 0.0), ("ae_wg_over_mma_", 1.0), ("ae_wg_lse_abs", 1e-4), ("ae_mma_lse_abs", 1e-4),
+    *[(f"ae_{i}_{n}_row", 1e-2) for i in ("wg", "mma") for n in ("o", "dq", "dk", "dv", "rope_dq", "rope_dk")],
     # LoRA (train.py:439-449): rank-64 GEMM shapes, adapter gradients vs the oracle's autograd, frozen base untouched
     ("lora_scale_mismatch", 0.0), ("lora_gemm_up_untouched", 0.0), ("lora_gemm_", 4e-3), ("lora_loss_abs", 3e-2),
     ("lora_grad_global_rel", 6e-2), ("lora_base_grads_present", 0.0), ("lora_frozen_changed", 0.0), ("min:lora_adapters_changed", 70.0),

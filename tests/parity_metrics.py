@@ -1,0 +1,115 @@
+"""Metrics that compare a bf16 kernel result with a high-precision reference element by element or row by row, and the
+NaN sentinel / poisoned-input buffers the conformance groups of gpu_checks.py build their operands in.
+
+Global norms hide localized errors: a wrong 8-column group in one row of a 1000 x 1024 GEMM, or a zeroed last row of
+one attention head, moves a relative Frobenius norm by less than its usual bound.  These helpers score the worst
+element or the worst row instead.  Pure PyTorch on any device, so tests/test_parity_metrics.py can show on the CPU that
+each metric fails on the corruptions it is meant to catch."""
+from __future__ import annotations
+
+import torch
+
+BF = torch.bfloat16
+NAN = float("nan")
+
+
+# ------------------------------------------------------------------------------------------ per-element exactness
+def ordered_bf16(t: torch.Tensor) -> torch.Tensor:
+    """bf16 bit patterns mapped to integers that are monotonic in the value (for ulp distances)."""
+    i = t.contiguous().view(torch.int16).int()
+    return torch.where(i >= 0, i, -(i & 0x7FFF))
+
+
+def round_bf16(x: torch.Tensor) -> torch.Tensor:
+    """x (fp64) rounded to bf16 and returned as fp64: one rounding point of a kernel's epilogue, restated."""
+    return x.to(torch.float32).to(BF).double()
+
+
+def exact_metrics(y: torch.Tensor, ref64: torch.Tensor, want: torch.Tensor | None = None,
+                  inter: torch.Tensor | None = None) -> dict:
+    """y (bf16) against an fp64 reference of the same bf16 operands.
+
+    want : the correctly rounded result the kernel should return (default bf16(ref64)); epilogues with several
+           rounding points pass the fp64 chain rounded at the same points.
+    inter: magnitude of the value rounded at an earlier rounding point (the bf16 accumulator before a residual add or
+           a rotation).  fp32 summation order may flip that rounding by one ulp, which moves a result that cancels
+           by many of its own ulps; such elements are left out of the ulp count and get that ulp in their tolerance.
+           Where they do not cancel, a flip can still cost two ulps of the result: an fp32 accumulator exactly on a
+           bf16 midpoint rounds to even, one ulp away from the fp64 one, and the sum with the residual then lands on
+           the next midpoint and rounds away from the reference.
+
+    Returns frac (elements != want), maxulp (largest ulp distance to want among elements that are not tiny) and
+    err_over_tol (worst |y - ref| / (2^-7 |ref| [+ 2^-7 inter] + 1e-3 rms)).  A non-finite y makes maxulp and
+    err_over_tol infinite."""
+    y = y.contiguous()
+    ref64 = ref64.double()
+    if want is None:
+        want = ref64.to(torch.float32).to(BF)
+    want = want.to(BF).contiguous()
+    finite = bool(torch.isfinite(y).all())
+    rms = float(ref64.pow(2).mean().sqrt()) if ref64.numel() else 0.0
+    big = ref64.abs() > 0.05 * rms
+    tol = ref64.abs() * 2.0 ** -7 + 1e-3 * rms + 1e-30
+    if inter is not None:
+        inter = inter.double().abs()
+        big &= ref64.abs() >= inter
+        tol = tol + inter * 2.0 ** -7
+    ulp = (ordered_bf16(y) - ordered_bf16(want)).abs()
+    maxulp = float(ulp[big].max()) if bool(big.any()) else 0.0
+    err = float(((y.double() - ref64).abs() / tol).max()) if y.numel() else 0.0
+    if not finite:
+        maxulp, err = float("inf"), float("inf")
+    return {"frac": float((y != want).float().mean()) if y.numel() else 0.0, "maxulp": maxulp, "err_over_tol": err}
+
+
+# ------------------------------------------------------------------------------------------ per-row error
+def row_rel(y: torch.Tensor, ref: torch.Tensor, floor_frac: float = 0.05, atol: float = 0.0) -> torch.Tensor:
+    """Relative L2 error of every row (last dimension) of y against ref, as a tensor of the leading shape.
+
+    The denominator is the row norm of ref, floored at floor_frac x the median row norm so that near-zero rows do not
+    divide by zero, and at `atol`, a row norm on the scale of the inputs, for references that are zero as a whole (the
+    dq of a one-key attention is exactly 0; its kernel value is fp32 rounding noise).  A row of y with a non-finite
+    value scores +inf."""
+    y64, r64 = y.double(), ref.double()
+    err = (y64 - r64).norm(dim=-1)
+    nrm = r64.norm(dim=-1)
+    floor = floor_frac * float(nrm.flatten().median()) if nrm.numel() else 0.0
+    score = err / nrm.clamp_min(max(floor, atol, 1e-30))
+    return torch.where(torch.isfinite(y64).all(-1), score, torch.full_like(score, float("inf")))
+
+
+def row_worst(y: torch.Tensor, ref: torch.Tensor, floor_frac: float = 0.05, atol: float = 0.0) -> float:
+    """Worst per-row relative error (see row_rel): one score per (batch, head, row) of an attention tensor."""
+    r = row_rel(y, ref, floor_frac, atol)
+    return float(r.max()) if r.numel() else 0.0
+
+
+# ------------------------------------------------------------------------------------------ sentinels / poison
+def nan_buffer(shape, dtype=BF, device="cpu") -> torch.Tensor:
+    return torch.full(shape, NAN, dtype=dtype, device=device)
+
+
+def poisoned(values: torch.Tensor, rows: int, ld: int) -> torch.Tensor:
+    """A [rows, ld] buffer filled with NaN whose top-left corner holds `values` (2-D).  Kernels get its data pointer
+    and ld: an operand read past its logical extent turns the result into NaN instead of passing silently."""
+    buf = nan_buffer((rows, ld), values.dtype, values.device)
+    buf[:values.shape[0], :values.shape[1]] = values
+    return buf
+
+
+def sentinel_report(buf: torch.Tensor, inside, zero=None) -> dict:
+    """buf was NaN-filled before the kernel wrote the region `inside` (an index expression, e.g. (slice(0, M),
+    slice(0, N))).  Returns the number of sentinels outside `inside` and `zero` that changed, the number of elements of
+    `inside` still NaN (not written) and, for the padding region `zero` that must be written as exact zeros, the number
+    of elements that are not 0."""
+    mask_in = torch.zeros(buf.shape, dtype=torch.bool, device=buf.device)
+    mask_in[inside] = True
+    mask_zero = torch.zeros_like(mask_in)
+    if zero is not None:
+        mask_zero[zero] = True
+    isnan = torch.isnan(buf.float())
+    out = {"sentinels_changed": float((~isnan & ~mask_in & ~mask_zero).sum()),
+           "nan_in_range": float((isnan & mask_in).sum())}
+    if zero is not None:
+        out["padcols_nonzero"] = float(((buf.float() != 0) & mask_zero).sum())
+    return out

@@ -9,7 +9,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 GROUP_NAMES = ["gemm_fwd", "gemm_swiglu", "gemm_dgrad", "gemm_wgrad", "elementwise", "fused_rope", "attn_flash", "attn_wgmma", "attn_tiny", "loss_optim", "decode",
                "model_forward", "model_layer_tf", "model_train", "model_generate", "model_peaked_greedy", "model_large",
-               "gemm_exact", "decode_paged", "lora_train", "model_vs_hf", "model_medium_long"]
+               "gemm_exact", "decode_paged", "lora_train", "model_vs_hf", "model_medium_long",
+               "gemm_matrix", "gemm_epilogues", "attn_edges"]
 
 
 @pytest.mark.gpu
@@ -30,5 +31,9 @@ def test_gpu_group(group):
     import gpu_checks as G
     metrics = G.GROUPS[group]()
     torch.cuda.synchronize()
-    bad = [(k, v, b) for k, v, b, ok in G.verdict(metrics) if not ok]
+    res = G.verdict(metrics)
+    if group in G.STRICT_GROUPS:
+        unbounded = [k for k, v, b, ok in res if b is None]
+        assert not unbounded, f"{group}: metrics without a bound in THRESH: {unbounded}"
+    bad = [(k, v, b) for k, v, b, ok in res if not ok]
     assert not bad, f"{group}: out of tolerance: {bad}"
