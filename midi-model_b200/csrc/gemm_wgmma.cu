@@ -20,6 +20,7 @@ constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
 constexpr int MMA_K = 16;
 constexpr int CONSUMERS = 2;                            // consumer warpgroups (64 rows each)
 constexpr int NUM_THREADS = CONSUMERS * 128 + 32;       // + the producer warp
+constexpr int EPI_BOX_BYTES = 64 * 64 * 2;              // one 64-row x 64-column bf16 box of the TMA store
 
 enum { EPI_STORE = 0, EPI_RESIDUAL = 1, EPI_PARTIAL_F32 = 2, EPI_ROPE = 3, EPI_SWIGLU = 4 };
 
@@ -53,8 +54,11 @@ struct SmemLayout {
     static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;   // 16 / 32 KB
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int STAGES = (BLOCK_N == 256) ? 4 : 6;   // 192 KB of operand stages either way
+    // bf16 epilogue staging: two 64 x 64 boxes (8 KB, 1024-byte aligned for the 128B swizzle) per consumer warpgroup
+    static constexpr int EPI_BYTES = CONSUMERS * 2 * EPI_BOX_BYTES;
     static constexpr int BAR_BYTES = 256;
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + BAR_BYTES + 1024;   // +1024 for manual alignment
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + EPI_BYTES + BAR_BYTES + 1024;   // +1024 for manual alignment
+    static_assert(TOTAL <= 227 * 1024, "shared memory budget of an sm_90 CTA");
 };
 
 struct WorkItem {
@@ -120,24 +124,66 @@ __device__ __forceinline__ void rope_fragment(float* acc, const GemmParams& p, i
     }
 }
 
+// One 64 x 64 bf16 box of a warpgroup's output, staged in shared memory and stored by TMA at (col, row0) of `tm`.
+// value(jj, h, r) is the thread's packed column pair of 8-column group jj of the box in fragment row half h; r is the
+// matching packed pair of the residual `res` (pitch ldr, read only inside rows < M and columns < N), 0 without one.
+// The warpgroup alternates between its two staging slots (`boxes` counts the boxes it has issued).  Slot layout = the
+// store map's 128B swizzle: row r at byte 128 r, 16-byte chunk c at chunk c ^ (r % 8).  One (jj, h) write of a warp
+// covers 8 rows with r % 8 = lane / 4, so 8 distinct chunks, each written by 4 lanes in its 4 banks: all 32 banks once,
+// no conflicts.  Before the barrier the elected thread waits until the previous box's store has read its slot, so after
+// the barrier the other slot (the next box's) is free; this box's own slot was freed the same way one box earlier.
+template <typename F>
+__device__ __forceinline__ void store_box(uint8_t* staging, uint32_t& boxes, const CUtensorMap* tm, int col, int row0,
+                                          int wg, int r_lo, int lane, bool elected, const bf16* res, int ldr, int M, int N,
+                                          F value) {
+    uint32_t rv[2][8];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const int row = row0 + r_lo + 8 * h;
+        const bf16* rp = res + (size_t)row * ldr + col + 2 * (lane & 3);
+#pragma unroll
+        for (int jj = 0; jj < 8; jj++)   // all of the box's residual loads in flight before the first shared store
+            rv[h][jj] = (res != nullptr && row < M && col + 8 * jj < N) ? *reinterpret_cast<const uint32_t*>(rp + 8 * jj) : 0u;
+    }
+    uint8_t* slot = staging + (boxes & 1) * EPI_BOX_BYTES;
+    // the slot is 1024-byte aligned and r_lo % 8 = lane / 4, so chunk jj ^ (r % 8) of row r is at address ^ (jj << 4)
+    const uint32_t s0 = smem_u32(slot) + r_lo * 128 + ((lane >> 2) << 4) + 4 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+#pragma unroll
+        for (int jj = 0; jj < 8; jj++) st_shared_u32((s0 + h * 8 * 128) ^ (jj << 4), value(jj, h, rv[h][jj]));
+    }
+    fence_proxy_async_smem();
+    if (elected) bulk_wait_read<0>();
+    named_bar_sync(1 + wg, 128);
+    if (elected) {
+        tma_store_2d(tm, slot, col, row0);
+        bulk_commit();
+    }
+    boxes++;
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmAct, const GemmParams p) {
     using L = SmemLayout<BLOCK_N>;
     B200_PDL_TRIGGER();
     constexpr int STAGES = L::STAGES;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * L::STAGE_BYTES);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * L::STAGE_BYTES + L::EPI_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == 2 * 4 && lane == 0) {
+    if (warp == CONSUMERS * 4 && lane == 0) {
         prefetch_tmap(&tmA);
         prefetch_tmap(&tmB);
+        if (p.epilogue != EPI_PARTIAL_F32) prefetch_tmap(&tmC);
+        if (p.epilogue == EPI_SWIGLU) prefetch_tmap(&tmAct);
         for (int s = 0; s < STAGES; s++) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], CONSUMERS * 4); // one arrival per consumer warp, each after its own wait
@@ -151,7 +197,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
     const int total_items = p.total_items;
 
-    if (warp == 2 * 4) {
+    if (warp == CONSUMERS * 4) {
         // ===================== TMA producer =====================
         if (lane == 0) {
             int stage = 0;
@@ -198,6 +244,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // the second 64-row TMA box).  K-major operands: SBO = 1024 B between 8-row groups, K step = 32 B; MN-major:
     // LBO = 8 KB between 64-element MN boxes, SBO = 1024 B between 8-deep K groups, K step = 16 rows x 128 B.
     const uint32_t a_off = wg * (64 * 128);
+    uint8_t* staging = smem + STAGES * L::STAGE_BYTES + wg * (2 * EPI_BOX_BYTES);
+    const bool elected = (threadIdx.x & 127) == 0;   // issues and waits for this warpgroup's TMA stores
+    const int r_lo = wr * 16 + (lane >> 2);          // the thread's first fragment row inside the warpgroup's 64
+    uint32_t boxes = 0;
     int stage = 0;
     uint32_t phase = 0;
     float acc[BLOCK_N / 2];
@@ -227,70 +277,98 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         wgmma_wait<0>();
         if (prev >= 0 && signal) mbar_arrive(&empty_bar[prev]);
 
-        // ---- epilogue straight from the accumulator registers
-        const int r0 = wi.m_blk * BLOCK_M + wg * 64 + wr * 16 + (lane >> 2);
-        if (p.epilogue == EPI_ROPE) {
+        // ---- epilogue from the accumulator registers
+        if (wi.tail >= 0 || p.epilogue == EPI_PARTIAL_F32) {
+            // fp32 partials, stored straight from the fragment
 #pragma unroll
             for (int h = 0; h < 2; h++) {
-                if (p.rope_D == 64) rope_fragment<BLOCK_N, 4>(acc, p, wi.n_blk, r0 + 8 * h, h, cq);
-                else if (p.rope_D == 128) rope_fragment<BLOCK_N, 8>(acc, p, wi.n_blk, r0 + 8 * h, h, cq);
-                else rope_fragment<BLOCK_N, 16>(acc, p, wi.n_blk, r0 + 8 * h, h, cq);
-            }
-        }
+                const int r_t = wg * 64 + r_lo + 8 * h;          // row inside the tile
+                if (wi.tail >= 0) {
+                    // K-slice of a tail tile: tile-local layout [128][BLOCK_N]
+                    float* dst = p.tail_ws + ((size_t)(wi.tail * p.tail_splits + wi.split) * BLOCK_M + r_t) * BLOCK_N + cq;
 #pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const int row = r0 + 8 * h;
-            if (wi.tail >= 0) {
-                // K-slice of a tail tile: fp32 partial, tile-local layout [128][BLOCK_N]
-                const int r_t = row - wi.m_blk * BLOCK_M;
-                float* dst = p.tail_ws + ((size_t)(wi.tail * p.tail_splits + wi.split) * BLOCK_M + r_t) * BLOCK_N + cq;
-#pragma unroll
-                for (int j = 0; j < BLOCK_N / 8; j++)
-                    *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-                continue;
-            }
-            if (row >= p.M) continue;
-            if (BLOCK_N == 256 && p.epilogue == EPI_SWIGLU) {
-                // gate|up projection with SwiGLU fused (hf modeling_llama.py:183): accumulator columns [0,128) are gate
-                // features, [128,256) the matching up features.  g, u = bf16(acc) are stored (backward needs them) and
-                // act = bf16(bf16(silu(g)) * u) -- same rounding points as the stand-alone kernel.
-                const int f0 = wi.n_blk * 128 + cq;
-                bf16* dg = p.C + (size_t)row * p.ldc + f0;
-                bf16* du = dg + p.swiglu_I;
-                bf16* da = p.act + (size_t)row * p.ld_act + f0;
-#pragma unroll
-                for (int j = 0; j < 16; j++) {
-                    const float g0 = bf16_round(acc[4 * j + 2 * h]), g1 = bf16_round(acc[4 * j + 2 * h + 1]);
-                    const float u0 = bf16_round(acc[4 * (j + 16) + 2 * h]), u1 = bf16_round(acc[4 * (j + 16) + 2 * h + 1]);
-                    *reinterpret_cast<uint32_t*>(dg + 8 * j) = pack2(g0, g1);
-                    *reinterpret_cast<uint32_t*>(du + 8 * j) = pack2(u0, u1);
-                    *reinterpret_cast<uint32_t*>(da + 8 * j) = pack2(bf16_round(silu_f(g0)) * u0, bf16_round(silu_f(g1)) * u1);
+                    for (int j = 0; j < BLOCK_N / 8; j++)
+                        *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                    continue;
                 }
-            } else if (p.epilogue == EPI_PARTIAL_F32) {
+                const int row = wi.m_blk * BLOCK_M + r_t;
+                if (row >= p.M) continue;
                 float* dst = p.ws + ((size_t)wi.split * p.M + row) * p.N + wi.n_blk * BLOCK_N + cq;
 #pragma unroll
                 for (int j = 0; j < BLOCK_N / 8; j++)
                     if (wi.n_blk * BLOCK_N + 8 * j < p.N)
                         *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-            } else {
-                // plain / residual / RoPE'd bf16 store (N is padded to a multiple of 8: whole 8-column groups only)
-                bf16* dst = p.C + (size_t)row * p.ldc + wi.n_blk * BLOCK_N + cq;
-                const bf16* res = (p.epilogue == EPI_RESIDUAL) ? p.R + (size_t)row * p.ldr + wi.n_blk * BLOCK_N + cq : nullptr;
+            }
+            continue;
+        }
+        // bf16 outputs go through shared memory in 64 x 64 boxes and are stored by TMA, which clips rows >= M and
+        // columns >= N (= roundup8 of the caller's N; the columns in between hold zeros: B rows >= N were zero-filled);
+        // the warpgroup goes on to its next tile's MMAs while the stores drain
+        const int row0 = wi.m_blk * BLOCK_M + wg * 64;
+        if (row0 >= p.M) continue;
+        if (p.epilogue == EPI_ROPE) {
 #pragma unroll
-                for (int j = 0; j < BLOCK_N / 8; j++) {
-                    if (wi.n_blk * BLOCK_N + 8 * j < p.N) {
-                        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-                        if (res != nullptr) {
-                            const float2 rr = __bfloat1622float2(*reinterpret_cast<const bf162*>(res + 8 * j));
-                            f0 = bf16_round(f0) + rr.x;
-                            f1 = bf16_round(f1) + rr.y;
-                        }
-                        *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2(f0, f1);
+            for (int h = 0; h < 2; h++) {
+                const int row = row0 + r_lo + 8 * h;
+                if (p.rope_D == 64) rope_fragment<BLOCK_N, 4>(acc, p, wi.n_blk, row, h, cq);
+                else if (p.rope_D == 128) rope_fragment<BLOCK_N, 8>(acc, p, wi.n_blk, row, h, cq);
+                else rope_fragment<BLOCK_N, 16>(acc, p, wi.n_blk, row, h, cq);
+            }
+        }
+        if (BLOCK_N == 256 && p.epilogue == EPI_SWIGLU) {
+            // gate|up projection with SwiGLU fused (hf modeling_llama.py:183): accumulator columns [0,128) are gate
+            // features, [128,256) the matching up features.  g, u = bf16(acc) are stored (backward needs them) and
+            // act = bf16(bf16(silu(g)) * u) -- same rounding points as the stand-alone kernel.
+            const int f0 = wi.n_blk * 128;
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                store_box(staging, boxes, &tmC, f0 + 64 * q, row0, wg, r_lo, lane, elected, nullptr, 0, 0, 0,
+                          [&](int jj, int h, uint32_t) {
+                    const int j = 8 * q + jj;
+                    return pack2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                });
+            }
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                store_box(staging, boxes, &tmC, p.swiglu_I + f0 + 64 * q, row0, wg, r_lo, lane, elected, nullptr, 0, 0, 0,
+                          [&](int jj, int h, uint32_t) {
+                    const int j = 16 + 8 * q + jj;
+                    return pack2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                });
+            }
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                store_box(staging, boxes, &tmAct, f0 + 64 * q, row0, wg, r_lo, lane, elected, nullptr, 0, 0, 0,
+                          [&](int jj, int h, uint32_t) {
+                    const int j = 8 * q + jj;
+                    const float g0 = bf16_round(acc[4 * j + 2 * h]), g1 = bf16_round(acc[4 * j + 2 * h + 1]);
+                    const float u0 = bf16_round(acc[4 * (j + 16) + 2 * h]), u1 = bf16_round(acc[4 * (j + 16) + 2 * h + 1]);
+                    return pack2(bf16_round(silu_f(g0)) * u0, bf16_round(silu_f(g1)) * u1);
+                });
+            }
+        } else {
+            // plain / residual / RoPE'd bf16 store
+            const bool residual = p.epilogue == EPI_RESIDUAL;
+#pragma unroll
+            for (int b = 0; b < BLOCK_N / 64; b++) {
+                const int col = wi.n_blk * BLOCK_N + 64 * b;
+                if (col >= p.N) break;
+                store_box(staging, boxes, &tmC, col, row0, wg, r_lo, lane, elected, residual ? p.R : nullptr, p.ldr, p.M,
+                          p.N, [&](int jj, int h, uint32_t r) {
+                    const int j = 8 * b + jj;
+                    float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                    if (residual) {
+                        const float2 rr = __bfloat1622float2(*reinterpret_cast<const bf162*>(&r));
+                        f0 = bf16_round(f0) + rr.x;
+                        f1 = bf16_round(f1) + rr.y;
                     }
-                }
+                    return pack2(f0, f1);
+                });
             }
         }
     }
+    // the staging slots must stay untouched until the last stores have read them; the CTA exits after they completed
+    if (elected) bulk_wait_all();
 }
 
 __global__ void splitk_reduce_kernel(const float* __restrict__ ws, bf16* __restrict__ out, size_t n, int splits,
@@ -337,7 +415,8 @@ __global__ void tail_reduce_kernel(const float* __restrict__ ws, bf16* __restric
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmAct,
+           const GemmParams& p, cudaStream_t stream) {
     using L = SmemLayout<BLOCK_N>;
     auto kern = gemm_wgmma_kernel<BLOCK_N, A_MN, B_MN>;
     static bool configured = false;
@@ -366,7 +445,7 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, 
     }
     cfg.attrs = attr;
     cfg.numAttrs = n_attr;
-    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p), "gemm launch");
+    B200_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, tmAct, p), "gemm launch");
     B200_CHECK_LAUNCH("gemm_wgmma");
     return B200_OK;
 }
@@ -641,13 +720,23 @@ static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M
     if (!b_mn_major) rc = hopper::make_tmap_2d(&tmB, B, K, N, ldb, BLOCK_K, swiglu ? 128 : block_n);
     else             rc = hopper::make_tmap_2d(&tmB, B, N, K, ldb, 64, BLOCK_K);
     if (rc) return rc;
+    // bf16 outputs: 64 x 64 boxes stored from the epilogue's staging slots (unused maps stay zero)
+    CUtensorMap tmC = {}, tmAct = {};
+    if (p.epilogue != EPI_PARTIAL_F32) {
+        rc = hopper::make_tmap_2d(&tmC, C, N8, M, ldc, 64, 64);
+        if (rc) return rc;
+    }
+    if (swiglu) {
+        rc = hopper::make_tmap_2d(&tmAct, p.act, p.swiglu_I, M, p.ld_act, 64, 64);
+        if (rc) return rc;
+    }
 
-#define B200_DISPATCH(BN)                                                                          \
-    do {                                                                                           \
-        if (!a_mn_major && !b_mn_major) rc = launch<BN, false, false>(tmA, tmB, p, stream);        \
-        else if (!a_mn_major && b_mn_major) rc = launch<BN, false, true>(tmA, tmB, p, stream);     \
-        else if (a_mn_major && b_mn_major) rc = launch<BN, true, true>(tmA, tmB, p, stream);       \
-        else rc = launch<BN, true, false>(tmA, tmB, p, stream);                                    \
+#define B200_DISPATCH(BN)                                                                                  \
+    do {                                                                                                   \
+        if (!a_mn_major && !b_mn_major) rc = launch<BN, false, false>(tmA, tmB, tmC, tmAct, p, stream);    \
+        else if (!a_mn_major && b_mn_major) rc = launch<BN, false, true>(tmA, tmB, tmC, tmAct, p, stream); \
+        else if (a_mn_major && b_mn_major) rc = launch<BN, true, true>(tmA, tmB, tmC, tmAct, p, stream);   \
+        else rc = launch<BN, true, false>(tmA, tmB, tmC, tmAct, p, stream);                                \
     } while (0)
     if (block_n == 256) B200_DISPATCH(256);
     else B200_DISPATCH(128);

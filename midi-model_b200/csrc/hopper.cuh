@@ -46,6 +46,29 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }
 
+// TMA store of one box from shared memory (laid out as the tensor map's swizzle expects) to global; elements outside
+// the tensor map's bounds are not written.  Completion is tracked per issuing thread through bulk async-groups.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tm),
+                 "r"(smem_u32(src)), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's committed bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// wait until every committed bulk group of this thread has completed (global writes done)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
+}
+// make this thread's generic-proxy shared-memory writes visible to the async proxy (TMA) before it reads them
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // Shared-memory matrix descriptor (sm_90 wgmma format): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
 // base offset [49,52) = 0 (stage buffers are 1024-byte aligned) | layout [62,64) (1 = SWIZZLE_128B).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
