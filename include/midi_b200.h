@@ -44,6 +44,16 @@ int b200_embed_sum_fwd(const long long* ids, const void* table, void* out, int M
 int b200_inner_input_fwd(const void* hidden /*may be NULL*/, const long long* ids, const void* table, void* out,
                          int n_events, int n_ids, int H, int V, cudaStream_t s);
 int b200_inner_input_bwd_hidden(const void* dx, void* dhidden, int n_events, int Tin, int H, cudaStream_t s);
+/* train.py --sample-seq (train.py:172-178: hidden[:, rand_idx], y[:, rand_idx]): event n of the token-level input is event
+   row rows[n] (device int32 [n_events]) of hidden [n_rows, H] and of the labels y int64 [n_rows, T]:
+   out[n*T] = hidden[rows[n]], out[n*T + 1 + t] = table[y[rows[n], t]] (t < T-1), and y_sel[n] = y[rows[n]] (int64
+   [n_events, T]).  A row outside [0, n_rows) gives zero input rows and labels -1. */
+int b200_inner_input_rows_fwd(const void* hidden, const long long* y, const int* rows, const void* table, void* out,
+                              long long* y_sel, int n_events, int n_rows, int T, int H, int V, cudaStream_t s);
+/* its backward for hidden: dhidden [n_rows, H] in full, dhidden[r] = dx[inv[r] * Tin] where inv[r] (device int32 [n_rows])
+   is in [0, n_events), zero for every other row (inv[r] = -1).  Each selected row must appear once in inv. */
+int b200_inner_input_rows_bwd_hidden(const void* dx, const int* inv, void* dhidden, int n_rows, int n_events, int Tin, int H,
+                                     cudaStream_t s);
 /* host data path (train.py:71 int16 token matrices; train.py:169-176 x = batch[:, :-1], y = batch[:, 1:]):
    batch int16 [B, S1, T] -> x, y int64 [B*(S1-1), T] in one pass */
 int b200_batch_to_xy_i16(const void* batch, int B, int S1, int T, long long* x, long long* y, cudaStream_t s);
@@ -150,6 +160,13 @@ int b200_ce_bwd(void* logits_inout, const long long* targets, const float* lse, 
                 long long rows, int V, int ld, long long ignore_index, float grad_scale,
                 const void* grad_scale_dev /*may be NULL: device scalar multiplied into grad_scale*/,
                 int grad_scale_is_bf16, cudaStream_t s);
+/*      validation accuracy (train.py:153-166, 204): per row of pitched logits [rows, ld >= V] the argmax over columns < V,
+ *      as torch.argmax gives it (NaN is the maximum, ties go to the lowest index; columns V..ld are not read);
+ *      hits_and_count = {#rows with argmax == target, #rows with a target in [0, V) other than ignore_index}.
+ *      workspace: int[2 * b200_argmax_hits_parts()] */
+int b200_argmax_hits_parts(void);
+int b200_argmax_hits(const void* logits, const long long* targets, long long rows, int V, int ld, long long ignore_index,
+                     float* hits_and_count /*float[2]*/, void* workspace, size_t workspace_bytes, cudaStream_t s);
 
 /* ---- optimizer (train.py:121-138 AdamW groups; :464 gradient_clip_val) ----------------------------- */
 int b200_gradnorm_parts(void);

@@ -58,6 +58,45 @@ __global__ void inner_input_bwd_hidden_kernel(const bf16* __restrict__ dx, bf16*
             *reinterpret_cast<const uint4*>(dx + (size_t)e * Tin * H + v * 8);
 }
 
+// train.py --sample-seq (train.py:172-178): event n is event row rows[n] of hidden [n_rows, H] / y [n_rows, T].
+// Block (n, j): out[n*T + j] = j == 0 ? hidden[rows[n]] : table[y[rows[n], j-1]], and y_sel[n, j] = y[rows[n], j].
+// A row outside [0, n_rows) reads nothing: its input rows are zero and its labels -1 (ignored by the loss and the
+// embedding backward).
+__global__ void inner_input_rows_fwd_kernel(const bf16* __restrict__ hidden, const long long* __restrict__ y,
+                                            const int* __restrict__ rows, const bf16* __restrict__ table,
+                                            bf16* __restrict__ out, long long* __restrict__ y_sel, int n_rows, int T,
+                                            int H, int V) {
+    const int n = blockIdx.x / T, j = blockIdx.x % T;
+    const int r = rows[n];
+    const bool live = r >= 0 && r < n_rows;
+    const bf16* src = nullptr;
+    if (live) {
+        if (j == 0) {
+            src = hidden + (size_t)r * H;
+        } else {
+            long long id = y[(size_t)r * T + j - 1];
+            if (id < 0 || id >= V) id = 0;
+            src = table + (size_t)id * H;
+        }
+    }
+    if (threadIdx.x == 0) y_sel[(size_t)n * T + j] = live ? y[(size_t)r * T + j] : -1;
+    bf16* dst = out + ((size_t)n * T + j) * H;
+    for (int v = threadIdx.x; v < H / 8; v += blockDim.x)
+        *reinterpret_cast<uint4*>(dst + v * 8) = live ? *reinterpret_cast<const uint4*>(src + v * 8) : make_uint4(0, 0, 0, 0);
+}
+
+// dhidden[r,:] = dx[inv[r]*Tin, :] for a selected row (inv[r] in [0, n_events)), zero for every other row: the full
+// gradient of the event-level output in one pass.  Indices are unique, so every row is written exactly once.
+__global__ void inner_input_rows_bwd_hidden_kernel(const bf16* __restrict__ dx, const int* __restrict__ inv,
+                                                   bf16* __restrict__ dhidden, int n_events, int Tin, int H) {
+    const int r = blockIdx.x;
+    const int e = inv[r];
+    const bool live = e >= 0 && e < n_events;
+    for (int v = threadIdx.x; v < H / 8; v += blockDim.x)
+        *reinterpret_cast<uint4*>(dhidden + (size_t)r * H + v * 8) =
+            live ? *reinterpret_cast<const uint4*>(dx + (size_t)e * Tin * H + v * 8) : make_uint4(0, 0, 0, 0);
+}
+
 // ---- embedding backward: counting sort of the ids, then one segment-sum per (id, slice) ----
 // id i (flat index) reads gradient row  (i / per_row) * row_stride + (i % per_row) * row_inner + row_off
 __global__ void embed_hist_kernel(const long long* __restrict__ ids, int n, int V, int* __restrict__ counts) {
@@ -594,6 +633,36 @@ extern "C" int b200_inner_input_bwd_hidden(const void* dx, void* dhidden, int n_
     if (n_events == 0) return B200_OK;
     inner_input_bwd_hidden_kernel<<<n_events, ROW_THREADS, 0, stream>>>((const bf16*)dx, (bf16*)dhidden, Tin, H);
     B200_CHECK_LAUNCH("inner_input_bwd_hidden");
+    return B200_OK;
+}
+
+extern "C" int b200_inner_input_rows_fwd(const void* hidden, const long long* y, const int* rows, const void* table,
+                                         void* out, long long* y_sel, int n_events, int n_rows, int T, int H, int V,
+                                         cudaStream_t stream) {
+    B200_CHECK_ARG(H % 8 == 0, "inner_input_rows_fwd: H must be a multiple of 8");
+    B200_CHECK_ARG(n_events >= 0 && n_rows >= 0 && T >= 1 && V >= 1,
+                   "inner_input_rows_fwd: bad sizes (n_events %d, n_rows %d, T %d, V %d)", n_events, n_rows, T, V);
+    B200_CHECK_ARG(n_events == 0 || (hidden && y && rows && table && out && y_sel),
+                   "inner_input_rows_fwd: null pointer");
+    B200_CHECK_ARG((long long)n_events * T <= 0x7fffffffLL, "inner_input_rows_fwd: too many rows");
+    if (n_events == 0) return B200_OK;
+    inner_input_rows_fwd_kernel<<<n_events * T, ROW_THREADS, 0, stream>>>((const bf16*)hidden, y, rows,
+                                                                          (const bf16*)table, (bf16*)out, y_sel, n_rows,
+                                                                          T, H, V);
+    B200_CHECK_LAUNCH("inner_input_rows_fwd");
+    return B200_OK;
+}
+
+extern "C" int b200_inner_input_rows_bwd_hidden(const void* dx, const int* inv, void* dhidden, int n_rows, int n_events,
+                                                int Tin, int H, cudaStream_t stream) {
+    B200_CHECK_ARG(H % 8 == 0, "inner_input_rows_bwd_hidden: H must be a multiple of 8");
+    B200_CHECK_ARG(n_rows >= 0 && n_events >= 0 && Tin >= 1,
+                   "inner_input_rows_bwd_hidden: bad sizes (n_rows %d, n_events %d, Tin %d)", n_rows, n_events, Tin);
+    B200_CHECK_ARG(n_rows == 0 || (inv && dhidden && (dx || n_events == 0)), "inner_input_rows_bwd_hidden: null pointer");
+    if (n_rows == 0) return B200_OK;
+    inner_input_rows_bwd_hidden_kernel<<<n_rows, ROW_THREADS, 0, stream>>>((const bf16*)dx, inv, (bf16*)dhidden,
+                                                                           n_events, Tin, H);
+    B200_CHECK_LAUNCH("inner_input_rows_bwd_hidden");
     return B200_OK;
 }
 

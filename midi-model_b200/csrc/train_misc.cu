@@ -172,6 +172,77 @@ ce_bwd_kernel(bf16* __restrict__ logits, const long long* __restrict__ targets, 
     }
 }
 
+// ---- validation accuracy (train.py:153-166, 204): argmax of each logits row vs its label ----------------------------
+// (a, ia) beats (b, ib) under torch.argmax's order: NaN is the maximum, ties go to the lower index; index -1 = no value yet
+__device__ __forceinline__ bool argmax_beats(float a, int ia, float b, int ib) {
+    if (ib < 0) return ia >= 0;
+    if (ia < 0) return false;
+    const bool na = isnan(a), nb = isnan(b);
+    if (na || nb) return na && (!nb || ia < ib);
+    return a > b || (a == b && ia < ib);
+}
+
+// One warp per row: 16-byte loads over the whole 8-column vectors below V, scalar loads for the last V % 8 columns
+// (the pad columns V..ld are never read).  Each CTA writes its (hits, count) pair to partial[blockIdx.x].
+constexpr int AH_WARPS = 4;
+__global__ void __launch_bounds__(AH_WARPS * 32)
+argmax_hits_kernel(const bf16* __restrict__ logits, const long long* __restrict__ targets, long long R, int V, int ld,
+                   long long ignore_index, int* __restrict__ partial) {
+    __shared__ int sh[AH_WARPS][2];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int nfull = V / 8;
+    int hits = 0, count = 0;
+    for (long long r = (long long)blockIdx.x * AH_WARPS + warp; r < R; r += (long long)gridDim.x * AH_WARPS) {
+        const bf16* row = logits + (size_t)r * ld;
+        float best = 0.f;
+        int bi = -1;
+#pragma unroll 4
+        for (int v = lane; v < nfull; v += 32) {
+            float f[8];
+            unpack8(ld_nc16(row + v * 8), f);
+#pragma unroll
+            for (int j = 0; j < 8; j++)
+                if (argmax_beats(f[j], v * 8 + j, best, bi)) { best = f[j]; bi = v * 8 + j; }
+        }
+        for (int c = nfull * 8 + lane; c < V; c += 32) {
+            const float f = __bfloat162float(row[c]);
+            if (argmax_beats(f, c, best, bi)) { best = f; bi = c; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (argmax_beats(ob, oi, best, bi)) { best = ob; bi = oi; }
+        }
+        if (lane == 0) {
+            const long long t = targets[r];
+            const bool live = !(t == ignore_index || t < 0 || t >= V);
+            count += live;
+            hits += live && (long long)bi == t;
+        }
+    }
+    if (lane == 0) { sh[warp][0] = hits; sh[warp][1] = count; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int h = 0, c = 0;
+        for (int w = 0; w < AH_WARPS; w++) { h += sh[w][0]; c += sh[w][1]; }
+        partial[2 * blockIdx.x] = h;
+        partial[2 * blockIdx.x + 1] = c;
+    }
+}
+
+// one warp: out = {hits, count} summed over the CTA partials (integer sums: exact, whatever the order)
+__global__ void argmax_hits_reduce_kernel(const int* __restrict__ partial, int nparts, float* __restrict__ out) {
+    long long h = 0, c = 0;
+    for (int i = threadIdx.x; i < nparts; i += 32) { h += partial[2 * i]; c += partial[2 * i + 1]; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        h += __shfl_xor_sync(0xffffffffu, h, o);
+        c += __shfl_xor_sync(0xffffffffu, c, o);
+    }
+    if (threadIdx.x == 0) { out[0] = (float)h; out[1] = (float)c; }
+}
+
 // ---- grad norm / clip / AdamW over flat buffers ---------------------------------------------
 __global__ void sumsq_kernel(const bf16* __restrict__ g, size_t n, float* __restrict__ partials) {
     __shared__ float sh[32];
@@ -269,6 +340,31 @@ extern "C" int b200_ce_bwd(void* logits_inout, const long long* targets, const f
                                                              n_cols_store, ignore_index, grad_scale, grad_scale_dev,
                                                              grad_scale_is_bf16);
     B200_CHECK_LAUNCH("ce_bwd");
+    return B200_OK;
+}
+
+extern "C" int b200_argmax_hits_parts(void) { return b200_num_sms() * 16; }
+
+// workspace: int[2 * b200_argmax_hits_parts()]; hits_and_count: float[2] on device
+extern "C" int b200_argmax_hits(const void* logits, const long long* targets, long long rows, int V, int ld,
+                                long long ignore_index, float* hits_and_count, void* workspace, size_t workspace_bytes,
+                                cudaStream_t stream) {
+    const int parts = b200_argmax_hits_parts();
+    B200_CHECK_ARG(V >= 1 && ld % 8 == 0 && ld >= V, "argmax_hits: ld (%d) must be a multiple of 8 and >= V (%d)", ld, V);
+    B200_CHECK_ARG(rows >= 0, "argmax_hits: negative row count");
+    B200_CHECK_ARG(workspace_bytes >= (size_t)parts * 2 * sizeof(int), "argmax_hits: workspace too small");
+    B200_CHECK_ARG(hits_and_count != nullptr && workspace != nullptr, "argmax_hits: null pointer");
+    B200_CHECK_ARG(rows == 0 || (logits != nullptr && targets != nullptr && (uintptr_t)logits % 16 == 0),
+                   "argmax_hits: logits must be 16-byte aligned");
+    long long blocks = (rows + AH_WARPS - 1) / AH_WARPS;
+    const int grid = (int)(blocks < parts ? blocks : parts);
+    if (grid > 0) {
+        argmax_hits_kernel<<<grid, AH_WARPS * 32, 0, stream>>>((const bf16*)logits, targets, rows, V, ld, ignore_index,
+                                                               (int*)workspace);
+        B200_CHECK_LAUNCH("argmax_hits");
+    }
+    argmax_hits_reduce_kernel<<<1, 32, 0, stream>>>((const int*)workspace, grid, hits_and_count);
+    B200_CHECK_LAUNCH("argmax_hits_reduce");
     return B200_OK;
 }
 

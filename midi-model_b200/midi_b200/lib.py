@@ -26,6 +26,8 @@ SIGNATURES = {
     "b200_embed_sum_fwd": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "b200_inner_input_fwd": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "b200_inner_input_bwd_hidden": (i32, [vp, vp, i32, i32, i32, vp]),
+    "b200_inner_input_rows_fwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+    "b200_inner_input_rows_bwd_hidden": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "b200_batch_to_xy_i16": (i32, [vp, i32, i32, i32, vp, vp, vp]),
     "b200_embed_bwd_workspace_bytes": (sz, [i32, i32, i32]),
     "b200_embed_bwd": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, sz, vp]),
@@ -53,6 +55,8 @@ SIGNATURES = {
     "b200_attn_tiny_bwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200_ce_fwd": (i32, [vp, vp, vp, vp, vp, i64, i32, i32, i64, vp]),
     "b200_ce_bwd": (i32, [vp, vp, vp, vp, i64, i32, i32, i64, f32, vp, i32, vp]),
+    "b200_argmax_hits_parts": (i32, []),
+    "b200_argmax_hits": (i32, [vp, vp, i64, i32, i32, i64, vp, vp, sz, vp]),
     "b200_gradnorm_parts": (i32, []),
     "b200_grad_clip_coef": (i32, [vp, i64, f32, vp, vp, sz, vp]),
     "b200_adamw_step": (i32, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, i32, vp, vp]),

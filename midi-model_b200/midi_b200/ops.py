@@ -60,6 +60,36 @@ def inner_input(hidden: Optional[torch.Tensor], ids: Optional[torch.Tensor], tab
     return out
 
 
+def inner_input_rows(hidden: torch.Tensor, y: torch.Tensor, rows: torch.Tensor, table: torch.Tensor):
+    """train.py --sample-seq: hidden [R, H], labels y int64 [R, T], rows int32 [n] (device) -> (xin [n*T, H] =
+    cat([hidden[rows], embed(y[rows, :-1])]) row by row, y_sel = y[rows] int64 [n, T])."""
+    V, H = table.shape
+    R, T = y.shape
+    if hidden.shape != (R, H) or rows.dtype != torch.int32 or rows.dim() != 1 or y.dtype != torch.long:
+        raise lib.B200Error(f"inner_input_rows: hidden {tuple(hidden.shape)}, y {tuple(y.shape)} {y.dtype}, rows "
+                            f"{tuple(rows.shape)} {rows.dtype}: expected [R, {H}], int64 [R, T], int32 [n]")
+    hidden, y, rows = hidden.contiguous(), y.contiguous(), rows.contiguous()
+    n = rows.shape[0]
+    out = torch.empty((n * T, H), dtype=BF16, device=table.device)
+    y_sel = torch.empty((n, T), dtype=torch.long, device=table.device)
+    lib.call("b200_inner_input_rows_fwd", hidden.data_ptr(), y.data_ptr(), rows.data_ptr(), table.data_ptr(), out.data_ptr(),
+             y_sel.data_ptr(), n, R, T, H, V, lib.stream())
+    return out, y_sel
+
+
+def inner_input_rows_bwd_hidden(dx: torch.Tensor, inv: torch.Tensor, n_events: int, Tin: int) -> torch.Tensor:
+    """dx [n_events*Tin, H], inv int32 [R] (device; event of each row or -1) -> dhidden [R, H]: position 0 of the row's
+    event, zero for unselected rows."""
+    H = dx.shape[1]
+    R = inv.shape[0]
+    if inv.dtype != torch.int32 or inv.dim() != 1 or dx.shape[0] != n_events * Tin:
+        raise lib.B200Error(f"inner_input_rows_bwd_hidden: dx {tuple(dx.shape)}, inv {tuple(inv.shape)} {inv.dtype}")
+    dhidden = torch.empty((R, H), dtype=BF16, device=dx.device)
+    lib.call("b200_inner_input_rows_bwd_hidden", dx.data_ptr(), inv.data_ptr(), dhidden.data_ptr(), R, n_events, Tin, H,
+             lib.stream())
+    return dhidden
+
+
 def batch_to_xy(batch: torch.Tensor):
     """int16 [B, S+1, T] token batch (train.py:71) -> (x, y) int64 [B*S, T]: x = batch[:, :-1], y = batch[:, 1:]."""
     if not batch.is_cuda or batch.dtype != torch.int16 or not batch.is_contiguous():
@@ -347,6 +377,18 @@ def ce_fwd(logits: torch.Tensor, targets: torch.Tensor, V: int, ignore_index: in
     lib.call("b200_ce_fwd", logits.data_ptr(), targets.data_ptr(), lse.data_ptr(), row_loss.data_ptr(), lac.data_ptr(), R, V,
              ld, ignore_index, lib.stream())
     return lac, lse
+
+
+def argmax_hits(logits: torch.Tensor, targets: torch.Tensor, V: int, ignore_index: int) -> torch.Tensor:
+    """logits [R, ld] bf16 (ld >= V), targets [R] int64 -> fp32[2] = {#rows whose argmax over the first V columns equals
+    the target, #rows whose target counts (not ignore_index, in [0, V))}."""
+    R, ld = logits.shape[0], logits.stride(0)
+    out = torch.empty((2,), dtype=torch.float32, device=logits.device)
+    parts = lib.query("b200_argmax_hits_parts")
+    ws = _ws("argmax_hits", parts * 8, logits.device)
+    lib.call("b200_argmax_hits", logits.data_ptr(), targets.data_ptr(), R, V, ld, ignore_index, out.data_ptr(),
+             ws.data_ptr(), ws.numel(), lib.stream())
+    return out
 
 
 def ce_bwd_(logits: torch.Tensor, targets: torch.Tensor, lse: torch.Tensor, lac: torch.Tensor, V: int, ignore_index: int,

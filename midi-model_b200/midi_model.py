@@ -15,14 +15,16 @@ LoRA (`train.py --task lora`, train.py:439-449): `add_adapter` injects adapters 
 peft is installed, midi_b200/lora.py otherwise); the engine then computes y = W x + (lora_alpha / r) B A x, trains A and B
 only, and `generate` reads merged copies.
 
-Extra (non-reference) entry points used by the fused trainer and the benchmark: `training_loss(batch)`,
-`fused_optimizer_step(...)`, `optimizer_state_dict()` / `load_optimizer_state_dict()`, `generate_stream(...)`
-(app.py:27-120), `load_adapter_weights(dir)`.
+Extra (non-reference) entry points used by the fused trainer and the benchmark: `training_loss(batch)` (with
+`sample_idx=` for train.py --sample-seq), `validation_metrics(batch)`, `fused_optimizer_step(...)`,
+`optimizer_state_dict()` / `load_optimizer_state_dict()`, `generate_stream(...)` (app.py:27-120), `load_adapter_weights(dir)`.
 """
 from __future__ import annotations
 
+import collections.abc
 import json
 import math
+import numbers
 import os
 import threading
 from typing import Any, Dict, Optional, Union
@@ -298,8 +300,9 @@ class LazyLogits(torch.Tensor):
             return _LazyCEFn.apply(input, buf, target.contiguous(), V, int(ignore_index))
 
 
-def _inner_backward(rt, model, sv, hs, dlogits, ids, N, L, n_ids, has_hidden, g, g_head, accumulate):
-    """dlogits [N*L, pitch] -> grads of lm_head, the token-level stack, its embedding; returns (dhidden,)."""
+def _inner_backward(rt, model, sv, hs, dlogits, ids, N, L, n_ids, has_hidden, g, g_head, accumulate, hidden_rows=None):
+    """dlogits [N*L, pitch] -> grads of lm_head, the token-level stack, its embedding; returns (dhidden,).
+    `hidden_rows` (int32 device [R], event of each hidden row or -1): dhidden is [R, H], zero for unselected rows."""
     # lm_head weight gradient on the engine's side stream (joined at the end of rt.inner.backward)
     side = _engine._side_stream(dlogits.device) if _engine.WGRAD_STREAM else None
     if g_head is not None:                       # None: lm_head is frozen (LoRA run, train.py:440)
@@ -315,10 +318,65 @@ def _inner_backward(rt, model, sv, hs, dlogits, ids, N, L, n_ids, has_hidden, g,
         if not accumulate:
             g.embed.zero_()
     dhidden = None
-    if has_hidden:
+    if has_hidden and hidden_rows is not None:
+        dhidden = _ops.inner_input_rows_bwd_hidden(dx, hidden_rows, N, L)
+    elif has_hidden:
         dhidden = torch.empty((N, rt.H), dtype=torch.bfloat16, device=dx.device)
         _lib.call("b200_inner_input_bwd_hidden", dx.data_ptr(), dhidden.data_ptr(), N, L, rt.H, _lib.stream())
     return (dhidden,)
+
+
+def _batch_xy(batch: torch.Tensor):
+    """train.py:169-170 on a (B, S+1, T) batch: x = batch[:, :-1], y = batch[:, 1:] as int64 [B*S, T]."""
+    B, S1, T = batch.shape
+    if batch.dtype == torch.int16:
+        return _ops.batch_to_xy(batch.contiguous())        # int16 host data path (midi_b200/data.py): one widening pass
+    batch = batch.to(torch.long)
+    return batch[:, :-1].contiguous().view(B * (S1 - 1), T), batch[:, 1:].contiguous().view(B * (S1 - 1), T)
+
+
+def _sample_positions(sample_idx, S: int) -> list:
+    """The event positions of train.py --sample-seq (train.py:173: `[-1] + random.sample(range(S - 2), k)`) as distinct
+    ints in [0, S); negative positions count from the end, as Python indexing does."""
+    what = "training_loss: sample_idx"
+    if isinstance(sample_idx, torch.Tensor):
+        if sample_idx.device.type != "cpu":
+            raise _lib.B200Error(f"{what} must be a CPU tensor or a Python sequence (checking a device index would need a "
+                                 "host sync)")
+        if sample_idx.dtype == torch.bool or sample_idx.is_floating_point() or sample_idx.is_complex():
+            raise _lib.B200Error(f"{what} must hold integers, got {sample_idx.dtype}")
+        if sample_idx.dim() != 1:
+            raise _lib.B200Error(f"{what} must be 1-D, got shape {tuple(sample_idx.shape)}")
+        vals = sample_idx.tolist()
+    elif isinstance(sample_idx, collections.abc.Sequence) and not isinstance(sample_idx, (str, bytes)):
+        vals = list(sample_idx)
+        bad = [v for v in vals if isinstance(v, bool) or not isinstance(v, numbers.Integral)]
+        if bad:
+            raise _lib.B200Error(f"{what} must be a 1-D sequence of integers, got {bad[0]!r}")
+        vals = [int(v) for v in vals]
+    else:
+        raise _lib.B200Error(f"{what} must be a Python sequence or a CPU integer tensor, got {type(sample_idx).__name__}")
+    if not vals:
+        raise _lib.B200Error(f"{what} is empty")
+    out_of_range = [v for v in vals if not -S <= v < S]
+    if out_of_range:
+        raise _lib.B200Error(f"{what}: position {out_of_range[0]} is outside [-{S}, {S})")
+    vals = [v + S if v < 0 else v for v in vals]
+    if len(set(vals)) != len(vals):
+        raise _lib.B200Error(f"{what} selects an event more than once (after counting negatives from the end)")
+    return vals
+
+
+def _sample_maps(positions: list, B: int, S: int, device):
+    """Row map rows[b*K + j] = b*S + positions[j] (the row order of hidden[:, idx].reshape(-1, H)) and its inverse over the
+    B*S event rows (-1 = not selected), as int32 device tensors; the copies are queued without a host sync."""
+    idx = torch.tensor(positions, dtype=torch.int32)
+    rows = (torch.arange(B, dtype=torch.int32)[:, None] * S + idx[None, :]).reshape(-1)
+    inv = torch.full((B * S,), -1, dtype=torch.int32)
+    inv[rows.long()] = torch.arange(rows.numel(), dtype=torch.int32)
+    if device.type == "cuda":
+        return rows.pin_memory().to(device, non_blocking=True), inv.pin_memory().to(device, non_blocking=True)
+    return rows, inv
 
 
 def _loop_mode(mode: str):
@@ -757,38 +815,47 @@ class MIDIModel(PreTrainedModel):
         return seq[:, :cur_len].cpu().numpy()
 
     # ------------------------------------------------------------------ fused training path (non-reference API)
-    def training_loss(self, batch: torch.Tensor, backward: bool = True, accumulate: bool = False, grad_ready=None):
-        """train.py:168-185 (sample_seq=False) fused: x = batch[:, :-1], y = batch[:, 1:], both stacks, lm_head,
+    def training_loss(self, batch: torch.Tensor, backward: bool = True, accumulate: bool = False, grad_ready=None,
+                      sample_idx=None):
+        """train.py:168-185 fused: x = batch[:, :-1], y = batch[:, 1:], both stacks, lm_head,
         mean CE with ignore_index=pad -- and, if `backward`, every gradient written to the flat gradient buffer
         (`.grad` of each parameter is a view of it).  Returns a 0-dim fp32 tensor (no host sync).
         `grad_ready(start, end)` (optional) is called as soon as a slice of the flat gradient buffer is final --
         first the token-level stack + lm_head, then the event-level stack -- so a data-parallel trainer can start
-        the all-reduce of the first slice while the second is still being computed (midi_b200/ddp.py)."""
+        the all-reduce of the first slice while the second is still being computed (midi_b200/ddp.py).
+        `sample_idx` (train.py --sample-seq, train.py:172-175): event positions (a Python sequence or a CPU integer
+        tensor, distinct, in [-S, S)) kept in every sequence, in the given order; the token-level stack, lm_head and the
+        loss then run on those B * len(sample_idx) events only.  None (the default) runs every event."""
         rt = self._rt()
         tok = self.tokenizer
         B, S1, T = batch.shape
         S = S1 - 1
-        if batch.dtype == torch.int16:
-            x, y = _ops.batch_to_xy(batch.contiguous())        # int16 host data path (midi_b200/data.py): one widening pass
-        else:
-            batch = batch.to(torch.long)
-            x = batch[:, :-1].contiguous().view(B * S, T)
-            y = batch[:, 1:].contiguous().view(B * S, T)
+        maps = None
+        if sample_idx is not None:
+            maps = _sample_maps(_sample_positions(sample_idx, S), B, S, rt.store.device)
+        x, y = _batch_xy(batch)
         e = _ops.embed_sum(x, rt.outer.embed)
         hidden, sv_o = rt.outer.forward(e, B, S, self.net.rotary_emb.inv_freq, save=backward)
-        ids_in = y[:, :-1].contiguous()
-        xin = _ops.inner_input(hidden, ids_in, rt.inner.embed)
-        hs, sv_i = rt.inner.forward(xin, B * S, T, self.net_token.rotary_emb.inv_freq, save=backward)
+        if maps is None:
+            N = B * S
+            ids_in = y[:, :-1].contiguous()
+            xin = _ops.inner_input(hidden, ids_in, rt.inner.embed)
+            targets = y.reshape(-1)
+        else:
+            N = maps[0].shape[0]
+            xin, y_sel = _ops.inner_input_rows(hidden, y, maps[0], rt.inner.embed)
+            ids_in = y_sel[:, :-1].contiguous()
+            targets = y_sel.view(-1)
+        hs, sv_i = rt.inner.forward(xin, N, T, self.net_token.rotary_emb.inv_freq, save=backward)
         del xin
         logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)
-        targets = y.reshape(-1)
         lac, lse = _ops.ce_fwd(logits, targets, rt.V, tok.pad_id)
         loss = lac[0]
         if backward:
             _ops.ce_bwd_(logits, targets, lse, lac, rt.V, tok.pad_id, 1.0)
             g_i, g_o = rt.inner.main_grads, rt.outer.main_grads
-            dhidden, = _inner_backward(rt, self, sv_i, hs, logits, ids_in, B * S, T, T - 1, True, g_i, rt.g_lm_head,
-                                       accumulate)
+            dhidden, = _inner_backward(rt, self, sv_i, hs, logits, ids_in, N, T, T - 1, True, g_i, rt.g_lm_head,
+                                       accumulate, hidden_rows=None if maps is None else maps[1])
             del logits, hs
             # Gradient hand-over to a data-parallel trainer.  Base parameters that train (full training): slices of the flat
             # buffer as backward finishes them.  Adapter matrices (LoRA, train.py:439-449) sit in the tail
@@ -819,6 +886,28 @@ class MIDIModel(PreTrainedModel):
                 grad_ready(rt.store.base_numel, rt.store.numel)
             rt.store.publish_grads()
         return loss
+
+    def validation_metrics(self, batch: torch.Tensor):
+        """train.py:190-206 (validation_step) fused: (val/loss, val/acc) as two 0-dim fp32 device tensors, no host sync.
+        The forward saves no activations and the gradient buffer is not touched.  The loss is the mean CE over the
+        non-pad targets (what training_loss(batch, backward=False) returns); the accuracy is the share of those targets
+        that are the argmax of their logits row (train.py:153-166).  Both are NaN when no target is a non-pad token."""
+        rt = self._rt()
+        tok = self.tokenizer
+        B, S1, T = batch.shape
+        S = S1 - 1
+        x, y = _batch_xy(batch)
+        e = _ops.embed_sum(x, rt.outer.embed)
+        hidden, _ = rt.outer.forward(e, B, S, self.net.rotary_emb.inv_freq, save=False)
+        xin = _ops.inner_input(hidden, y[:, :-1].contiguous(), rt.inner.embed)
+        hs, _ = rt.inner.forward(xin, B * S, T, self.net_token.rotary_emb.inv_freq, save=False)
+        del xin, hidden
+        logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)
+        targets = y.reshape(-1)
+        lac, _ = _ops.ce_fwd(logits, targets, rt.V, tok.pad_id)
+        hits = _ops.argmax_hits(logits, targets, rt.V, tok.pad_id)
+        loss = torch.where(lac[1] > 0, lac[0], float("nan"))
+        return loss, hits[0] / hits[1]
 
     def _opt_state(self, rt):
         """AdamW moments (fp32) over the trainable span of the flat parameter buffer -- everything in full training, the
