@@ -207,7 +207,6 @@ int b200_sample_from_logits(const void* logits, int rows, int V, int ld, float t
                             int out_stride, cudaStream_t s);
 /* state_dev = {call counter (incremented), device-side seed}: u[i] = hash(seed ^ state[1], state[0], i) */
 int b200_uniform_fill(float* u, int n, unsigned long long seed, unsigned long long* state_dev, cudaStream_t s);
-int b200_add_int(int* p, int v, cudaStream_t s);
 /* graph-captured generate loop: commit the event sampled into ev_t [T][B] to seq[:, *pos+1] and ev_next; (*pos)++ */
 int b200_event_commit(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T, int max_len,
                       cudaStream_t s);

@@ -16,6 +16,9 @@ namespace {
 // ---------------------------------------------------------------------------------------------
 constexpr int GV_WARPS = 8;
 
+// Plain skinny GEMM (b200_gemv_bf16).  gemv_fused_kernel without its options gives the same bits, but it stages x one
+// warp per row and holds 70-80 registers: through it, 1-3 rows and the vocabulary projection ran up to 1.5x slower
+// (profiles/h100_decode_ab.txt), so both kernels stay.
 template <int B>
 __global__ void __launch_bounds__(GV_WARPS * 32)
 gemv_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, const bf16* __restrict__ res, bf16* __restrict__ y,
@@ -211,43 +214,56 @@ __global__ void kv_append_kernel(const bf16* __restrict__ qkv, KVLayout L, int s
     }
 }
 
-// single-query attention over the cache.  Row r = b * s_q + i attends to keys 0 .. past + i.
-// grid (rows * n_heads, n_split); partial: [rows*n_heads][n_split][D + 2] = (m, l, o[D])
+// K / V rows of one (batch row, head) in the cache; K is read through the non-coherent, L1-bypassing path
+struct CacheRows {
+    KVLayout L;
+    int b, h;
+    __device__ __forceinline__ const bf16* key(int t) const { return L.k_pool + kv_off(L, b, h, t); }
+    __device__ __forceinline__ const bf16* value(int t) const { return L.v_pool + kv_off(L, b, h, t); }
+    __device__ __forceinline__ void unpack_key8(const bf16* p, float* f) const { unpack8(ld_nc16(p), f); }
+};
+// the same, except that position `pos` comes from shared memory (the kernel appends it to the cache itself), so K is
+// read with generic loads
+struct CacheRowsWithNew {
+    CacheRows cache;
+    const bf16* s_k;
+    const bf16* s_v;
+    int pos;
+    __device__ __forceinline__ const bf16* key(int t) const { return t == pos ? s_k : cache.key(t); }
+    __device__ __forceinline__ const bf16* value(int t) const { return t == pos ? s_v : cache.value(t); }
+    __device__ __forceinline__ void unpack_key8(const bf16* p, float* f) const {
+        unpack8(*reinterpret_cast<const uint4*>(p), f);
+    }
+};
+
+// partial record of a split with no keys: it drops out of the combine pass
 template <int D>
-__global__ void __launch_bounds__(128)
-decode_attn_kernel(const bf16* __restrict__ q, KVLayout L, float* __restrict__ partial, int s_q, int past,
-                   const int* past_dev, int ldq, float scale, int n_split) {
+__device__ __forceinline__ void write_empty_partial(float* pout) {
+    if (threadIdx.x == 0) { pout[0] = -INFINITY; pout[1] = 0.f; }
+    for (int d = threadIdx.x; d < D; d += blockDim.x) pout[2 + d] = 0.f;
+}
+
+// Single-query attention of q (in shared memory) over keys [t0, t1), t0 < t1, by one 128-thread CTA.  Writes the partial
+// record pout = (m, l, o[D]) for the combine pass or, when `direct` (the chunk is the whole context), the normalised
+// output row out_row()[0..D).  out_row is called only then: an output address formed up front would hold registers
+// through the key loops and cut the loads ptxas keeps in flight there.
+template <int D, typename Rows, typename OutRow>
+__device__ __forceinline__ void attend_chunk(const bf16* s_q, const Rows& rows, int t0, int t1, float scale, float* pout,
+                                             bool direct, OutRow out_row) {
     constexpr int CHUNK_MAX = 1024;
     __shared__ float s_sc[CHUNK_MAX];
-    __shared__ __align__(16) bf16 s_q_sh[D];
     __shared__ float s_red[8];
     __shared__ float s_out[2][D];
-    const int rh = blockIdx.x;
-    const int r = rh / L.n_heads, h = rh % L.n_heads;
-    const int b = r / s_q, i = r % s_q;
-    const int T = (past_dev ? *past_dev : past) + i + 1;
-    const int chunk = (T + n_split - 1) / n_split;
-    const int t0 = blockIdx.y * chunk;
-    const int t1 = min(T, t0 + chunk);
-    float* pout = partial + ((size_t)rh * n_split + blockIdx.y) * (D + 2);
-    if (t0 >= t1) {
-        if (threadIdx.x == 0) { pout[0] = -INFINITY; pout[1] = 0.f; }
-        for (int d = threadIdx.x; d < D; d += blockDim.x) pout[2 + d] = 0.f;
-        return;
-    }
-    for (int d = threadIdx.x; d < D / 8; d += blockDim.x)
-        *reinterpret_cast<uint4*>(s_q_sh + d * 8) = *reinterpret_cast<const uint4*>(q + (size_t)r * ldq + h * D + d * 8);
-    __syncthreads();
     // scores: one thread per key
     float mx = -INFINITY;
     for (int t = t0 + threadIdx.x; t < t1; t += blockDim.x) {
-        const bf16* kp = L.k_pool + kv_off(L, b, h, t);
+        const bf16* kp = rows.key(t);
         float s = 0.f;
 #pragma unroll
         for (int d = 0; d < D / 8; d++) {
             float kf[8], qf[8];
-            unpack8(ld_nc16(kp + d * 8), kf);
-            unpack8(*reinterpret_cast<const uint4*>(s_q_sh + d * 8), qf);
+            rows.unpack_key8(kp + d * 8, kf);
+            unpack8(*reinterpret_cast<const uint4*>(s_q + d * 8), qf);
 #pragma unroll
             for (int j = 0; j < 8; j++) s = fmaf(kf[j], qf[j], s);
         }
@@ -279,7 +295,7 @@ decode_attn_kernel(const bf16* __restrict__ q, KVLayout L, float* __restrict__ p
 #pragma unroll
     for (int j = 0; j < DPT; j++) acc[j] = 0.f;
     for (int t = t0 + grp; t < t1; t += GROUPS) {
-        const bf16* vp = L.v_pool + kv_off(L, b, h, t);
+        const bf16* vp = rows.value(t);
         const float p = s_sc[t - t0];
 #pragma unroll
         for (int j = 0; j < DPT; j++) acc[j] = fmaf(p, __bfloat162float(vp[d0 + j]), acc[j]);
@@ -287,12 +303,46 @@ decode_attn_kernel(const bf16* __restrict__ q, KVLayout L, float* __restrict__ p
     if (GROUPS == 2) {
         s_out[grp][d0] = acc[0];
         __syncthreads();
-        if (grp == 0) pout[2 + d0] = s_out[0][d0] + s_out[1][d0];
-    } else {
-#pragma unroll
-        for (int j = 0; j < DPT; j++) pout[2 + d0 + j] = acc[j];
+        acc[0] = s_out[0][d0] + s_out[1][d0];
     }
-    if (threadIdx.x == 0) { pout[0] = mx; pout[1] = sum; }
+    if (direct) {
+        bf16* out = out_row();
+        if (grp == 0) {
+#pragma unroll
+            for (int j = 0; j < DPT; j++) out[d0 + j] = __float2bfloat16_rn(acc[j] / sum);
+        }
+    } else {
+        if (grp == 0) {
+#pragma unroll
+            for (int j = 0; j < DPT; j++) pout[2 + d0 + j] = acc[j];
+        }
+        if (threadIdx.x == 0) { pout[0] = mx; pout[1] = sum; }
+    }
+}
+
+// single-query attention over the cache.  Row r = b * s_q + i attends to keys 0 .. past + i.
+// grid (rows * n_heads, n_split); partial: [rows*n_heads][n_split][D + 2] = (m, l, o[D])
+template <int D>
+__global__ void __launch_bounds__(128)
+decode_attn_kernel(const bf16* __restrict__ q, KVLayout L, float* __restrict__ partial, int s_q, int past,
+                   const int* past_dev, int ldq, float scale, int n_split) {
+    __shared__ __align__(16) bf16 s_q_sh[D];
+    const int rh = blockIdx.x;
+    const int r = rh / L.n_heads, h = rh % L.n_heads;
+    const int b = r / s_q, i = r % s_q;
+    const int T = (past_dev ? *past_dev : past) + i + 1;
+    const int chunk = (T + n_split - 1) / n_split;
+    const int t0 = blockIdx.y * chunk;
+    const int t1 = min(T, t0 + chunk);
+    float* pout = partial + ((size_t)rh * n_split + blockIdx.y) * (D + 2);
+    if (t0 >= t1) {
+        write_empty_partial<D>(pout);
+        return;
+    }
+    for (int d = threadIdx.x; d < D / 8; d += blockDim.x)
+        *reinterpret_cast<uint4*>(s_q_sh + d * 8) = *reinterpret_cast<const uint4*>(q + (size_t)r * ldq + h * D + d * 8);
+    __syncthreads();
+    attend_chunk<D>(s_q_sh, CacheRows{L, b, h}, t0, t1, scale, pout, false, [] { return (bf16*)nullptr; });
 }
 
 // Fused single-token attention step: RoPE on the new q and k (hf :146-168, same three roundings as rope_kernel), append
@@ -303,13 +353,9 @@ __global__ void __launch_bounds__(128)
 decode_attn_fused_kernel(const bf16* __restrict__ qkv, KVLayout L, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
                          float* __restrict__ partial, bf16* __restrict__ out, int pos0, const int* pos_dev, int ldq, int ldo,
                          float scale, int n_split) {
-    constexpr int CHUNK_MAX = 1024;
-    __shared__ float s_sc[CHUNK_MAX];
     __shared__ __align__(16) bf16 s_q[D];
     __shared__ __align__(16) bf16 s_k[D];
     __shared__ __align__(16) bf16 s_v[D];
-    __shared__ float s_red[8];
-    __shared__ float s_out[2][D];
     const int rh = blockIdx.x;
     const int b = rh / L.n_heads, h = rh % L.n_heads;
     const int pos = (pos_dev ? *pos_dev : 0) + pos0;     // position of the new token
@@ -346,71 +392,12 @@ decode_attn_fused_kernel(const bf16* __restrict__ qkv, KVLayout L, const bf16* _
     }
     float* pout = partial + ((size_t)rh * n_split + blockIdx.y) * (D + 2);
     if (t0 >= t1) {
-        if (threadIdx.x == 0) { pout[0] = -INFINITY; pout[1] = 0.f; }
-        for (int d = threadIdx.x; d < D; d += blockDim.x) pout[2 + d] = 0.f;
+        write_empty_partial<D>(pout);
         return;
     }
-    float mx = -INFINITY;
-    for (int t = t0 + threadIdx.x; t < t1; t += blockDim.x) {
-        const bf16* kp = (t == pos) ? s_k : L.k_pool + kv_off(L, b, h, t);
-        float s = 0.f;
-#pragma unroll
-        for (int d = 0; d < D / 8; d++) {
-            float kf[8], qf[8];
-            unpack8(*reinterpret_cast<const uint4*>(kp + d * 8), kf);
-            unpack8(*reinterpret_cast<const uint4*>(s_q + d * 8), qf);
-#pragma unroll
-            for (int j = 0; j < 8; j++) s = fmaf(kf[j], qf[j], s);
-        }
-        s *= scale;
-        s_sc[t - t0] = s;
-        mx = fmaxf(mx, s);
-    }
-    mx = warp_max(mx);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = mx;
-    __syncthreads();
-    mx = fmaxf(fmaxf(s_red[0], s_red[1]), fmaxf(s_red[2], s_red[3]));
-    float sum = 0.f;
-    for (int t = t0 + threadIdx.x; t < t1; t += blockDim.x) {
-        const float p = __expf(s_sc[t - t0] - mx);
-        sum += p;
-        s_sc[t - t0] = bf16_round(p);
-    }
-    sum = warp_sum(sum);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) s_red[4 + (threadIdx.x >> 5)] = sum;
-    __syncthreads();
-    sum = s_red[4] + s_red[5] + s_red[6] + s_red[7];
-    constexpr int GROUPS = (D >= 128) ? 1 : 128 / D;
-    constexpr int DPT = (D >= 128) ? D / 128 : 1;
-    const int grp = (D >= 128) ? 0 : threadIdx.x / D;
-    const int d0 = (D >= 128) ? threadIdx.x * DPT : threadIdx.x % D;
-    float acc[DPT];
-#pragma unroll
-    for (int j = 0; j < DPT; j++) acc[j] = 0.f;
-    for (int t = t0 + grp; t < t1; t += GROUPS) {
-        const bf16* vp = (t == pos) ? s_v : L.v_pool + kv_off(L, b, h, t);
-        const float p = s_sc[t - t0];
-#pragma unroll
-        for (int j = 0; j < DPT; j++) acc[j] = fmaf(p, __bfloat162float(vp[d0 + j]), acc[j]);
-    }
-    if (GROUPS == 2) {
-        s_out[grp][d0] = acc[0];
-        __syncthreads();
-        acc[0] = s_out[0][d0] + s_out[1][d0];
-    }
-    if (n_split == 1) {        // whole context in this CTA: normalise and write the attention output directly
-        if (grp == 0) {
-#pragma unroll
-            for (int j = 0; j < DPT; j++) out[(size_t)b * ldo + h * D + d0 + j] = __float2bfloat16_rn(acc[j] / sum);
-        }
-    } else {
-        if (grp == 0) {
-#pragma unroll
-            for (int j = 0; j < DPT; j++) pout[2 + d0 + j] = acc[j];
-        }
-        if (threadIdx.x == 0) { pout[0] = mx; pout[1] = sum; }
-    }
+    // n_split == 1: the whole context is in this CTA, which normalises and writes the attention output directly
+    attend_chunk<D>(s_q, CacheRowsWithNew{{L, b, h}, s_k, s_v, pos}, t0, t1, scale, pout, n_split == 1,
+                    [&] { return out + (size_t)b * ldo + h * D; });
 }
 
 // Token-level stack variant (context <= 32 positions): one WARP per (batch row, head); each lane owns D/32 consecutive
@@ -582,8 +569,6 @@ __global__ void philox_uniform_kernel(float* __restrict__ u, int n, unsigned lon
     __syncthreads();
     if (i == 0) *counter = c + 1;
 }
-
-__global__ void add_int_kernel(int* p, int v) { *p += v; }
 
 // End of one generated event (graph-captured loop): ev_t [T][B] (token-major scratch written by the sampler)
 // -> seq[b, *pos + 1, :] and ev_next[b, :] (input of the next outer step); then (*pos)++.
@@ -815,11 +800,5 @@ extern "C" int b200_event_commit(const long long* ev_t, long long* seq, long lon
                                  int max_len, cudaStream_t stream) {
     event_commit_kernel<<<1, 256, 0, stream>>>(ev_t, seq, ev_next, pos_dev, B, T, max_len);
     B200_CHECK_LAUNCH("event_commit");
-    return B200_OK;
-}
-
-extern "C" int b200_add_int(int* p, int v, cudaStream_t stream) {
-    add_int_kernel<<<1, 1, 0, stream>>>(p, v);
-    B200_CHECK_LAUNCH("add_int");
     return B200_OK;
 }

@@ -62,27 +62,23 @@ class PagedKV:
             self.batch, self.max_pages).contiguous()
 
 
-def _linear(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """nn.Linear on a few rows: weight-streaming skinny GEMM for <= 16 rows, tensor-core GEMM otherwise."""
+def _linear(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None,
+            pitch: Optional[int] = None) -> torch.Tensor:
+    """nn.Linear on a few rows: weight-streaming skinny GEMM for <= 16 rows, tensor-core GEMM otherwise.  `pitch`: row
+    pitch of the output when N is not a multiple of 8 (lm_head, V = 3406 -> 3408)."""
     M, K = x.shape
     N = w.shape[0]
     if M > 16:
-        return ops.linear(x, w, residual=residual)
-    y = torch.empty((M, N), dtype=BF16, device=x.device)
+        return ops.linear(x, w, residual=residual, pitch=pitch)
+    y = torch.empty((M, pitch or N), dtype=BF16, device=x.device)
     lib.call("b200_gemv_bf16", x.data_ptr(), w.data_ptr(), lib.ptr(residual), y.data_ptr(), M, N, K, x.stride(0),
-             w.stride(0), residual.stride(0) if residual is not None else 0, N, lib.stream())
+             w.stride(0), residual.stride(0) if residual is not None else 0, y.stride(0), lib.stream())
     return y
 
 
 def _lm_head(x: torch.Tensor, w: torch.Tensor, pitch: int) -> torch.Tensor:
-    M, K = x.shape
-    N = w.shape[0]
-    if M > 16:
-        return ops.linear(x, w, pitch=pitch)
-    y = torch.empty((M, pitch), dtype=BF16, device=x.device)
-    lib.call("b200_gemv_bf16", x.data_ptr(), w.data_ptr(), None, y.data_ptr(), M, N, K, x.stride(0), w.stride(0), 0, pitch,
-             lib.stream())
-    return y
+    """Logits projection into rows of `pitch` columns (kept for existing callers; same code path as _linear)."""
+    return _linear(x, w, pitch=pitch)
 
 
 def _gemv_fused(x, w, n_out, *, ids=None, table=None, norm_w=None, eps=0.0, residual=None, swiglu=False, ldy=None):
@@ -147,27 +143,23 @@ class CachedStack:
             return self._step_fused(x, kv, past, pos_dev, T, n_split, ws_bytes, final_norm)
         if not final_norm:
             raise lib.B200Error("final_norm=False is only available on the fused single-token path")
+        prefill = not dev_pos and past == 0 and s_new > 1        # prompt into an empty cache: causal attention kernels
         for li, w in enumerate(self.eng.layers):
             n1 = ops.rmsnorm(x, w.ln1, c.eps)
             qkv = _linear(n1, w.qkv)
             ops.rope_qk_(qkv, self.cos, self.sin, s_new, H, D, pos0=past, pos0_dev=pos_dev)
             lib.call("b200_kv_append", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(), kv.block_table.data_ptr(),
                      kv.max_pages, kv.page, nh, D, B, s_new, past, pd, qkv.stride(0), lib.stream())
-            if dev_pos:
-                attn = torch.empty((B * s_new, H), dtype=BF16, device=x.device)
-                ws = ops._ws("attn_decode", ws_bytes, x.device)
-                lib.call("b200_attn_decode", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
-                         kv.block_table.data_ptr(), kv.max_pages, kv.page, attn.data_ptr(), B, s_new, nh, D, 0, pd, T,
-                         qkv.stride(0), H, scale, n_split, ws.data_ptr(), ws.numel(), lib.stream())
-            elif past == 0 and s_new > 1 and D == 64:
+            if prefill and D == 64:
                 attn, _ = ops.attn_causal_fwd(qkv, B, s_new, nh, D, want_lse=False)
-            elif past == 0 and s_new > 1 and D == 256 and s_new <= 8:
+            elif prefill and D == 256 and s_new <= 8:
                 attn = ops.attn_tiny_fwd(qkv, B, s_new, nh, D)
             else:
+                # the cached length is `past` (host) or *pos_dev (graph replay, past = 0)
                 attn = torch.empty((B * s_new, H), dtype=BF16, device=x.device)
                 ws = ops._ws("attn_decode", ws_bytes, x.device)
                 lib.call("b200_attn_decode", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
-                         kv.block_table.data_ptr(), kv.max_pages, kv.page, attn.data_ptr(), B, s_new, nh, D, past, None, T,
+                         kv.block_table.data_ptr(), kv.max_pages, kv.page, attn.data_ptr(), B, s_new, nh, D, past, pd, T,
                          qkv.stride(0), H, scale, n_split, ws.data_ptr(), ws.numel(), lib.stream())
             h = _linear(attn, w.o, residual=x)
             n2 = ops.rmsnorm(h, w.ln2, c.eps)
@@ -348,7 +340,7 @@ class GraphGenerator:
                                      ldy=self.pitch)
             else:
                 hs = self.inner.step(xin, self.kv2, 1)
-                logits = _lm_head(hs, self.lm_head, self.pitch)
+                logits = _linear(hs, self.lm_head, pitch=self.pitch)
             lib.call("b200_uniform_fill", self.u.data_ptr(), B, 0, self.counter.data_ptr(), lib.stream())
             lib.call("b200_sample_from_logits", logits.data_ptr(), B, self.V, logits.stride(0), self.temp, self.top_p,
                      self.top_k, i, self.ev_t.data_ptr(), self.g.lut.data_ptr(), self.g.n_event_types, self.g.eos, self.g.pad,

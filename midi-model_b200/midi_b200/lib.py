@@ -69,7 +69,6 @@ SIGNATURES = {
     "b200_sample_topp_topk": (i32, [vp, i32, i32, i32, i32, f32, i32, vp, vp, vp]),
     "b200_sample_from_logits": (i32, [vp, i32, i32, i32, f32, f32, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, i32, vp]),
     "b200_uniform_fill": (i32, [vp, i32, u64, vp, vp]),
-    "b200_add_int": (i32, [vp, i32, vp]),
     "b200_event_commit": (i32, [vp, vp, vp, vp, i32, i32, i32, vp]),
     "b200_decode_desc_bytes": (sz, []),
     "b200_decode_events_workspace_bytes": (sz, [vp]),

@@ -612,7 +612,7 @@ class MIDIModel(PreTrainedModel):
         xin = _ops.inner_input(hid, ids, rt.inner.embed)
         L = xin.shape[0] // N
         hs = self._cached_stack("inner").step(xin, kv, L)
-        logits = _dec._lm_head(hs, rt.lm_head, rt.pitch)
+        logits = _dec._linear(hs, rt.lm_head, pitch=rt.pitch)
         return logits.view(N, L, rt.pitch)[:, :, :rt.V]
 
     def forward(self, x, cache=None):
@@ -790,7 +790,7 @@ class MIDIModel(PreTrainedModel):
                     else:
                         xin = _ops.inner_input(None, evb[:, i - 1:i].contiguous(), rt.inner.embed)
                     hs = inner.step(xin, kv2, 1)
-                    logits = _dec._lm_head(hs, rt.lm_head, rt.pitch)
+                    logits = _dec._linear(hs, rt.lm_head, pitch=rt.pitch)
                     u = torch.rand(batch_size, generator=generator, device=gen_dev, dtype=torch.float32).to(dev)
                     _dec.sample_from_logits(logits, rt.V, float(temp), float(top_p), int(top_k), i, evt0, g, u, evb)
                     if i == 0:
