@@ -6,7 +6,8 @@ that order, the fused `[3H, H]` QKV and `[2I, H]` gate|up weights are *views* --
 `state_dict` keys stay the source of truth and no packed
 copies exist.  One flat gradient buffer means one all-reduce and one AdamW launch per step.
 
-`StackEngine` runs forward (saving exactly what backward needs) and an explicit backward; there
+`StackEngine` runs forward (saving exactly what backward needs, or with `checkpoint` only each layer's input and
+attention output, the rest recomputed in backward) and an explicit backward; there
 is no autograd graph inside -- `autograd.Function`s in midi_model.py wrap whole stacks.
 Math per layer: hf modeling_llama.py:303-332; rounding points: DESIGN.md 3.3.
 """
@@ -380,15 +381,61 @@ class StackEngine:
                  residual=dx)
 
     # ------------------------------------------------------------------ forward
-    def forward(self, x: torch.Tensor, n_seq: int, S: int, inv_freq: torch.Tensor, save: bool):
-        """x: [n_seq * S, H] inputs_embeds (row-major, sequences contiguous) -> (final-normed hidden, saved)."""
+    # The layer body is split around the attention so that the forward and the backward's recompute of a checkpointed
+    # layer (_recompute) issue the same kernels in the same order on the same operands: every forward kernel is
+    # deterministic and the GEMM plan is a function of the shape, so the recomputed tensors equal the forward's bit for bit.
+    def _qkv(self, w: LayerW, n1: torch.Tensor, cos, sin, S: int, lsv: dict, rotate: bool) -> torch.Tensor:
+        """Packed QKV projection of n1, the q/k/v adapters added BEFORE the rotation, and RoPE on the q and k thirds.
+        rotate=False leaves the rotation to the token-level attention kernel (fused RoPE, the forward's default there);
+        the stand-alone RoPE kernel performs the same three roundings (csrc/attn_tiny.cu rope_fwd_lane, csrc/elementwise.cu
+        rope_kernel), so a recompute that does not run attention gets the rotated q, k the forward's kernel wrote back."""
+        H, D = self.cfg.hidden, self.cfg.head_dim
+        lo = w.lora
+        if FUSE_ROPE_FWD and not any(k in lo for k in ("q", "k", "v")):
+            return ops.linear_rope(n1, w.qkv, cos, sin, S, D)         # QKV GEMM with RoPE in the epilogue
+        qkv = ops.linear(n1, w.qkv)
+        for j, key in enumerate(("q", "k", "v")):
+            if key in lo:
+                lsv[key] = self._lora_fwd(lo[key], n1, qkv, j * H, H)
+        if rotate:
+            ops.rope_qk_(qkv, cos, sin, S, H, D)
+        return qkv
+
+    def _mlp_in(self, w: LayerW, x: torch.Tensor, attn: torch.Tensor, lsv: dict):
+        """From the layer input x and the attention output: o_proj (+ adapter), the residual add fused into the
+        post-attention norm, and the gate|up projection (+ adapters) with SwiGLU -> (h, n2, rstd2, gu, act)."""
         c = self.cfg
-        H, D, nh, I = c.hidden, c.head_dim, c.n_head, c.inner
+        H, I = c.hidden, c.inner
+        lo = w.lora
+        y1 = ops.linear(attn, w.o)
+        if "o" in lo:
+            lsv["o"] = self._lora_fwd(lo["o"], attn, y1, 0, H)
+        h, n2, rstd2 = ops.add_rmsnorm(x, y1, w.ln2, c.eps)
+        del y1
+        if FUSE_SWIGLU and I % 128 == 0 and "gate" not in lo and "up" not in lo:
+            gu, act = ops.linear_swiglu(n2, w.gu)
+        else:
+            gu = ops.linear(n2, w.gu)
+            if "gate" in lo:
+                lsv["gate"] = self._lora_fwd(lo["gate"], n2, gu, 0, I)
+            if "up" in lo:
+                lsv["up"] = self._lora_fwd(lo["up"], n2, gu, I, I)
+            act = ops.swiglu(gu)
+        return h, n2, rstd2, gu, act
+
+    def forward(self, x: torch.Tensor, n_seq: int, S: int, inv_freq: torch.Tensor, save: bool, checkpoint: bool = False):
+        """x: [n_seq * S, H] inputs_embeds (row-major, sequences contiguous) -> (final-normed hidden, saved).
+        checkpoint (with save): keep per layer only its input x, the attention output, the attention's log-sum-exp and
+        the down_proj adapter's scaled down-projection; backward recomputes the rest of the layer (_recompute)."""
+        c = self.cfg
+        H, D, nh = c.hidden, c.head_dim, c.n_head
         cos, sin = ops.rope_table(inv_freq, S)
         saved = [] if save else None
+        checkpoint = checkpoint and save
         # Residual adds are fused into the norm that follows them (x + y is formed, rounded to bf16 and written by
         # the norm kernel), so every GEMM keeps the plain store epilogue.
         pending = None                                   # output of the previous layer's down_proj, not yet added
+        fuse_tiny = self.tiny and FUSE_ROPE and not FUSE_ROPE_FWD     # token-level stack: RoPE inside the attention kernel
         for w in self.layers:
             lo = w.lora
             lsv = {}                                     # projection key -> scaled LoRA down-projection (backward operand)
@@ -396,44 +443,37 @@ class StackEngine:
                 n1, rstd1 = ops.rmsnorm(x, w.ln1, c.eps, want_rstd=True)
             else:
                 x, n1, rstd1 = ops.add_rmsnorm(x, pending, w.ln1, c.eps)
-            fuse_tiny = self.tiny and FUSE_ROPE and not FUSE_ROPE_FWD     # token-level stack: RoPE inside the attention kernel
-            qkv_lora = any(k in lo for k in ("q", "k", "v"))
-            if FUSE_ROPE_FWD and not qkv_lora:
-                qkv = ops.linear_rope(n1, w.qkv, cos, sin, S, D)      # QKV GEMM with RoPE in the epilogue
-            else:
-                qkv = ops.linear(n1, w.qkv)
-                for j, key in enumerate(("q", "k", "v")):              # adapters add to the projections BEFORE the rotation
-                    if key in lo:
-                        lsv[key] = self._lora_fwd(lo[key], n1, qkv, j * H, H)
-                if not fuse_tiny:
-                    ops.rope_qk_(qkv, cos, sin, S, H, D)
+            qkv = self._qkv(w, n1, cos, sin, S, lsv, rotate=not fuse_tiny)
             if self.tiny:
                 attn, lse = ops.attn_tiny_fwd(qkv, n_seq, S, nh, D, rope=(cos, sin) if fuse_tiny else None), None
             else:
                 attn, lse = ops.attn_causal_fwd(qkv, n_seq, S, nh, D, want_lse=save)
-            y1 = ops.linear(attn, w.o)
-            if "o" in lo:
-                lsv["o"] = self._lora_fwd(lo["o"], attn, y1, 0, H)
-            h, n2, rstd2 = ops.add_rmsnorm(x, y1, w.ln2, c.eps)
-            del y1
-            if FUSE_SWIGLU and I % 128 == 0 and "gate" not in lo and "up" not in lo:
-                gu, act = ops.linear_swiglu(n2, w.gu)
-            else:
-                gu = ops.linear(n2, w.gu)
-                if "gate" in lo:
-                    lsv["gate"] = self._lora_fwd(lo["gate"], n2, gu, 0, I)
-                if "up" in lo:
-                    lsv["up"] = self._lora_fwd(lo["up"], n2, gu, I, I)
-                act = ops.swiglu(gu)
+            h, n2, rstd2, gu, act = self._mlp_in(w, x, attn, lsv)
             pending = ops.linear(act, w.down)
             if "down" in lo:
                 lsv["down"] = self._lora_fwd(lo["down"], act, pending, 0, H)
-            if save:
+            if checkpoint:
+                # [rows, r]: kept rather than recomputed from act, so that the recompute never touches down_proj
+                saved.append((x, attn, lse, {"down": lsv["down"]} if "down" in lsv else {}))
+            elif save:
                 saved.append((x, n1, rstd1, qkv, attn, lse, h, n2, rstd2, gu, act, lsv))
             x = h
         x, y, rstd_f = ops.add_rmsnorm(x, pending, self.norm, c.eps)
-        sv = dict(layers=saved, x_last=x, rstd_f=rstd_f, n_seq=n_seq, S=S, cos=cos, sin=sin) if save else None
+        sv = dict(layers=saved, checkpoint=checkpoint, x_last=x, rstd_f=rstd_f, n_seq=n_seq, S=S, cos=cos,
+                  sin=sin) if save else None
         return y, sv
+
+    def _recompute(self, w: LayerW, kept, cos, sin, S: int):
+        """A checkpointed layer's saved set, in the layout forward() saves without checkpointing, from what it kept.
+        n1 comes from rmsnorm(x) where the forward formed it with add_rmsnorm(x_prev, down_out) (layer 0: rmsnorm too):
+        at every supported hidden size both run the same warp kernel, which sums the squares of the already-rounded bf16
+        residual in the same order.  Attention and down_proj are not re-run: attn and lse are kept, and this layer's
+        backward does not read the down_proj output."""
+        x, attn, lse, lsv = kept
+        n1, rstd1 = ops.rmsnorm(x, w.ln1, self.cfg.eps, want_rstd=True)
+        qkv = self._qkv(w, n1, cos, sin, S, lsv, rotate=True)
+        h, n2, rstd2, gu, act = self._mlp_in(w, x, attn, lsv)
+        return x, n1, rstd1, qkv, attn, lse, h, n2, rstd2, gu, act, lsv
 
     # ------------------------------------------------------------------ backward
     def layer_range(self, li: int):
@@ -464,8 +504,22 @@ class StackEngine:
             g = grads.layers[li]
             lo = w.lora
             hold = []
-            x, n1, rstd1, qkv, attn, lse, h, n2, rstd2, gu, act, lsv = sv["layers"][li]
+            ent = sv["layers"][li]
             sv["layers"][li] = None   # free as we go
+            if sv["checkpoint"]:
+                # The recomputed n1, n2 and act are wgrad operands on the side stream: _wgrad puts them in `hold`.  The
+                # previous layer's holds are released before the recompute allocates, once the main stream has waited for
+                # that layer's last wgrad (a short wait: the recompute's GEMMs would share the SMs with it anyway), so the
+                # allocator can hand their blocks to this layer and one recomputed set is alive at a time.  Released one
+                # layer late as below, the held set and the new one would both be alive: 0.52x instead of 0.40x of the
+                # default step's activation memory (tv2o-medium, B = 4 x 2048, H100), at the same step time.
+                while pending:
+                    old_ev, old_hold = pending.pop(0)
+                    torch.cuda.current_stream().wait_event(old_ev)
+                    old_hold.clear()
+                ent = self._recompute(w, ent, cos, sin, S)
+            x, n1, rstd1, qkv, attn, lse, h, n2, rstd2, gu, act, lsv = ent
+            del ent
             # ---- MLP block: x_out = h + down(act)
             dact = ops.linear_dgrad(dx, w.down)
             if g.down is not None:

@@ -146,10 +146,30 @@ class _Runtime:
         # then returns it.  `pool_lock` only guards the free list.
         self.gen_pool = {}                      # key -> [idle GraphGenerator]
         self.pool_lock = threading.Lock()
+        # activation checkpointing (MIDIModel.gradient_checkpointing_enable); the containers' flag outlives a rebuild
+        self.checkpoint = bool(model.net.gradient_checkpointing)
 
     def lora_version(self):
         """Changes whenever an adapter matrix was updated (torch optimizers bump _version; the fused AdamW bumps lora_step)."""
         return (self.lora_step, sum(p._version for p in self.lora_params))
+
+    def param_version(self):
+        """Changes whenever any parameter was modified in place: through torch (each parameter has its own version
+        counter, separate from the flat buffer's) or by the fused AdamW's raw-pointer update (lora_step)."""
+        return (self.lora_step, self.store.flat._version, sum(p._version for p in self.store._params.values()))
+
+
+def _checkpoint_guard(rt, sv):
+    """At a checkpointed drop-in forward: what _check_checkpoint_guard compares against in backward (None otherwise)."""
+    return (rt, rt.param_version()) if sv is not None and sv["checkpoint"] else None
+
+
+def _check_checkpoint_guard(guard, rt) -> None:
+    """The drop-in path's backward recomputes checkpointed layers from the CURRENT weights: refuse if they are not the
+    weights the forward ran with, which would silently give wrong gradients."""
+    if guard is not None and (guard[0] is not rt or guard[1] != rt.param_version()):
+        raise _lib.B200Error("backward of a checkpointed forward: the parameters were modified in place (or re-created) "
+                             "after the forward; recomputing its layers from the new weights would give wrong gradients")
 
 
 def _flat_ids(x: torch.Tensor) -> torch.Tensor:
@@ -167,14 +187,16 @@ class _OuterFn(torch.autograd.Function):
         ids = _flat_ids(x_ids).view(B * S, T)
         need = any(ctx.needs_input_grad)   # (grad mode is off inside Function.forward; this is the reliable signal)
         e = _ops.embed_sum(ids, rt.outer.embed)
-        y, sv = rt.outer.forward(e, B, S, model.net.rotary_emb.inv_freq, save=need)
+        y, sv = rt.outer.forward(e, B, S, model.net.rotary_emb.inv_freq, save=need, checkpoint=rt.checkpoint)
         ctx.model, ctx.sv, ctx.ids, ctx.shape = model, sv, ids, (B, S, T)
+        ctx.guard = _checkpoint_guard(rt, sv)
         return y.view(B, S, -1)
 
     @staticmethod
     def backward(ctx, dy):
         model = ctx.model
         rt = model._rt()
+        _check_checkpoint_guard(ctx.guard, rt)
         B, S, T = ctx.shape
         g = rt.outer.fresh_grads()
         dy2 = dy.reshape(B * S, -1).to(torch.bfloat16).contiguous()
@@ -199,16 +221,18 @@ class _InnerFn(torch.autograd.Function):
         need = any(ctx.needs_input_grad)
         hid = hidden.to(torch.bfloat16).contiguous() if hidden is not None else None
         xin = _ops.inner_input(hid, ids, rt.inner.embed)
-        hs, sv = rt.inner.forward(xin, N, L, model.net_token.rotary_emb.inv_freq, save=need)
+        hs, sv = rt.inner.forward(xin, N, L, model.net_token.rotary_emb.inv_freq, save=need, checkpoint=rt.checkpoint)
         logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)          # [N*L, pitch]
         ctx.model, ctx.sv, ctx.ids, ctx.hs = model, sv, ids, (hs if need else None)
         ctx.dims = (N, L, n_ids, hidden is not None)
+        ctx.guard = _checkpoint_guard(rt, sv)
         return logits.view(N, L, rt.pitch)[:, :, :rt.V]
 
     @staticmethod
     def backward(ctx, dlogits):
         model = ctx.model
         rt = model._rt()
+        _check_checkpoint_guard(ctx.guard, rt)
         N, L, n_ids, has_hidden = ctx.dims
         dl = _as_pitched(dlogits, N * L, rt.pitch)
         if dl is None:
@@ -396,6 +420,7 @@ class _KVState:
 
 class MIDIModel(PreTrainedModel):
     config_class = MIDIModelConfig
+    supports_gradient_checkpointing = True
 
     def __init__(self, config: MIDIModelConfig, *args, **kwargs):
         super(MIDIModel, self).__init__(config, *args, **kwargs)
@@ -414,6 +439,29 @@ class MIDIModel(PreTrainedModel):
             rt = _Runtime(self)
             self.__dict__["_b200_rt"] = rt
         return rt
+
+    # ------------------------------------------------------------------ activation checkpointing
+    def gradient_checkpointing_enable(self, gradient_checkpointing_kwargs=None):
+        """Activation checkpointing for both training paths (training_loss, and forward / forward_token under autograd):
+        the forward keeps per decoder layer only its input, its attention output and (event-level stack) the attention's
+        log-sum-exp; backward recomputes the layer's norms, projections and SwiGLU from them before the layer's gradients.
+        The recompute runs the forward's own kernels, so loss and gradients are those of a step without checkpointing;
+        a step costs the extra projections (no attention forward, no down_proj) and saves most activation memory.
+        Inference calls save nothing and are unaffected.  `gradient_checkpointing_kwargs` is accepted for signature
+        compatibility with transformers and has no effect: there is one fixed policy and no torch.utils.checkpoint."""
+        self._set_activation_checkpointing(True)
+
+    def gradient_checkpointing_disable(self):
+        """Turn activation checkpointing off again: every intermediate of every layer is saved until backward."""
+        self._set_activation_checkpointing(False)
+
+    def _set_activation_checkpointing(self, on: bool) -> None:
+        # the HF containers' flag makes `is_gradient_checkpointing` tell the truth, and a rebuilt runtime inherits it
+        self.net.gradient_checkpointing = on
+        self.net_token.gradient_checkpointing = on
+        rt = self.__dict__.get("_b200_rt")
+        if rt is not None:
+            rt.checkpoint = on
 
     # ------------------------------------------------------------------ LoRA (train.py:439-449, 234-244, 263-264)
     def add_adapter(self, adapter_config, adapter_name: Optional[str] = None):
@@ -835,7 +883,7 @@ class MIDIModel(PreTrainedModel):
             maps = _sample_maps(_sample_positions(sample_idx, S), B, S, rt.store.device)
         x, y = _batch_xy(batch)
         e = _ops.embed_sum(x, rt.outer.embed)
-        hidden, sv_o = rt.outer.forward(e, B, S, self.net.rotary_emb.inv_freq, save=backward)
+        hidden, sv_o = rt.outer.forward(e, B, S, self.net.rotary_emb.inv_freq, save=backward, checkpoint=rt.checkpoint)
         if maps is None:
             N = B * S
             ids_in = y[:, :-1].contiguous()
@@ -846,7 +894,8 @@ class MIDIModel(PreTrainedModel):
             xin, y_sel = _ops.inner_input_rows(hidden, y, maps[0], rt.inner.embed)
             ids_in = y_sel[:, :-1].contiguous()
             targets = y_sel.view(-1)
-        hs, sv_i = rt.inner.forward(xin, N, T, self.net_token.rotary_emb.inv_freq, save=backward)
+        hs, sv_i = rt.inner.forward(xin, N, T, self.net_token.rotary_emb.inv_freq, save=backward,
+                                    checkpoint=rt.checkpoint)
         del xin
         logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)
         lac, lse = _ops.ce_fwd(logits, targets, rt.V, tok.pad_id)
