@@ -10,7 +10,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 GROUP_NAMES = ["gemm_fwd", "gemm_swiglu", "gemm_dgrad", "gemm_wgrad", "elementwise", "fused_rope", "attn_flash", "attn_wgmma", "attn_tiny", "loss_optim", "decode",
                "model_forward", "model_layer_tf", "model_train", "model_generate", "model_peaked_greedy", "model_large",
                "gemm_exact", "decode_paged", "lora_train", "model_vs_hf", "model_medium_long",
-               "gemm_matrix", "gemm_epilogues", "attn_edges"]
+               "gemm_matrix", "gemm_epilogues", "attn_edges", "gemv_matrix", "decode_attn_edges", "sampler_exact",
+               "persist_vs_phase"]
 
 
 @pytest.mark.gpu
