@@ -57,6 +57,11 @@ int b200_inner_input_rows_bwd_hidden(const void* dx, const int* inv, void* dhidd
 /* host data path (train.py:71 int16 token matrices; train.py:169-176 x = batch[:, :-1], y = batch[:, 1:]):
    batch int16 [B, S1, T] -> x, y int64 [B*(S1-1), T] in one pass */
 int b200_batch_to_xy_i16(const void* batch, int B, int S1, int T, long long* x, long long* y, cudaStream_t s);
+/* the same into a ragged (segment-packed) layout: packed row r gets x = batch row src[r], y = the batch row after it, where
+   src (device int32 [n_rows]) indexes the B*S1 rows of the int16 batch; src[r] < 0 (a gap row) gives x = y = pad_id in every
+   column.  No other batch row is read. */
+int b200_batch_to_xy_packed_i16(const void* batch, int T, const int* src, int n_rows, int pad_id, long long* x, long long* y,
+                                cudaStream_t s);
 size_t b200_embed_bwd_workspace_bytes(int n_ids, int V, int H);
 /* id i reads gradient row (i / per_row) * row_stride + (i % per_row) * row_inner + row_off; pad row gets 0 */
 int b200_embed_bwd(const long long* ids, int n_ids, const void* dout, void* dtable, int V, int H, int per_row,
@@ -83,6 +88,10 @@ int b200_rope_table(const float* inv_freq, int half, int n_pos, int pos0, const 
 /* row r sits at absolute position pos0 (+ *pos0_dev) + r % S; tables are indexed by absolute position */
 int b200_rope_qk(void* qkv, const void* cos_t, const void* sin_t, int rows, int S, int H, int D, int ld, int backward,
                  int pos0, const int* pos0_dev /*may be NULL*/, cudaStream_t s);
+/* segment-packed rows (rows % 64 == 0): seg (device int32 [rows/64][2]) = {first, last} 64-row tile of each tile's segment;
+   row r sits at position r - 64 * seg[2 * (r / 64)] */
+int b200_rope_qk_seg(void* qkv, const void* cos_t, const void* sin_t, int rows, const int* seg, int H, int D, int ld,
+                     int backward, cudaStream_t s);
 
 /* ---- SwiGLU (hf modeling_llama.py:183) on packed [rows, 2I] = [gate | up] ------------------------- */
 int b200_swiglu_fwd(const void* gu, void* act, long long rows, int I, cudaStream_t s);
@@ -116,6 +125,10 @@ int b200_gemm_bf16(const void* A, const void* B, void* C, const void* R, int M, 
  *      r % S, columns [0, rope_cols) are rotated per head of width head_dim, the rest (v) is stored unrotated. */
 int b200_gemm_bf16_rope(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                         const void* rope_cos, const void* rope_sin, int S, int head_dim, int rope_cols, cudaStream_t s);
+/*      the same with the positions of a segment table (see b200_rope_qk_seg); M % 64 == 0 */
+int b200_gemm_bf16_rope_seg(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
+                            const void* rope_cos, const void* rope_sin, const int* seg, int head_dim, int rope_cols,
+                            cudaStream_t s);
 
 /*      gate|up projection with SwiGLU fused (hf modeling_llama.py:182-184): gu[M,2I] = A . Wgu^T is stored (backward
  *      needs g, u) and act[M,I] = bf16(bf16(silu(g)) * u) is produced by the same epilogue; I % 128 == 0 */
@@ -144,6 +157,19 @@ int b200_attn_causal_bwd_wgmma(const void* q, const void* k, const void* v, cons
                                const long long* strides /*8x3: q,k,v,o,do,dq,dk,dv*/, int batch, int n_heads, int Sq,
                                int Sk, int head_dim, float scale, const void* rope_cos /*may be NULL*/,
                                const void* rope_sin, cudaStream_t s);
+/*      segment mode: one packed batch of N = 64 * n_tiles rows holding several sequences, each a segment of whole 64-row
+ *      tiles (seg: device int32 [n_tiles][2] = {first, last} tile of each tile's segment).  Every query attends causally
+ *      to the keys of its own segment; RoPE positions (fused backward) are in-segment.  strides are {row, head} element
+ *      strides per operand; lse and delta are [n_heads, N].  order (device int32) lists tiles longest loop first:
+ *      [n_tiles] query tiles for the forward; [2][n_tiles] query tiles (dq) then key tiles (dk, dv) for the backward. */
+int b200_attn_causal_fwd_seg_wgmma(const void* q, const void* k, const void* v, void* o, float* lse /*may be NULL*/,
+                                   const long long* strides /*4x2: q,k,v,o*/, int n_tiles, int n_heads, int head_dim,
+                                   float scale, const int* seg, const int* order, cudaStream_t s);
+int b200_attn_causal_bwd_seg_wgmma(const void* q, const void* k, const void* v, const void* o, const void* d_o,
+                                   const float* lse, float* delta /*float[n_heads*N]*/, void* dq, void* dk, void* dv,
+                                   const long long* strides /*8x2: q,k,v,o,do,dq,dk,dv*/, int n_tiles, int n_heads,
+                                   int head_dim, float scale, const void* rope_cos /*may be NULL*/, const void* rope_sin,
+                                   const int* seg, const int* order, cudaStream_t s);
 /*      inner stack: L <= 8 positions per event, head_dim 256, packed qkv rows [n_events*L, ld_qkv]. */
 /*      rope_cos/sin != NULL: qkv holds PRE-RoPE projections; q and k are rotated in place (fused RoPE) before use */
 int b200_attn_tiny_fwd(void* qkv, void* out, int n_events, int L, int n_heads, int head_dim, int ld_qkv, int ld_out,

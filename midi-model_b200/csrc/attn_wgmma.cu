@@ -10,6 +10,11 @@
 //   dkv : CTA = 64 keys x (batch, head), loops over query tiles: dV += P^T dO, dK += dS^T Q   (no atomics)
 //   dq  : CTA = 64 query rows x (batch, head), loops over key tiles: dQ += dS K                (no atomics)
 // The RoPE backward can be fused into the dK / dQ stores (gradient w.r.t. the pre-rotation projections).
+// Segment mode (SEG = true): one packed "batch" of N rows holding several sequences, each a segment of whole 64-row
+// tiles.  seg[2 t] / seg[2 t + 1] = first / last tile of tile t's segment: a query tile's key loop starts at its
+// segment's first tile, a key tile's query loop ends at its segment's last tile, so no tile mixes sequences and the
+// causal mask inside a tile is the unsegmented one.  RoPE positions are in-segment (row - 64 * first).  `order` lists
+// the tiles by descending loop length (longest first, as the unsegmented grids run them).
 // Same semantics as the mma.sync kernels of attn_flash.cu, which the tests use as the second implementation.
 #include "hopper.cuh"
 
@@ -84,20 +89,22 @@ __device__ __forceinline__ uint8_t* smem_base() {
 
 // ------------------------------------------------------------------------------------------------ forward
 // smem: Q | K[2] | V[2] | barriers
+template <bool SEG>
 __global__ void __launch_bounds__(NT)
 attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                       const __grid_constant__ CUtensorMap tmV, bf16* __restrict__ o, float* __restrict__ lse, Strides so,
-                      const Params p) {
+                      const Params p, const int* __restrict__ seg, const int* __restrict__ order) {
     uint8_t* sm = smem_base();
     uint8_t* sQ = sm;
     uint8_t* sK = sm + TILE_BYTES;
     uint8_t* sV = sK + 2 * TILE_BYTES;
     uint64_t* bar = reinterpret_cast<uint64_t*>(sV + 2 * TILE_BYTES);     // [0]: Q, [1 + s]: K/V stage s
     const int bh = blockIdx.x, b = bh / p.n_heads, h = bh % p.n_heads;
-    const int q_blk = gridDim.y - 1 - blockIdx.y;                          // longest rows first
+    const int q_blk = SEG ? order[blockIdx.y] : gridDim.y - 1 - blockIdx.y;   // longest rows first
     const int q0 = q_blk * T;
     const int last_key = min(q0 + T - 1 + p.off, p.Sk - 1);
     const int nk = last_key / T + 1;
+    const int j0 = SEG ? seg[2 * q_blk] : 0;                                // first key tile
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, cq = 2 * (lane & 3);
     if (tid == 0) {
         for (int i = 0; i < 3; i++) mbar_init(&bar[i], 1);
@@ -105,8 +112,8 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         mbar_expect_tx(&bar[0], TILE_BYTES);
         tma_load_3d(sQ, &tmQ, &bar[0], h * D, q0, b);
         mbar_expect_tx(&bar[1], 2 * TILE_BYTES);
-        tma_load_3d(sK, &tmK, &bar[1], h * D, 0, b);
-        tma_load_3d(sV, &tmV, &bar[1], h * D, 0, b);
+        tma_load_3d(sK, &tmK, &bar[1], h * D, j0 * T, b);
+        tma_load_3d(sV, &tmV, &bar[1], h * D, j0 * T, b);
     }
     __syncthreads();
     float oacc[32], s[32];
@@ -116,14 +123,14 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const float sl2 = p.scale * LOG2E;
     const int r0 = warp * 16 + (lane >> 2);
     mbar_wait(&bar[0], 0);
-    for (int j = 0; j < nk; j++) {
-        const int st = j & 1;
+    for (int j = j0; j < nk; j++) {
+        const int st = (j - j0) & 1;
         if (tid == 0 && j + 1 < nk) {           // stage st ^ 1 was released by the barrier that ended iteration j - 1
             mbar_expect_tx(&bar[1 + (st ^ 1)], 2 * TILE_BYTES);
             tma_load_3d(sK + (st ^ 1) * TILE_BYTES, &tmK, &bar[1 + (st ^ 1)], h * D, (j + 1) * T, b);
             tma_load_3d(sV + (st ^ 1) * TILE_BYTES, &tmV, &bar[1 + (st ^ 1)], h * D, (j + 1) * T, b);
         }
-        mbar_wait(&bar[1 + st], (j >> 1) & 1);
+        mbar_wait(&bar[1 + st], ((j - j0) >> 1) & 1);
         mma_tt(s, smem_u32(sQ), smem_u32(sK + st * TILE_BYTES));
         const int k0 = j * T;
         const bool edge = k0 + T - 1 > q0 + p.off || k0 + T > p.Sk;
@@ -181,12 +188,13 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 
 // ------------------------------------------------------------------------------------------------ backward dK, dV
 // smem: K | V | Q[2] | dO[2] | lse[2][64] | delta[2][64] | barriers
+template <bool SEG>
 __global__ void __launch_bounds__(NT)
 attn_bwd_dkv_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
                           const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dk,
                           bf16* __restrict__ dv, Strides sdk, Strides sdv, const Params p, const bf16* __restrict__ rope_cos,
-                          const bf16* __restrict__ rope_sin) {
+                          const bf16* __restrict__ rope_sin, const int* __restrict__ seg, const int* __restrict__ order) {
     uint8_t* sm = smem_base();
     uint8_t* sK = sm;
     uint8_t* sV = sm + TILE_BYTES;
@@ -196,9 +204,11 @@ attn_bwd_dkv_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     float* s_del = s_lse + 2 * T;                                   // [2][64]
     uint64_t* bar = reinterpret_cast<uint64_t*>(s_del + 2 * T);     // [0]: K/V, [1 + s]: Q/dO stage s
     const int bh = blockIdx.x, b = bh / p.n_heads, h = bh % p.n_heads;
-    const int k0 = blockIdx.y * T;
+    const int k_blk = SEG ? order[blockIdx.y] : blockIdx.y;
+    const int k0 = k_blk * T;
     const int q_first = max(0, k0 - p.off) / T;
-    const int q_end = (p.Sq + T - 1) / T;
+    const int q_end = SEG ? seg[2 * k_blk + 1] + 1 : (p.Sq + T - 1) / T;
+    const int pos0 = SEG ? seg[2 * k_blk] * T : 0;                  // RoPE position of row r: r - pos0
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, cq = 2 * (lane & 3);
     const float* lse_g = lse + (long long)bh * p.Sq;
     const float* del_g = delta + (long long)bh * p.Sq;
@@ -262,7 +272,7 @@ attn_bwd_dkv_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     for (int hh = 0; hh < 2; hh++) {
         const int key = k0 + r0 + 8 * hh;
         if (key < p.Sk) {
-            if (rope_cos) rope_bwd(dkacc, hh, rope_cos, rope_sin, key, cq);   // linear: commutes with the scale below
+            if (rope_cos) rope_bwd(dkacc, hh, rope_cos, rope_sin, key - pos0, cq);   // linear: commutes with the scale below
             bf16* dkg = dk + b * sdk.b + (long long)key * sdk.r + h * sdk.h + cq;
             bf16* dvg = dv + b * sdv.b + (long long)key * sdv.r + h * sdv.h + cq;
 #pragma unroll
@@ -276,11 +286,13 @@ attn_bwd_dkv_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
 
 // ------------------------------------------------------------------------------------------------ backward dQ
 // smem: Q | dO | K[2] | V[2] | barriers
+template <bool SEG>
 __global__ void __launch_bounds__(NT)
 attn_bwd_dq_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                          const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
                          const float* __restrict__ lse, const float* __restrict__ delta, bf16* __restrict__ dq, Strides sdq,
-                         const Params p, const bf16* __restrict__ rope_cos, const bf16* __restrict__ rope_sin) {
+                         const Params p, const bf16* __restrict__ rope_cos, const bf16* __restrict__ rope_sin,
+                         const int* __restrict__ seg, const int* __restrict__ order) {
     uint8_t* sm = smem_base();
     uint8_t* sQ = sm;
     uint8_t* sdO = sm + TILE_BYTES;
@@ -288,8 +300,10 @@ attn_bwd_dq_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     uint8_t* sV = sK + 2 * TILE_BYTES;
     uint64_t* bar = reinterpret_cast<uint64_t*>(sV + 2 * TILE_BYTES);     // [0]: Q/dO, [1 + s]: K/V stage s
     const int bh = blockIdx.x, b = bh / p.n_heads, h = bh % p.n_heads;
-    const int q0 = (gridDim.y - 1 - blockIdx.y) * T;
+    const int q_blk = SEG ? order[blockIdx.y] : gridDim.y - 1 - blockIdx.y;
+    const int q0 = q_blk * T;
     const int nk = min(q0 + T - 1 + p.off, p.Sk - 1) / T + 1;
+    const int j0 = SEG ? seg[2 * q_blk] : 0;                                // first key tile
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, cq = 2 * (lane & 3);
     if (tid == 0) {
         for (int i = 0; i < 3; i++) mbar_init(&bar[i], 1);
@@ -298,8 +312,8 @@ attn_bwd_dq_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
         tma_load_3d(sQ, &tmQ, &bar[0], h * D, q0, b);
         tma_load_3d(sdO, &tmdO, &bar[0], h * D, q0, b);
         mbar_expect_tx(&bar[1], 2 * TILE_BYTES);
-        tma_load_3d(sK, &tmK, &bar[1], h * D, 0, b);
-        tma_load_3d(sV, &tmV, &bar[1], h * D, 0, b);
+        tma_load_3d(sK, &tmK, &bar[1], h * D, j0 * T, b);
+        tma_load_3d(sV, &tmV, &bar[1], h * D, j0 * T, b);
     }
     const int r0 = warp * 16 + (lane >> 2);
     float lse_r[2], del_r[2];
@@ -315,14 +329,14 @@ attn_bwd_dq_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     const float sl2 = p.scale * LOG2E;
     __syncthreads();
     mbar_wait(&bar[0], 0);
-    for (int j = 0; j < nk; j++) {
-        const int st = j & 1;
+    for (int j = j0; j < nk; j++) {
+        const int st = (j - j0) & 1;
         if (tid == 0 && j + 1 < nk) {
             mbar_expect_tx(&bar[1 + (st ^ 1)], 2 * TILE_BYTES);
             tma_load_3d(sK + (st ^ 1) * TILE_BYTES, &tmK, &bar[1 + (st ^ 1)], h * D, (j + 1) * T, b);
             tma_load_3d(sV + (st ^ 1) * TILE_BYTES, &tmV, &bar[1 + (st ^ 1)], h * D, (j + 1) * T, b);
         }
-        mbar_wait(&bar[1 + st], (j >> 1) & 1);
+        mbar_wait(&bar[1 + st], ((j - j0) >> 1) & 1);
         const uint32_t aK = smem_u32(sK + st * TILE_BYTES);
         mma_tt(s, smem_u32(sQ), aK);              // S = Q K^T
         mma_tt(dp, smem_u32(sdO), smem_u32(sV + st * TILE_BYTES));   // dP = dO V^T
@@ -350,7 +364,7 @@ attn_bwd_dq_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     for (int hh = 0; hh < 2; hh++) {
         const int q = q0 + r0 + 8 * hh;
         if (q < p.Sq) {
-            if (rope_cos) rope_bwd(dqacc, hh, rope_cos, rope_sin, q + p.off, cq);
+            if (rope_cos) rope_bwd(dqacc, hh, rope_cos, rope_sin, q + p.off - (SEG ? seg[2 * q_blk] * T : 0), cq);
             bf16* dst = dq + b * sdq.b + (long long)q * sdq.r + h * sdq.h + cq;
 #pragma unroll
             for (int g = 0; g < 8; g++)
@@ -399,13 +413,13 @@ extern "C" int b200_attn_causal_fwd_wgmma(const void* q, const void* k, const vo
     if ((rc = tmap_of(&tv, v, strides + 6, n_heads, Sk, batch, "v"))) return rc;
     static bool configured = false;
     if (!configured) {
-        if ((rc = set_smem(attn_fwd_wgmma_kernel, SMEM_FWD))) return rc;
+        if ((rc = set_smem(attn_fwd_wgmma_kernel<false>, SMEM_FWD))) return rc;
         configured = true;
     }
     const Strides so{strides[9], strides[10], strides[11]};
     const Params p{n_heads, Sq, Sk, Sk - Sq, scale};
     dim3 grid(batch * n_heads, (Sq + T - 1) / T);
-    attn_fwd_wgmma_kernel<<<grid, NT, SMEM_FWD, stream>>>(tq, tk, tv, (bf16*)o, lse, so, p);
+    attn_fwd_wgmma_kernel<false><<<grid, NT, SMEM_FWD, stream>>>(tq, tk, tv, (bf16*)o, lse, so, p, nullptr, nullptr);
     B200_CHECK_LAUNCH("attn_causal_fwd_wgmma");
     return B200_OK;
 }
@@ -427,20 +441,102 @@ extern "C" int b200_attn_causal_bwd_wgmma(const void* q, const void* k, const vo
     if ((rc = b200_attn_bwd_delta_launch(o, d_o, delta, strides + 9, strides + 12, batch, n_heads, Sq, stream))) return rc;
     static bool configured = false;
     if (!configured) {
-        if ((rc = set_smem(attn_bwd_dkv_wgmma_kernel, SMEM_DKV))) return rc;
-        if ((rc = set_smem(attn_bwd_dq_wgmma_kernel, SMEM_DQ))) return rc;
+        if ((rc = set_smem(attn_bwd_dkv_wgmma_kernel<false>, SMEM_DKV))) return rc;
+        if ((rc = set_smem(attn_bwd_dq_wgmma_kernel<false>, SMEM_DQ))) return rc;
         configured = true;
     }
     const Params p{n_heads, Sq, Sk, Sk - Sq, scale};
     const Strides sdq{strides[15], strides[16], strides[17]}, sdk{strides[18], strides[19], strides[20]},
         sdv{strides[21], strides[22], strides[23]};
     dim3 gkv(batch * n_heads, (Sk + T - 1) / T);
-    attn_bwd_dkv_wgmma_kernel<<<gkv, NT, SMEM_DKV, stream>>>(tq, tk, tv, tdo, lse, delta, (bf16*)dk, (bf16*)dv, sdk, sdv, p,
-                                                             (const bf16*)rope_cos, (const bf16*)rope_sin);
+    attn_bwd_dkv_wgmma_kernel<false><<<gkv, NT, SMEM_DKV, stream>>>(tq, tk, tv, tdo, lse, delta, (bf16*)dk, (bf16*)dv, sdk,
+                                                                    sdv, p, (const bf16*)rope_cos, (const bf16*)rope_sin,
+                                                                    nullptr, nullptr);
     B200_CHECK_LAUNCH("attn_causal_bwd_dkv_wgmma");
     dim3 gq(batch * n_heads, (Sq + T - 1) / T);
-    attn_bwd_dq_wgmma_kernel<<<gq, NT, SMEM_DQ, stream>>>(tq, tk, tv, tdo, lse, delta, (bf16*)dq, sdq, p,
-                                                          (const bf16*)rope_cos, (const bf16*)rope_sin);
+    attn_bwd_dq_wgmma_kernel<false><<<gq, NT, SMEM_DQ, stream>>>(tq, tk, tv, tdo, lse, delta, (bf16*)dq, sdq, p,
+                                                                 (const bf16*)rope_cos, (const bf16*)rope_sin, nullptr, nullptr);
     B200_CHECK_LAUNCH("attn_causal_bwd_dq_wgmma");
+    return B200_OK;
+}
+
+// ===========================================================================
+// Segment mode: the same kernels over one packed batch of N = 64 * n_tiles rows (see the top of this file).  strides are
+// {row, head} element strides per operand; lse / delta are [n_heads, N].
+// ===========================================================================
+namespace {
+// {batch, row, head} strides of a one-sequence batch of `rows` rows, from {row, head}
+void seg_strides(long long* out, const long long* st, int n_ops, int rows) {
+    for (int i = 0; i < n_ops; i++) {
+        out[3 * i] = st[2 * i] * rows;
+        out[3 * i + 1] = st[2 * i];
+        out[3 * i + 2] = st[2 * i + 1];
+    }
+}
+}   // namespace
+
+extern "C" int b200_attn_causal_fwd_seg_wgmma(const void* q, const void* k, const void* v, void* o, float* lse,
+                                              const long long* strides /* 4 x {r,h}: q,k,v,o */, int n_tiles, int n_heads,
+                                              int head_dim, float scale, const int* seg, const int* order,
+                                              cudaStream_t stream) {
+    B200_CHECK_ARG(head_dim == D, "attn_causal_fwd_seg_wgmma: head_dim %d unsupported (64 only)", head_dim);
+    B200_CHECK_ARG(n_tiles >= 0 && (n_tiles == 0 || (seg && order)), "attn_causal_fwd_seg_wgmma: missing segment tables");
+    if (n_tiles == 0) return B200_OK;
+    const int N = n_tiles * T;
+    long long st[12];
+    seg_strides(st, strides, 4, N);
+    CUtensorMap tq, tk, tv;
+    int rc;
+    if ((rc = tmap_of(&tq, q, st, n_heads, N, 1, "q"))) return rc;
+    if ((rc = tmap_of(&tk, k, st + 3, n_heads, N, 1, "k"))) return rc;
+    if ((rc = tmap_of(&tv, v, st + 6, n_heads, N, 1, "v"))) return rc;
+    static bool configured = false;
+    if (!configured) {
+        if ((rc = set_smem(attn_fwd_wgmma_kernel<true>, SMEM_FWD))) return rc;
+        configured = true;
+    }
+    const Strides so{st[9], st[10], st[11]};
+    const Params p{n_heads, N, N, 0, scale};
+    dim3 grid(n_heads, n_tiles);
+    attn_fwd_wgmma_kernel<true><<<grid, NT, SMEM_FWD, stream>>>(tq, tk, tv, (bf16*)o, lse, so, p, seg, order);
+    B200_CHECK_LAUNCH("attn_causal_fwd_seg_wgmma");
+    return B200_OK;
+}
+
+extern "C" int b200_attn_causal_bwd_seg_wgmma(const void* q, const void* k, const void* v, const void* o, const void* d_o,
+                                              const float* lse, float* delta, void* dq, void* dk, void* dv,
+                                              const long long* strides /* 8 x {r,h}: q,k,v,o,do,dq,dk,dv */, int n_tiles,
+                                              int n_heads, int head_dim, float scale, const void* rope_cos,
+                                              const void* rope_sin, const int* seg, const int* order,
+                                              cudaStream_t stream) {
+    B200_CHECK_ARG(head_dim == D, "attn_causal_bwd_seg_wgmma: head_dim %d unsupported (64 only)", head_dim);
+    B200_CHECK_ARG(n_tiles >= 0 && (n_tiles == 0 || (seg && order)), "attn_causal_bwd_seg_wgmma: missing segment tables");
+    if (n_tiles == 0) return B200_OK;
+    const int N = n_tiles * T;
+    long long st[24];
+    seg_strides(st, strides, 8, N);
+    CUtensorMap tq, tk, tv, tdo;
+    int rc;
+    if ((rc = tmap_of(&tq, q, st, n_heads, N, 1, "q"))) return rc;
+    if ((rc = tmap_of(&tk, k, st + 3, n_heads, N, 1, "k"))) return rc;
+    if ((rc = tmap_of(&tv, v, st + 6, n_heads, N, 1, "v"))) return rc;
+    if ((rc = tmap_of(&tdo, d_o, st + 12, n_heads, N, 1, "dO"))) return rc;
+    if ((rc = b200_attn_bwd_delta_launch(o, d_o, delta, st + 9, st + 12, 1, n_heads, N, stream))) return rc;
+    static bool configured = false;
+    if (!configured) {
+        if ((rc = set_smem(attn_bwd_dkv_wgmma_kernel<true>, SMEM_DKV))) return rc;
+        if ((rc = set_smem(attn_bwd_dq_wgmma_kernel<true>, SMEM_DQ))) return rc;
+        configured = true;
+    }
+    const Params p{n_heads, N, N, 0, scale};
+    const Strides sdq{st[15], st[16], st[17]}, sdk{st[18], st[19], st[20]}, sdv{st[21], st[22], st[23]};
+    dim3 grid(n_heads, n_tiles);
+    attn_bwd_dkv_wgmma_kernel<true><<<grid, NT, SMEM_DKV, stream>>>(tq, tk, tv, tdo, lse, delta, (bf16*)dk, (bf16*)dv, sdk,
+                                                                   sdv, p, (const bf16*)rope_cos, (const bf16*)rope_sin,
+                                                                   seg, order + n_tiles);
+    B200_CHECK_LAUNCH("attn_causal_bwd_dkv_seg_wgmma");
+    attn_bwd_dq_wgmma_kernel<true><<<grid, NT, SMEM_DQ, stream>>>(tq, tk, tv, tdo, lse, delta, (bf16*)dq, sdq, p,
+                                                                (const bf16*)rope_cos, (const bf16*)rope_sin, seg, order);
+    B200_CHECK_LAUNCH("attn_causal_bwd_dq_seg_wgmma");
     return B200_OK;
 }

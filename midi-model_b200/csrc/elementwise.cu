@@ -501,14 +501,15 @@ __global__ void rope_table_kernel(const float* __restrict__ inv_freq, int half, 
 }
 
 // In place on the q and k thirds of packed qkv rows [rows, 3*H]; position of row r = pos0 (+ *pos0_dev) + r % S
-// (the tables cover absolute positions).
+// (the tables cover absolute positions), or with a segment table r - 64 * seg[2 * (r / 64)] (first row of r's segment).
 // forward : o1 = bf16(bf16(x1*c) + bf16(-x2*s)), o2 = bf16(bf16(x2*c) + bf16(x1*s))   (three roundings, A.4)
 // backward: dx1 = do1*c + do2*s, dx2 = do2*c - do1*s  (one rounding)
 template <bool BWD>
 __global__ void rope_kernel(bf16* __restrict__ qkv, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
-                            int rows, int S, int H, int D, int ld, int pos0, const int* __restrict__ pos0_dev) {
+                            int rows, int S, int H, int D, int ld, int pos0, const int* __restrict__ pos0_dev,
+                            const int* __restrict__ seg) {
     const int r = blockIdx.x;
-    const int s = pos0 + (pos0_dev ? *pos0_dev : 0) + r % S;
+    const int s = seg ? r - 64 * seg[2 * (r >> 6)] : pos0 + (pos0_dev ? *pos0_dev : 0) + r % S;
     const int half = D / 2;
     const int vec_per_head = half / 8;
     const int heads2 = 2 * (H / D);   // q heads then k heads (k third starts at column H)
@@ -690,6 +691,39 @@ extern "C" int b200_batch_to_xy_i16(const void* batch, int B, int S1, int T, lon
     return B200_OK;
 }
 
+// The same widening into a ragged (segment-packed) layout: packed row r takes x from batch row src[r] and y from the row
+// after it (src[r] indexes the B * S1 rows of the batch), or pad_id in every column when src[r] < 0 (a gap row).  Only
+// rows named by src and the row after each are read.
+namespace {
+__global__ void batch_to_xy_packed_kernel(const short* __restrict__ b, const int* __restrict__ src, long long* __restrict__ x,
+                                          long long* __restrict__ y, long long n, int T, int pad_id) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long r = i / T;
+        const int c = (int)(i - r * T);
+        const int s = src[r];
+        if (s < 0) {
+            x[i] = pad_id;
+            y[i] = pad_id;
+        } else {
+            const short* p = b + (long long)s * T + c;
+            x[i] = p[0];
+            y[i] = p[T];
+        }
+    }
+}
+}   // namespace
+
+extern "C" int b200_batch_to_xy_packed_i16(const void* batch, int T, const int* src, int n_rows, int pad_id, long long* x,
+                                           long long* y, cudaStream_t stream) {
+    B200_CHECK_ARG(T >= 1 && n_rows >= 0 && (n_rows == 0 || src), "batch_to_xy_packed: bad arguments (T %d, rows %d)", T,
+                   n_rows);
+    const long long n = (long long)n_rows * T;
+    if (n == 0) return B200_OK;
+    batch_to_xy_packed_kernel<<<grid_for((size_t)n, 256), 256, 0, stream>>>((const short*)batch, src, x, y, n, T, pad_id);
+    B200_CHECK_LAUNCH("batch_to_xy_packed");
+    return B200_OK;
+}
+
 extern "C" size_t b200_embed_bwd_workspace_bytes(int n_ids, int V, int H) {
     return (size_t)(3 * (V + 1) + n_ids) * sizeof(int) + 256 + (size_t)V * H * sizeof(float);
 }
@@ -823,10 +857,24 @@ extern "C" int b200_rope_qk(void* qkv, const void* cos_t, const void* sin_t, int
     B200_CHECK_ARG(D % 16 == 0 && H % D == 0 && ld % 8 == 0, "rope: head_dim must be a multiple of 16");
     if (rows == 0) return B200_OK;
     if (backward)
-        rope_kernel<true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev);
+        rope_kernel<true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev, nullptr);
     else
-        rope_kernel<false><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev);
+        rope_kernel<false><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev, nullptr);
     B200_CHECK_LAUNCH("rope");
+    return B200_OK;
+}
+
+extern "C" int b200_rope_qk_seg(void* qkv, const void* cos_t, const void* sin_t, int rows, const int* seg, int H, int D,
+                                int ld, int backward, cudaStream_t stream) {
+    B200_CHECK_ARG(D % 16 == 0 && H % D == 0 && ld % 8 == 0, "rope_seg: head_dim must be a multiple of 16");
+    B200_CHECK_ARG(rows % 64 == 0 && (rows == 0 || seg), "rope_seg: rows (%d) must be whole 64-row tiles of a segment table",
+                   rows);
+    if (rows == 0) return B200_OK;
+    if (backward)
+        rope_kernel<true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, 1, H, D, ld, 0, nullptr, seg);
+    else
+        rope_kernel<false><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, 1, H, D, ld, 0, nullptr, seg);
+    B200_CHECK_LAUNCH("rope_seg");
     return B200_OK;
 }
 

@@ -37,9 +37,11 @@ struct GemmParams {
     int tail_tile0, tail_splits, tail_kb, total_items;
     float* tail_ws;
     int m_tiles, n_tiles;
-    // EPI_ROPE: rotary embedding applied to columns [0, rope_cols) (the q and k thirds of a packed QKV row)
+    // EPI_ROPE: rotary embedding applied to columns [0, rope_cols) (the q and k thirds of a packed QKV row); row r sits at
+    // position r % rope_S, or r - 64 * rope_seg[2 * (r / 64)] with a segment table (segments of whole 64-row tiles)
     const bf16* rope_cos;
     const bf16* rope_sin;
+    const int* rope_seg;
     int rope_S, rope_D, rope_cols;
     // EPI_SWIGLU: B = [gate | up] weight rows; tile n covers gate rows [128n, 128n+128) and up rows [I + 128n, ...)
     bf16* act;
@@ -103,7 +105,7 @@ __device__ __forceinline__ void wgmma_tile(float* acc, uint64_t da, uint64_t db,
 template <int BLOCK_N, int HALF8>
 __device__ __forceinline__ void rope_fragment(float* acc, const GemmParams& p, int n_blk, int row, int h, int cq) {
     if (row >= p.M) return;
-    const int pos = row % p.rope_S;
+    const int pos = p.rope_seg ? row - 64 * p.rope_seg[2 * (row >> 6)] : row % p.rope_S;
     const int half = HALF8 * 8;
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; j++) {
@@ -611,7 +613,7 @@ extern "C" int b200_gemm_suggest_splits(int M, int N, int K, int block_n) {
 static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda, int ldb, int ldc,
                      int ldr, int a_mn_major, int b_mn_major, int accumulate, int block_n, int splits, void* workspace,
                      size_t workspace_bytes, const bf16* rope_cos, const bf16* rope_sin, int rope_S, int rope_D,
-                     int rope_cols, cudaStream_t stream);
+                     int rope_cols, cudaStream_t stream, const int* rope_seg = nullptr);
 
 extern "C" int b200_gemm_bf16(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda, int ldb,
                               int ldc, int ldr, int a_mn_major, int b_mn_major, int accumulate, int block_n, int splits,
@@ -632,6 +634,18 @@ extern "C" int b200_gemm_bf16_rope(const void* A, const void* B, void* C, int M,
                      (const bf16*)rope_sin, S, head_dim, rope_cols, stream);
 }
 
+// The same with in-segment positions: row r sits at r - 64 * seg[2 * (r / 64)] (segments of whole 64-row tiles).
+extern "C" int b200_gemm_bf16_rope_seg(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
+                                       const void* rope_cos, const void* rope_sin, const int* seg, int head_dim,
+                                       int rope_cols, cudaStream_t stream) {
+    B200_CHECK_ARG(head_dim == 64 || head_dim == 128 || head_dim == 256, "gemm_rope_seg: head_dim %d unsupported", head_dim);
+    B200_CHECK_ARG(N % 256 == 0 && rope_cols % 256 == 0, "gemm_rope_seg: N and rope_cols must be multiples of 256");
+    B200_CHECK_ARG(M % 64 == 0 && seg && rope_cos && rope_sin, "gemm_rope_seg: M (%d) must be whole 64-row tiles; tables "
+                   "required", M);
+    return gemm_impl(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, 256, 1, nullptr, 0, (const bf16*)rope_cos,
+                     (const bf16*)rope_sin, 1, head_dim, rope_cols, stream, seg);
+}
+
 // Fused gate|up projection + SwiGLU: gu[M, 2I] = A . Wgu^T (stored, the backward pass needs g and u) and
 // act[M, I] = bf16(bf16(silu(g)) * u) written by the same epilogue.  Wgu = [gate rows | up rows], K-major operands.
 extern "C" int b200_gemm_bf16_swiglu(const void* A, const void* Wgu, void* gu, void* act, int M, int I, int K, int lda,
@@ -645,7 +659,7 @@ extern "C" int b200_gemm_bf16_swiglu(const void* A, const void* Wgu, void* gu, v
 static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda, int ldb, int ldc,
                      int ldr, int a_mn_major, int b_mn_major, int accumulate, int block_n, int splits, void* workspace,
                      size_t workspace_bytes, const bf16* rope_cos, const bf16* rope_sin, int rope_S, int rope_D,
-                     int rope_cols, cudaStream_t stream) {
+                     int rope_cols, cudaStream_t stream, const int* rope_seg) {
     const bool swiglu = (rope_S == -1);      // internal marker set by b200_gemm_bf16_swiglu (workspace = act, bytes = I | ld<<32)
     B200_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
     // N need not be a multiple of 8: B rows >= N are out of bounds for the tensor map (zero-filled), so the
@@ -682,7 +696,7 @@ static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M
     } else {
         p.epilogue = R ? EPI_RESIDUAL : EPI_STORE;
     }
-    p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.rope_S = rope_S; p.rope_D = rope_D; p.rope_cols = rope_cols;
+    p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.rope_seg = rope_seg; p.rope_S = rope_S; p.rope_D = rope_D; p.rope_cols = rope_cols;
     if (rope_cos) p.epilogue = EPI_ROPE;
     p.act = nullptr; p.swiglu_I = 0; p.ld_act = 0;
     if (swiglu) {

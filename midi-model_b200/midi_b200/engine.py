@@ -192,6 +192,21 @@ class ParamStore:
         self.gflat.zero_()
 
 
+SEG_TILE = 64   # rows per segment tile: the event-level attention's tile height (csrc/attn_wgmma.cu T)
+
+
+@dataclass
+class Segments:
+    """Ragged sequences packed tile-aligned into one buffer of `rows` rows: every sequence owns a segment of whole 64-row
+    tiles (its own rows, then gap rows), segments follow each other.  `tiles` int32 [rows / 64, 2] (device): {first, last}
+    tile of each tile's segment -- row r sits at RoPE position r - 64 * tiles[r // 64, 0]; `order` int32 [2, rows / 64]
+    (device): query tiles, then key tiles, by descending attention loop length; `max_len`: the longest segment's rows."""
+    rows: int
+    max_len: int
+    tiles: torch.Tensor
+    order: torch.Tensor
+
+
 @dataclass
 class StackCfg:
     prefix: str
@@ -384,22 +399,33 @@ class StackEngine:
     # The layer body is split around the attention so that the forward and the backward's recompute of a checkpointed
     # layer (_recompute) issue the same kernels in the same order on the same operands: every forward kernel is
     # deterministic and the GEMM plan is a function of the shape, so the recomputed tensors equal the forward's bit for bit.
-    def _qkv(self, w: LayerW, n1: torch.Tensor, cos, sin, S: int, lsv: dict, rotate: bool) -> torch.Tensor:
+    def _qkv(self, w: LayerW, n1: torch.Tensor, cos, sin, S: int, lsv: dict, rotate: bool,
+             seg: Optional[Segments] = None) -> torch.Tensor:
         """Packed QKV projection of n1, the q/k/v adapters added BEFORE the rotation, and RoPE on the q and k thirds.
         rotate=False leaves the rotation to the token-level attention kernel (fused RoPE, the forward's default there);
+        with `seg` rows sit at in-segment positions instead of r % S;
         the stand-alone RoPE kernel performs the same three roundings (csrc/attn_tiny.cu rope_fwd_lane, csrc/elementwise.cu
         rope_kernel), so a recompute that does not run attention gets the rotated q, k the forward's kernel wrote back."""
         H, D = self.cfg.hidden, self.cfg.head_dim
         lo = w.lora
         if FUSE_ROPE_FWD and not any(k in lo for k in ("q", "k", "v")):
+            if seg is not None:
+                return ops.linear_rope_seg(n1, w.qkv, cos, sin, seg.tiles, D)
             return ops.linear_rope(n1, w.qkv, cos, sin, S, D)         # QKV GEMM with RoPE in the epilogue
         qkv = ops.linear(n1, w.qkv)
         for j, key in enumerate(("q", "k", "v")):
             if key in lo:
                 lsv[key] = self._lora_fwd(lo[key], n1, qkv, j * H, H)
         if rotate:
-            ops.rope_qk_(qkv, cos, sin, S, H, D)
+            self._rope(qkv, cos, sin, S, seg, backward=False)
         return qkv
+
+    def _rope(self, qkv: torch.Tensor, cos, sin, S: int, seg: Optional[Segments], backward: bool) -> None:
+        H, D = self.cfg.hidden, self.cfg.head_dim
+        if seg is not None:
+            ops.rope_qk_seg_(qkv, cos, sin, seg.tiles, H, D, backward=backward)
+        else:
+            ops.rope_qk_(qkv, cos, sin, S, H, D, backward=backward)
 
     def _mlp_in(self, w: LayerW, x: torch.Tensor, attn: torch.Tensor, lsv: dict):
         """From the layer input x and the attention output: o_proj (+ adapter), the residual add fused into the
@@ -423,13 +449,19 @@ class StackEngine:
             act = ops.swiglu(gu)
         return h, n2, rstd2, gu, act
 
-    def forward(self, x: torch.Tensor, n_seq: int, S: int, inv_freq: torch.Tensor, save: bool, checkpoint: bool = False):
+    def forward(self, x: torch.Tensor, n_seq: int, S: int, inv_freq: torch.Tensor, save: bool, checkpoint: bool = False,
+                seg: Optional[Segments] = None):
         """x: [n_seq * S, H] inputs_embeds (row-major, sequences contiguous) -> (final-normed hidden, saved).
+        seg (event-level stack only): x holds the seg.rows rows of ragged sequences packed by `Segments` instead, and
+        (n_seq, S) must be (1, seg.rows); RoPE and attention then keep to each row's own segment.
         checkpoint (with save): keep per layer only its input x, the attention output, the attention's log-sum-exp and
         the down_proj adapter's scaled down-projection; backward recomputes the rest of the layer (_recompute)."""
         c = self.cfg
         H, D, nh = c.hidden, c.head_dim, c.n_head
-        cos, sin = ops.rope_table(inv_freq, S)
+        if seg is not None and (self.tiny or (n_seq, S) != (1, seg.rows) or x.shape[0] != seg.rows):
+            raise lib.B200Error(f"segment-packed forward: {x.shape[0]} rows as ({n_seq}, {S}) for {seg.rows} packed rows "
+                                f"(event-level stack only)")
+        cos, sin = ops.rope_table(inv_freq, S if seg is None else seg.max_len)
         saved = [] if save else None
         checkpoint = checkpoint and save
         # Residual adds are fused into the norm that follows them (x + y is formed, rounded to bf16 and written by
@@ -443,9 +475,11 @@ class StackEngine:
                 n1, rstd1 = ops.rmsnorm(x, w.ln1, c.eps, want_rstd=True)
             else:
                 x, n1, rstd1 = ops.add_rmsnorm(x, pending, w.ln1, c.eps)
-            qkv = self._qkv(w, n1, cos, sin, S, lsv, rotate=not fuse_tiny)
+            qkv = self._qkv(w, n1, cos, sin, S, lsv, rotate=not fuse_tiny, seg=seg)
             if self.tiny:
                 attn, lse = ops.attn_tiny_fwd(qkv, n_seq, S, nh, D, rope=(cos, sin) if fuse_tiny else None), None
+            elif seg is not None:
+                attn, lse = ops.attn_causal_fwd_seg(qkv, seg.tiles, seg.order, nh, D, want_lse=save)
             else:
                 attn, lse = ops.attn_causal_fwd(qkv, n_seq, S, nh, D, want_lse=save)
             h, n2, rstd2, gu, act = self._mlp_in(w, x, attn, lsv)
@@ -460,10 +494,10 @@ class StackEngine:
             x = h
         x, y, rstd_f = ops.add_rmsnorm(x, pending, self.norm, c.eps)
         sv = dict(layers=saved, checkpoint=checkpoint, x_last=x, rstd_f=rstd_f, n_seq=n_seq, S=S, cos=cos,
-                  sin=sin) if save else None
+                  sin=sin, seg=seg) if save else None
         return y, sv
 
-    def _recompute(self, w: LayerW, kept, cos, sin, S: int):
+    def _recompute(self, w: LayerW, kept, cos, sin, S: int, seg: Optional[Segments] = None):
         """A checkpointed layer's saved set, in the layout forward() saves without checkpointing, from what it kept.
         n1 comes from rmsnorm(x) where the forward formed it with add_rmsnorm(x_prev, down_out) (layer 0: rmsnorm too):
         at every supported hidden size both run the same warp kernel, which sums the squares of the already-rounded bf16
@@ -471,7 +505,7 @@ class StackEngine:
         backward does not read the down_proj output."""
         x, attn, lse, lsv = kept
         n1, rstd1 = ops.rmsnorm(x, w.ln1, self.cfg.eps, want_rstd=True)
-        qkv = self._qkv(w, n1, cos, sin, S, lsv, rotate=True)
+        qkv = self._qkv(w, n1, cos, sin, S, lsv, rotate=True, seg=seg)
         h, n2, rstd2, gu, act = self._mlp_in(w, x, attn, lsv)
         return x, n1, rstd1, qkv, attn, lse, h, n2, rstd2, gu, act, lsv
 
@@ -495,7 +529,7 @@ class StackEngine:
         H, D, nh, I = c.hidden, c.head_dim, c.n_head, c.inner
         if sv is None or sv["layers"] is None:
             raise lib.B200Error("backward called without a saved forward")
-        n_seq, S, cos, sin = sv["n_seq"], sv["S"], sv["cos"], sv["sin"]
+        n_seq, S, cos, sin, seg = sv["n_seq"], sv["S"], sv["cos"], sv["sin"], sv["seg"]
         side = _side_stream(dy.device) if WGRAD_STREAM else None
         pending = []          # (event on the side stream, operands of the wgrads issued before it), released one layer late
         dx = ops.rmsnorm_bwd(dy, sv["x_last"], self.norm, sv["rstd_f"], None, grads.norm, accumulate)
@@ -517,7 +551,7 @@ class StackEngine:
                     old_ev, old_hold = pending.pop(0)
                     torch.cuda.current_stream().wait_event(old_ev)
                     old_hold.clear()
-                ent = self._recompute(w, ent, cos, sin, S)
+                ent = self._recompute(w, ent, cos, sin, S, seg)
             x, n1, rstd1, qkv, attn, lse, h, n2, rstd2, gu, act, lsv = ent
             del ent
             # ---- MLP block: x_out = h + down(act)
@@ -548,11 +582,13 @@ class StackEngine:
             rope = (cos, sin) if FUSE_ROPE else None
             if self.tiny:
                 dqkv = ops.attn_tiny_bwd(qkv, dattn, n_seq, S, nh, D, rope=rope)
+            elif seg is not None:
+                dqkv = ops.attn_causal_bwd_seg(qkv, attn, dattn, lse, seg.tiles, seg.order, nh, D, rope=rope)
             else:
                 dqkv = ops.attn_causal_bwd(qkv, attn, dattn, lse, n_seq, S, nh, D, rope=rope)
             del dattn, attn, qkv
             if not FUSE_ROPE:
-                ops.rope_qk_(dqkv, cos, sin, S, H, D, backward=True)
+                self._rope(dqkv, cos, sin, S, seg, backward=True)
             dn1 = ops.linear_dgrad(dqkv, w.qkv)
             if g.qkv is not None:
                 _wgrad(dqkv, n1, g.qkv, accumulate, side, hold)

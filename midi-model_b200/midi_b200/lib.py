@@ -29,6 +29,7 @@ SIGNATURES = {
     "b200_inner_input_rows_fwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "b200_inner_input_rows_bwd_hidden": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "b200_batch_to_xy_i16": (i32, [vp, i32, i32, i32, vp, vp, vp]),
+    "b200_batch_to_xy_packed_i16": (i32, [vp, i32, vp, i32, i32, vp, vp, vp]),
     "b200_embed_bwd_workspace_bytes": (sz, [i32, i32, i32]),
     "b200_embed_bwd": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, sz, vp]),
     "b200_rmsnorm_fwd": (i32, [vp, vp, vp, vp, i32, i32, f32, vp]),
@@ -37,6 +38,7 @@ SIGNATURES = {
     "b200_rmsnorm_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, sz, vp]),
     "b200_rope_table": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
     "b200_rope_qk": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp]),
+    "b200_rope_qk_seg": (i32, [vp, vp, vp, i32, vp, i32, i32, i32, i32, vp]),
     "b200_swiglu_fwd": (i32, [vp, vp, i64, i32, vp]),
     "b200_swiglu_bwd": (i32, [vp, vp, vp, i64, i32, vp]),
     "b200_scale_bf16": (i32, [vp, vp, i64, f32, vp]),
@@ -46,11 +48,14 @@ SIGNATURES = {
     "b200_gemm_plan": (i32, [i32, i32, i32, i32, vp, vp]),
     "b200_gemm_bf16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, sz, vp]),
     "b200_gemm_bf16_rope": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp]),
+    "b200_gemm_bf16_rope_seg": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp]),
     "b200_gemm_bf16_swiglu": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "b200_attn_causal_fwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp]),
     "b200_attn_causal_fwd_wgmma": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp]),
     "b200_attn_causal_bwd_wgmma": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200_attn_causal_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
+    "b200_attn_causal_fwd_seg_wgmma": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp, vp, vp]),
+    "b200_attn_causal_bwd_seg_wgmma": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp, vp, vp, vp, vp]),
     "b200_attn_tiny_fwd": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200_attn_tiny_bwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200_ce_fwd": (i32, [vp, vp, vp, vp, vp, i64, i32, i32, i64, vp]),

@@ -101,6 +101,22 @@ def batch_to_xy(batch: torch.Tensor):
     return x, y
 
 
+def batch_to_xy_packed(batch: torch.Tensor, src: torch.Tensor, pad_id: int):
+    """int16 [B, S+1, T] batch + src int32 [N] (device; batch row b * (S+1) + i of each packed row, -1 for a gap row) ->
+    (x, y) int64 [N, T]: x = that batch row, y = the row after it; x = y = pad_id on gap rows."""
+    if not batch.is_cuda or batch.dtype != torch.int16 or not batch.is_contiguous():
+        raise lib.B200Error(f"batch_to_xy_packed: expected a contiguous CUDA int16 batch, got {batch.dtype} on {batch.device}")
+    if src.dtype != torch.int32 or src.dim() != 1 or src.device != batch.device:
+        raise lib.B200Error(f"batch_to_xy_packed: src must be int32 [N] on {batch.device}, got {src.dtype} {tuple(src.shape)}")
+    T = batch.shape[2]
+    src = src.contiguous()
+    x = torch.empty((src.shape[0], T), dtype=torch.long, device=batch.device)
+    y = torch.empty_like(x)
+    lib.call("b200_batch_to_xy_packed_i16", batch.data_ptr(), T, src.data_ptr(), src.shape[0], int(pad_id), x.data_ptr(),
+             y.data_ptr(), lib.stream())
+    return x, y
+
+
 def embed_bwd(ids: torch.Tensor, dout: torch.Tensor, dtable: torch.Tensor, per_row: int, row_stride: int, row_inner: int,
               row_off: int, pad_id: int, accumulate: bool):
     V, H = dtable.shape
@@ -158,6 +174,14 @@ def rope_qk_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, S: int, H:
     rows, ld = qkv.shape
     lib.call("b200_rope_qk", qkv.data_ptr(), cos.data_ptr(), sin.data_ptr(), rows, S, H, D, ld, int(backward), pos0,
              lib.ptr(pos0_dev), lib.stream())
+
+
+def rope_qk_seg_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, tiles: torch.Tensor, H: int, D: int,
+                 backward: bool = False):
+    """rope_qk_ on segment-packed rows: row r sits at r - 64 * tiles[r // 64, 0] (int32 [rows / 64, 2] device table)."""
+    rows, ld = qkv.shape
+    lib.call("b200_rope_qk_seg", qkv.data_ptr(), cos.data_ptr(), sin.data_ptr(), rows, tiles.data_ptr(), H, D, ld,
+             int(backward), lib.stream())
 
 
 def swiglu(gu: torch.Tensor) -> torch.Tensor:
@@ -333,6 +357,45 @@ def attn_causal_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, ls
     return dqkv
 
 
+def _require_wgmma(impl: Optional[str], what: str):
+    if (impl or ATTN_IMPL) != "wgmma":
+        raise lib.B200Error(f"{what}: ragged (segment-packed) batches run on the wgmma attention only "
+                            f"(B200_ATTN={impl or ATTN_IMPL} has no segment mode)")
+
+
+def attn_causal_fwd_seg(qkv: torch.Tensor, tiles: torch.Tensor, order: torch.Tensor, n_heads: int, D: int, want_lse: bool,
+                        impl: Optional[str] = None):
+    """qkv: [N, 3H] segment-packed post-RoPE rows (N = 64 * n_tiles), tiles int32 [n_tiles, 2] = {first, last} tile of each
+    tile's segment, order int32 [2, n_tiles] (query tiles, key tiles; longest loop first) -> out [N, H], lse [h, N] fp32."""
+    _require_wgmma(impl, "attn_causal_fwd_seg")
+    H = n_heads * D
+    N, ld = qkv.shape[0], qkv.stride(0)
+    out = torch.empty((N, H), dtype=BF16, device=qkv.device)
+    lse = torch.empty((n_heads, N), dtype=torch.float32, device=qkv.device) if want_lse else None
+    st = torch.tensor([ld, D] * 3 + [H, D], dtype=torch.int64)
+    base = qkv.data_ptr()
+    lib.call("b200_attn_causal_fwd_seg_wgmma", base, base + 2 * H, base + 4 * H, out.data_ptr(), lib.ptr(lse), st.data_ptr(),
+             tiles.shape[0], n_heads, D, 1.0 / math.sqrt(D), tiles.data_ptr(), order.data_ptr(), lib.stream())
+    return out, lse
+
+
+def attn_causal_bwd_seg(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, tiles: torch.Tensor,
+                        order: torch.Tensor, n_heads: int, D: int, rope=None, impl: Optional[str] = None) -> torch.Tensor:
+    """Backward of attn_causal_fwd_seg; `rope=(cos, sin)` also applies the RoPE backward at in-segment positions."""
+    _require_wgmma(impl, "attn_causal_bwd_seg")
+    H = n_heads * D
+    N, ld = qkv.shape[0], qkv.stride(0)
+    dqkv = torch.empty_like(qkv)
+    delta = torch.empty((n_heads, N), dtype=torch.float32, device=qkv.device)
+    st = torch.tensor([ld, D] * 3 + [H, D] * 2 + [ld, D] * 3, dtype=torch.int64)
+    b, d = qkv.data_ptr(), dqkv.data_ptr()
+    lib.call("b200_attn_causal_bwd_seg_wgmma", b, b + 2 * H, b + 4 * H, out.data_ptr(), dout.data_ptr(), lse.data_ptr(),
+             delta.data_ptr(), d, d + 2 * H, d + 4 * H, st.data_ptr(), tiles.shape[0], n_heads, D, 1.0 / math.sqrt(D),
+             rope[0].data_ptr() if rope else None, rope[1].data_ptr() if rope else None, tiles.data_ptr(), order.data_ptr(),
+             lib.stream())
+    return dqkv
+
+
 def attn_tiny_fwd(qkv: torch.Tensor, n_events: int, L: int, n_heads: int, D: int, rope=None) -> torch.Tensor:
     """`rope=(cos, sin)`: qkv holds pre-RoPE projections; q and k are rotated IN PLACE inside the kernel (fused RoPE)."""
     H = n_heads * D
@@ -361,6 +424,24 @@ def linear_rope(x: torch.Tensor, w_qkv: torch.Tensor, cos: torch.Tensor, sin: to
         e0.record()
     lib.call("b200_gemm_bf16_rope", x.data_ptr(), w_qkv.data_ptr(), out.data_ptr(), M, N, K, x.stride(0), w_qkv.stride(0), N,
              cos.data_ptr(), sin.data_ptr(), S, D, 2 * N // 3, lib.stream())
+    if prof is not None:
+        e1.record()
+        prof.append((e0, e1, 2.0 * M * N * K, (M, N, K, 0, 0, 256, 1)))
+    return out
+
+
+def linear_rope_seg(x: torch.Tensor, w_qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, tiles: torch.Tensor,
+                    D: int) -> torch.Tensor:
+    """linear_rope on segment-packed rows: row r sits at r - 64 * tiles[r // 64, 0]."""
+    M, K = x.shape
+    N = w_qkv.shape[0]
+    out = torch.empty((M, N), dtype=BF16, device=x.device)
+    prof = GEMM_PROFILE
+    if prof is not None:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    lib.call("b200_gemm_bf16_rope_seg", x.data_ptr(), w_qkv.data_ptr(), out.data_ptr(), M, N, K, x.stride(0), w_qkv.stride(0),
+             N, cos.data_ptr(), sin.data_ptr(), tiles.data_ptr(), D, 2 * N // 3, lib.stream())
     if prof is not None:
         e1.record()
         prof.append((e0, e1, 2.0 * M * N * K, (M, N, K, 0, 0, 256, 1)))

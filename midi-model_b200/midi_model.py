@@ -403,6 +403,87 @@ def _sample_maps(positions: list, B: int, S: int, device):
     return rows, inv
 
 
+def _ragged_rows(lengths, B: int, S: int, what: str) -> list:
+    """Event rows each sample trains on, from `lengths` (the number of real events of every sample of a [B, S+1, T]
+    batch, in [0, S+1]): S_b = L_b - 1 positions have a real target, a sample with L_b <= 1 has none."""
+    if isinstance(lengths, torch.Tensor):
+        if lengths.device.type != "cpu":
+            raise _lib.B200Error(f"{what} must be a CPU tensor or a Python sequence (checking device lengths would need a "
+                                 "host sync)")
+        if lengths.dtype == torch.bool or lengths.is_floating_point() or lengths.is_complex():
+            raise _lib.B200Error(f"{what} must hold integers, got {lengths.dtype}")
+        if lengths.dim() != 1:
+            raise _lib.B200Error(f"{what} must be 1-D, got shape {tuple(lengths.shape)}")
+        vals = lengths.tolist()
+    elif isinstance(lengths, collections.abc.Sequence) and not isinstance(lengths, (str, bytes)):
+        vals = list(lengths)
+        bad = [v for v in vals if isinstance(v, bool) or not isinstance(v, numbers.Integral)]
+        if bad:
+            raise _lib.B200Error(f"{what} must be a 1-D sequence of integers, got {bad[0]!r}")
+        vals = [int(v) for v in vals]
+    else:
+        raise _lib.B200Error(f"{what} must be a Python sequence or a CPU integer tensor, got {type(lengths).__name__}")
+    if len(vals) != B:
+        raise _lib.B200Error(f"{what} has {len(vals)} entries for a batch of {B} samples")
+    out_of_range = [v for v in vals if not 0 <= v <= S + 1]
+    if out_of_range:
+        raise _lib.B200Error(f"{what}: length {out_of_range[0]} is outside [0, {S + 1}] (the batch holds {S + 1} events)")
+    rows = [max(v - 1, 0) for v in vals]
+    if not any(rows):
+        raise _lib.B200Error(f"{what}: every sample has at most one event, so no position has a target")
+    return rows
+
+
+def _ragged_layout(rows: list, S1: int, device):
+    """Tile-aligned packing of B ragged sequences (DESIGN.md 1): sequence b owns a segment of roundup(rows[b], 64) packed
+    rows -- its rows 0 .. rows[b]-1, then gap rows -- and the segments follow in batch order.  Returns the source-row map
+    (int32 [N]: batch row b * S1 + i of packed row r, -1 for a gap row) and the engine's `Segments` (tile table and
+    longest-first tile orders), copied to `device` without a host sync."""
+    T = _engine.SEG_TILE
+    seg_rows = [(r + T - 1) // T * T for r in rows]
+    N = sum(seg_rows)
+    src = torch.full((N,), -1, dtype=torch.int32)
+    tiles = torch.empty((N // T, 2), dtype=torch.int32)
+    off = 0
+    for b, (r, R) in enumerate(zip(rows, seg_rows)):
+        src[off:off + r] = b * S1 + torch.arange(r, dtype=torch.int32)
+        t0, nt = off // T, R // T
+        tiles[t0:t0 + nt, 0] = t0
+        tiles[t0:t0 + nt, 1] = t0 + nt - 1
+        off += R
+    t = torch.arange(N // T, dtype=torch.int32)
+    # key tiles a query tile visits (forward, dq) / query tiles a key tile visits (dk, dv): longest first
+    order = torch.stack([torch.argsort(tiles[:, 0] - t, stable=True), torch.argsort(t - tiles[:, 1], stable=True)])
+    order = order.to(torch.int32)
+    if device.type == "cuda":
+        src, tiles, order = (v.pin_memory().to(device, non_blocking=True) for v in (src, tiles, order))
+    return src, _engine.Segments(rows=N, max_len=max(seg_rows), tiles=tiles, order=order)
+
+
+def _ragged_xy(batch: torch.Tensor, src: torch.Tensor, pad_id: int):
+    """(x, y) int64 [N, T] of the packed rows: x = the batch row src[r], y = the row after it, pad_id on gap rows.  Rows a
+    sample does not train on (positions >= its length - 1 as x, >= its length as y) are never read."""
+    B, S1, T = batch.shape
+    if batch.dtype == torch.int16:
+        return _ops.batch_to_xy_packed(batch.contiguous(), src, pad_id)
+    flat = batch.to(torch.long).reshape(B * S1, T)
+    idx = src.long().clamp(min=0)
+    gap = (src < 0)[:, None]
+    return flat[idx].masked_fill(gap, pad_id), flat[idx + 1].masked_fill(gap, pad_id)
+
+
+def _step_xy(batch: torch.Tensor, lengths, device, pad_id: int, what: str):
+    """(x, y, n_seq, S, seg) of a fused step: the padded batch's x = batch[:, :-1], y = batch[:, 1:] as B sequences of S
+    events, or with `lengths` the packed rows of the ragged layout as one sequence of N rows and its `Segments`."""
+    B, S1, T = batch.shape
+    if lengths is None:
+        x, y = _batch_xy(batch)
+        return x, y, B, S1 - 1, None
+    src, seg = _ragged_layout(_ragged_rows(lengths, B, S1 - 1, what), S1, device)
+    x, y = _ragged_xy(batch, src, pad_id)
+    return x, y, 1, seg.rows, seg
+
+
 def _loop_mode(mode: str):
     """B200_GENERATE: "persist" (default: one persistent cooperative kernel per block of events), "graph" (one CUDA-graph
     replay per event), "nograph" (the graph's launches issued from the host), "eager" (host-driven reference-shaped loop)."""
@@ -864,7 +945,7 @@ class MIDIModel(PreTrainedModel):
 
     # ------------------------------------------------------------------ fused training path (non-reference API)
     def training_loss(self, batch: torch.Tensor, backward: bool = True, accumulate: bool = False, grad_ready=None,
-                      sample_idx=None):
+                      sample_idx=None, lengths=None):
         """train.py:168-185 fused: x = batch[:, :-1], y = batch[:, 1:], both stacks, lm_head,
         mean CE with ignore_index=pad -- and, if `backward`, every gradient written to the flat gradient buffer
         (`.grad` of each parameter is a view of it).  Returns a 0-dim fp32 tensor (no host sync).
@@ -873,19 +954,28 @@ class MIDIModel(PreTrainedModel):
         the all-reduce of the first slice while the second is still being computed (midi_b200/ddp.py).
         `sample_idx` (train.py --sample-seq, train.py:172-175): event positions (a Python sequence or a CPU integer
         tensor, distinct, in [-S, S)) kept in every sequence, in the given order; the token-level stack, lm_head and the
-        loss then run on those B * len(sample_idx) events only.  None (the default) runs every event."""
+        loss then run on those B * len(sample_idx) events only.  None (the default) runs every event.
+        `lengths` (a Python sequence or a CPU integer tensor of B values in [0, S+1]: `len(sample)` before the batch was
+        right-padded, midi_b200/data.py) trains every sample on its own events only: sample b's first L_b - 1 positions,
+        the ones with a real target, packed tile-aligned with the other samples' (DESIGN.md 1).  Loss and gradients are the
+        padded step's -- padding rows only ever have ignored targets -- without its work on those rows; events at
+        positions >= L_b are never read.  Not combinable with `sample_idx`.  None (the default) runs the padded batch."""
         rt = self._rt()
         tok = self.tokenizer
         B, S1, T = batch.shape
         S = S1 - 1
         maps = None
+        if lengths is not None and sample_idx is not None:
+            raise _lib.B200Error("training_loss: lengths and sample_idx cannot be combined (sample_idx positions are "
+                                 "defined on the padded batch)")
         if sample_idx is not None:
             maps = _sample_maps(_sample_positions(sample_idx, S), B, S, rt.store.device)
-        x, y = _batch_xy(batch)
+        x, y, n_seq, S_ev, seg = _step_xy(batch, lengths, rt.store.device, tok.pad_id, "training_loss: lengths")
         e = _ops.embed_sum(x, rt.outer.embed)
-        hidden, sv_o = rt.outer.forward(e, B, S, self.net.rotary_emb.inv_freq, save=backward, checkpoint=rt.checkpoint)
+        hidden, sv_o = rt.outer.forward(e, n_seq, S_ev, self.net.rotary_emb.inv_freq, save=backward,
+                                        checkpoint=rt.checkpoint, seg=seg)
         if maps is None:
-            N = B * S
+            N = n_seq * S_ev
             ids_in = y[:, :-1].contiguous()
             xin = _ops.inner_input(hidden, ids_in, rt.inner.embed)
             targets = y.reshape(-1)
@@ -936,20 +1026,20 @@ class MIDIModel(PreTrainedModel):
             rt.store.publish_grads()
         return loss
 
-    def validation_metrics(self, batch: torch.Tensor):
+    def validation_metrics(self, batch: torch.Tensor, lengths=None):
         """train.py:190-206 (validation_step) fused: (val/loss, val/acc) as two 0-dim fp32 device tensors, no host sync.
         The forward saves no activations and the gradient buffer is not touched.  The loss is the mean CE over the
         non-pad targets (what training_loss(batch, backward=False) returns); the accuracy is the share of those targets
-        that are the argmax of their logits row (train.py:153-166).  Both are NaN when no target is a non-pad token."""
+        that are the argmax of their logits row (train.py:153-166).  Both are NaN when no target is a non-pad token.
+        `lengths`: as in training_loss, each sample evaluated on its own events only."""
         rt = self._rt()
         tok = self.tokenizer
-        B, S1, T = batch.shape
-        S = S1 - 1
-        x, y = _batch_xy(batch)
+        T = batch.shape[2]
+        x, y, n_seq, S_ev, seg = _step_xy(batch, lengths, rt.store.device, tok.pad_id, "validation_metrics: lengths")
         e = _ops.embed_sum(x, rt.outer.embed)
-        hidden, _ = rt.outer.forward(e, B, S, self.net.rotary_emb.inv_freq, save=False)
+        hidden, _ = rt.outer.forward(e, n_seq, S_ev, self.net.rotary_emb.inv_freq, save=False, seg=seg)
         xin = _ops.inner_input(hidden, y[:, :-1].contiguous(), rt.inner.embed)
-        hs, _ = rt.inner.forward(xin, B * S, T, self.net_token.rotary_emb.inv_freq, save=False)
+        hs, _ = rt.inner.forward(xin, n_seq * S_ev, T, self.net_token.rotary_emb.inv_freq, save=False)
         del xin, hidden
         logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)
         targets = y.reshape(-1)
