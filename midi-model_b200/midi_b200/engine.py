@@ -192,6 +192,11 @@ class ParamStore:
         self.gflat.zero_()
 
 
+def host_to_device(t: torch.Tensor, device) -> torch.Tensor:
+    """A table built on the host, on `device`: on a GPU the copy is queued from pinned memory without a host sync."""
+    return t.pin_memory().to(device, non_blocking=True) if device.type == "cuda" else t
+
+
 SEG_TILE = 64   # rows per segment tile: the event-level attention's tile height (csrc/attn_wgmma.cu T)
 
 
@@ -205,6 +210,29 @@ class Segments:
     max_len: int
     tiles: torch.Tensor
     order: torch.Tensor
+
+    @staticmethod
+    def pack(rows: List[int], src_stride: int, device):
+        """The packed layout of sequences of rows[b] rows (DESIGN.md 1): sequence b owns a segment of roundup(rows[b], 64)
+        packed rows -- its rows, then gap rows -- and the segments follow in order.  Returns the source-row map (int32 [N]:
+        source row b * src_stride + i of packed row r, -1 for a gap row) and the `Segments`, on `device` (host_to_device)."""
+        T = SEG_TILE
+        seg_rows = [(r + T - 1) // T * T for r in rows]
+        N = sum(seg_rows)
+        src = torch.full((N,), -1, dtype=torch.int32)
+        tiles = torch.empty((N // T, 2), dtype=torch.int32)
+        off = 0
+        for b, (r, R) in enumerate(zip(rows, seg_rows)):
+            src[off:off + r] = b * src_stride + torch.arange(r, dtype=torch.int32)
+            t0, nt = off // T, R // T
+            tiles[t0:t0 + nt, 0] = t0
+            tiles[t0:t0 + nt, 1] = t0 + nt - 1
+            off += R
+        t = torch.arange(N // T, dtype=torch.int32)
+        # key tiles a query tile visits (forward, dq) / query tiles a key tile visits (dk, dv): longest first
+        order = torch.stack([torch.argsort(tiles[:, 0] - t, stable=True), torch.argsort(t - tiles[:, 1], stable=True)])
+        src, tiles, order = (host_to_device(v, device) for v in (src, tiles, order.to(torch.int32)))
+        return src, Segments(rows=N, max_len=max(seg_rows), tiles=tiles, order=order)
 
 
 @dataclass

@@ -27,7 +27,7 @@ import math
 import numbers
 import os
 import threading
-from typing import Any, Dict, Optional, Union
+from typing import Any, Dict, NamedTuple, Optional, Union
 
 import numpy as np
 import torch
@@ -350,36 +350,30 @@ def _inner_backward(rt, model, sv, hs, dlogits, ids, N, L, n_ids, has_hidden, g,
     return (dhidden,)
 
 
-def _batch_xy(batch: torch.Tensor):
-    """train.py:169-170 on a (B, S+1, T) batch: x = batch[:, :-1], y = batch[:, 1:] as int64 [B*S, T]."""
-    B, S1, T = batch.shape
-    if batch.dtype == torch.int16:
-        return _ops.batch_to_xy(batch.contiguous())        # int16 host data path (midi_b200/data.py): one widening pass
-    batch = batch.to(torch.long)
-    return batch[:, :-1].contiguous().view(B * (S1 - 1), T), batch[:, 1:].contiguous().view(B * (S1 - 1), T)
-
-
-def _sample_positions(sample_idx, S: int) -> list:
-    """The event positions of train.py --sample-seq (train.py:173: `[-1] + random.sample(range(S - 2), k)`) as distinct
-    ints in [0, S); negative positions count from the end, as Python indexing does."""
-    what = "training_loss: sample_idx"
-    if isinstance(sample_idx, torch.Tensor):
-        if sample_idx.device.type != "cpu":
-            raise _lib.B200Error(f"{what} must be a CPU tensor or a Python sequence (checking a device index would need a "
+def _host_ints(value, what: str) -> list:
+    """`value` -- a Python sequence or a CPU integer tensor, 1-D -- as a list of ints; a device tensor is refused, since
+    checking its values would need a host sync."""
+    if isinstance(value, torch.Tensor):
+        if value.device.type != "cpu":
+            raise _lib.B200Error(f"{what} must be a CPU tensor or a Python sequence (checking device values would need a "
                                  "host sync)")
-        if sample_idx.dtype == torch.bool or sample_idx.is_floating_point() or sample_idx.is_complex():
-            raise _lib.B200Error(f"{what} must hold integers, got {sample_idx.dtype}")
-        if sample_idx.dim() != 1:
-            raise _lib.B200Error(f"{what} must be 1-D, got shape {tuple(sample_idx.shape)}")
-        vals = sample_idx.tolist()
-    elif isinstance(sample_idx, collections.abc.Sequence) and not isinstance(sample_idx, (str, bytes)):
-        vals = list(sample_idx)
-        bad = [v for v in vals if isinstance(v, bool) or not isinstance(v, numbers.Integral)]
+        if value.dtype == torch.bool or value.is_floating_point() or value.is_complex():
+            raise _lib.B200Error(f"{what} must hold integers, got {value.dtype}")
+        if value.dim() != 1:
+            raise _lib.B200Error(f"{what} must be 1-D, got shape {tuple(value.shape)}")
+        return value.tolist()
+    if isinstance(value, collections.abc.Sequence) and not isinstance(value, (str, bytes)):
+        bad = [v for v in value if isinstance(v, bool) or not isinstance(v, numbers.Integral)]
         if bad:
             raise _lib.B200Error(f"{what} must be a 1-D sequence of integers, got {bad[0]!r}")
-        vals = [int(v) for v in vals]
-    else:
-        raise _lib.B200Error(f"{what} must be a Python sequence or a CPU integer tensor, got {type(sample_idx).__name__}")
+        return [int(v) for v in value]
+    raise _lib.B200Error(f"{what} must be a Python sequence or a CPU integer tensor, got {type(value).__name__}")
+
+
+def _sample_positions(sample_idx, S: int, what: str) -> list:
+    """The event positions of train.py --sample-seq (train.py:173: `[-1] + random.sample(range(S - 2), k)`) as distinct
+    ints in [0, S); negative positions count from the end, as Python indexing does."""
+    vals = _host_ints(sample_idx, what)
     if not vals:
         raise _lib.B200Error(f"{what} is empty")
     out_of_range = [v for v in vals if not -S <= v < S]
@@ -391,38 +385,10 @@ def _sample_positions(sample_idx, S: int) -> list:
     return vals
 
 
-def _sample_maps(positions: list, B: int, S: int, device):
-    """Row map rows[b*K + j] = b*S + positions[j] (the row order of hidden[:, idx].reshape(-1, H)) and its inverse over the
-    B*S event rows (-1 = not selected), as int32 device tensors; the copies are queued without a host sync."""
-    idx = torch.tensor(positions, dtype=torch.int32)
-    rows = (torch.arange(B, dtype=torch.int32)[:, None] * S + idx[None, :]).reshape(-1)
-    inv = torch.full((B * S,), -1, dtype=torch.int32)
-    inv[rows.long()] = torch.arange(rows.numel(), dtype=torch.int32)
-    if device.type == "cuda":
-        return rows.pin_memory().to(device, non_blocking=True), inv.pin_memory().to(device, non_blocking=True)
-    return rows, inv
-
-
 def _ragged_rows(lengths, B: int, S: int, what: str) -> list:
     """Event rows each sample trains on, from `lengths` (the number of real events of every sample of a [B, S+1, T]
     batch, in [0, S+1]): S_b = L_b - 1 positions have a real target, a sample with L_b <= 1 has none."""
-    if isinstance(lengths, torch.Tensor):
-        if lengths.device.type != "cpu":
-            raise _lib.B200Error(f"{what} must be a CPU tensor or a Python sequence (checking device lengths would need a "
-                                 "host sync)")
-        if lengths.dtype == torch.bool or lengths.is_floating_point() or lengths.is_complex():
-            raise _lib.B200Error(f"{what} must hold integers, got {lengths.dtype}")
-        if lengths.dim() != 1:
-            raise _lib.B200Error(f"{what} must be 1-D, got shape {tuple(lengths.shape)}")
-        vals = lengths.tolist()
-    elif isinstance(lengths, collections.abc.Sequence) and not isinstance(lengths, (str, bytes)):
-        vals = list(lengths)
-        bad = [v for v in vals if isinstance(v, bool) or not isinstance(v, numbers.Integral)]
-        if bad:
-            raise _lib.B200Error(f"{what} must be a 1-D sequence of integers, got {bad[0]!r}")
-        vals = [int(v) for v in vals]
-    else:
-        raise _lib.B200Error(f"{what} must be a Python sequence or a CPU integer tensor, got {type(lengths).__name__}")
+    vals = _host_ints(lengths, what)
     if len(vals) != B:
         raise _lib.B200Error(f"{what} has {len(vals)} entries for a batch of {B} samples")
     out_of_range = [v for v in vals if not 0 <= v <= S + 1]
@@ -434,54 +400,61 @@ def _ragged_rows(lengths, B: int, S: int, what: str) -> list:
     return rows
 
 
-def _ragged_layout(rows: list, S1: int, device):
-    """Tile-aligned packing of B ragged sequences (DESIGN.md 1): sequence b owns a segment of roundup(rows[b], 64) packed
-    rows -- its rows 0 .. rows[b]-1, then gap rows -- and the segments follow in batch order.  Returns the source-row map
-    (int32 [N]: batch row b * S1 + i of packed row r, -1 for a gap row) and the engine's `Segments` (tile table and
-    longest-first tile orders), copied to `device` without a host sync."""
-    T = _engine.SEG_TILE
-    seg_rows = [(r + T - 1) // T * T for r in rows]
-    N = sum(seg_rows)
-    src = torch.full((N,), -1, dtype=torch.int32)
-    tiles = torch.empty((N // T, 2), dtype=torch.int32)
-    off = 0
-    for b, (r, R) in enumerate(zip(rows, seg_rows)):
-        src[off:off + r] = b * S1 + torch.arange(r, dtype=torch.int32)
-        t0, nt = off // T, R // T
-        tiles[t0:t0 + nt, 0] = t0
-        tiles[t0:t0 + nt, 1] = t0 + nt - 1
-        off += R
-    t = torch.arange(N // T, dtype=torch.int32)
-    # key tiles a query tile visits (forward, dq) / query tiles a key tile visits (dk, dv): longest first
-    order = torch.stack([torch.argsort(tiles[:, 0] - t, stable=True), torch.argsort(t - tiles[:, 1], stable=True)])
-    order = order.to(torch.int32)
-    if device.type == "cuda":
-        src, tiles, order = (v.pin_memory().to(device, non_blocking=True) for v in (src, tiles, order))
-    return src, _engine.Segments(rows=N, max_len=max(seg_rows), tiles=tiles, order=order)
+_ragged_layout = _engine.Segments.pack      # (src, Segments) of a ragged batch's packed rows (DESIGN.md 1)
 
 
-def _ragged_xy(batch: torch.Tensor, src: torch.Tensor, pad_id: int):
-    """(x, y) int64 [N, T] of the packed rows: x = the batch row src[r], y = the row after it, pad_id on gap rows.  Rows a
-    sample does not train on (positions >= its length - 1 as x, >= its length as y) are never read."""
+class _StepRows(NamedTuple):
+    """The rows of one fused step.  x, y: int64 [n_seq * S, T] inputs and targets of the event-level stack: n_seq
+    sequences of S events, or with `seg` one sequence of seg.rows segment-packed rows.  rows, inv: the event row of each
+    token-level sequence j (int32 device [N]) and its inverse (int32 device [n_seq * S]: j, or -1 for an unselected row);
+    both None when every event row feeds the token-level stack."""
+    x: torch.Tensor
+    y: torch.Tensor
+    n_seq: int
+    S: int
+    seg: Optional[_engine.Segments]
+    rows: Optional[torch.Tensor]
+    inv: Optional[torch.Tensor]
+
+    @property
+    def n_tok(self) -> int:                          # number of token-level sequences
+        return self.n_seq * self.S if self.rows is None else self.rows.shape[0]
+
+
+def _step_rows(batch: torch.Tensor, sample_idx, lengths, device, pad_id: int, what: str) -> _StepRows:
+    """train.py:169-175 on a (B, S+1, T) batch: x = batch[:, :-1], y = batch[:, 1:], every event row or those `sample_idx`
+    selects (in order, per sequence) feeding the token-level stack; with `lengths`, the packed rows of the ragged layout
+    (x = batch row src[r], y = the row after it, pad_id on gap rows), which never read a row a sample does not train on.
+    Host tables reach `device` without a host sync."""
     B, S1, T = batch.shape
+    S = S1 - 1
+    if lengths is not None and sample_idx is not None:
+        raise _lib.B200Error(f"{what}: lengths and sample_idx cannot be combined (sample_idx positions are defined on the "
+                             "padded batch)")
+    if lengths is not None:
+        src, seg = _ragged_layout(_ragged_rows(lengths, B, S, f"{what}: lengths"), S1, device)
+        if batch.dtype == torch.int16:
+            x, y = _ops.batch_to_xy_packed(batch.contiguous(), src, pad_id)
+        else:
+            flat = batch.to(torch.long).reshape(B * S1, T)
+            idx = src.long().clamp(min=0)
+            gap = (src < 0)[:, None]
+            x, y = flat[idx].masked_fill(gap, pad_id), flat[idx + 1].masked_fill(gap, pad_id)
+        return _StepRows(x, y, 1, seg.rows, seg, None, None)
+    rows = inv = None
+    if sample_idx is not None:
+        # rows[b*K + j] = b*S + positions[j]: the row order of hidden[:, idx].reshape(-1, H)
+        idx = torch.tensor(_sample_positions(sample_idx, S, f"{what}: sample_idx"), dtype=torch.int32)
+        rows = (torch.arange(B, dtype=torch.int32)[:, None] * S + idx[None, :]).reshape(-1)
+        inv = torch.full((B * S,), -1, dtype=torch.int32)
+        inv[rows.long()] = torch.arange(rows.numel(), dtype=torch.int32)
+        rows, inv = _engine.host_to_device(rows, device), _engine.host_to_device(inv, device)
     if batch.dtype == torch.int16:
-        return _ops.batch_to_xy_packed(batch.contiguous(), src, pad_id)
-    flat = batch.to(torch.long).reshape(B * S1, T)
-    idx = src.long().clamp(min=0)
-    gap = (src < 0)[:, None]
-    return flat[idx].masked_fill(gap, pad_id), flat[idx + 1].masked_fill(gap, pad_id)
-
-
-def _step_xy(batch: torch.Tensor, lengths, device, pad_id: int, what: str):
-    """(x, y, n_seq, S, seg) of a fused step: the padded batch's x = batch[:, :-1], y = batch[:, 1:] as B sequences of S
-    events, or with `lengths` the packed rows of the ragged layout as one sequence of N rows and its `Segments`."""
-    B, S1, T = batch.shape
-    if lengths is None:
-        x, y = _batch_xy(batch)
-        return x, y, B, S1 - 1, None
-    src, seg = _ragged_layout(_ragged_rows(lengths, B, S1 - 1, what), S1, device)
-    x, y = _ragged_xy(batch, src, pad_id)
-    return x, y, 1, seg.rows, seg
+        x, y = _ops.batch_to_xy(batch.contiguous())        # int16 host data path (midi_b200/data.py): one widening pass
+    else:
+        batch = batch.to(torch.long)
+        x, y = batch[:, :-1].contiguous().view(B * S, T), batch[:, 1:].contiguous().view(B * S, T)
+    return _StepRows(x, y, B, S, None, rows, inv)
 
 
 def _loop_mode(mode: str):
@@ -962,39 +935,17 @@ class MIDIModel(PreTrainedModel):
         positions >= L_b are never read.  Not combinable with `sample_idx`.  None (the default) runs the padded batch."""
         rt = self._rt()
         tok = self.tokenizer
-        B, S1, T = batch.shape
-        S = S1 - 1
-        maps = None
-        if lengths is not None and sample_idx is not None:
-            raise _lib.B200Error("training_loss: lengths and sample_idx cannot be combined (sample_idx positions are "
-                                 "defined on the padded batch)")
-        if sample_idx is not None:
-            maps = _sample_maps(_sample_positions(sample_idx, S), B, S, rt.store.device)
-        x, y, n_seq, S_ev, seg = _step_xy(batch, lengths, rt.store.device, tok.pad_id, "training_loss: lengths")
-        e = _ops.embed_sum(x, rt.outer.embed)
-        hidden, sv_o = rt.outer.forward(e, n_seq, S_ev, self.net.rotary_emb.inv_freq, save=backward,
-                                        checkpoint=rt.checkpoint, seg=seg)
-        if maps is None:
-            N = n_seq * S_ev
-            ids_in = y[:, :-1].contiguous()
-            xin = _ops.inner_input(hidden, ids_in, rt.inner.embed)
-            targets = y.reshape(-1)
-        else:
-            N = maps[0].shape[0]
-            xin, y_sel = _ops.inner_input_rows(hidden, y, maps[0], rt.inner.embed)
-            ids_in = y_sel[:, :-1].contiguous()
-            targets = y_sel.view(-1)
-        hs, sv_i = rt.inner.forward(xin, N, T, self.net_token.rotary_emb.inv_freq, save=backward,
-                                    checkpoint=rt.checkpoint)
-        del xin
-        logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)
+        T = batch.shape[2]
+        st = _step_rows(batch, sample_idx, lengths, rt.store.device, tok.pad_id, "training_loss")
+        # (`hidden` is not read again; the step holds it until it returns, like every tensor of its forward)
+        logits, targets, hidden, hs, ids_in, sv_o, sv_i = self._step_forward(rt, st, save=backward)
         lac, lse = _ops.ce_fwd(logits, targets, rt.V, tok.pad_id)
         loss = lac[0]
         if backward:
             _ops.ce_bwd_(logits, targets, lse, lac, rt.V, tok.pad_id, 1.0)
             g_i, g_o = rt.inner.main_grads, rt.outer.main_grads
-            dhidden, = _inner_backward(rt, self, sv_i, hs, logits, ids_in, N, T, T - 1, True, g_i, rt.g_lm_head,
-                                       accumulate, hidden_rows=None if maps is None else maps[1])
+            dhidden, = _inner_backward(rt, self, sv_i, hs, logits, ids_in, st.n_tok, T, T - 1, True, g_i, rt.g_lm_head,
+                                       accumulate, hidden_rows=st.inv)
             del logits, hs
             # Gradient hand-over to a data-parallel trainer.  Base parameters that train (full training): slices of the flat
             # buffer as backward finishes them.  Adapter matrices (LoRA, train.py:439-449) sit in the tail
@@ -1017,7 +968,7 @@ class MIDIModel(PreTrainedModel):
                         hi[0] = lo
             de = rt.outer.backward(sv_o, dhidden, g_o, accumulate=accumulate, layer_done=layer_done)
             if g_o.embed is not None:
-                _ops.embed_bwd(x.view(-1), de, g_o.embed, per_row=T, row_stride=1, row_inner=0, row_off=0,
+                _ops.embed_bwd(st.x.view(-1), de, g_o.embed, per_row=T, row_stride=1, row_inner=0, row_off=0,
                                pad_id=self.config.net_config.pad_token_id, accumulate=accumulate)
             if base_sync:
                 grad_ready(0, hi[0])          # embedding table (+ whatever is left)
@@ -1034,19 +985,37 @@ class MIDIModel(PreTrainedModel):
         `lengths`: as in training_loss, each sample evaluated on its own events only."""
         rt = self._rt()
         tok = self.tokenizer
-        T = batch.shape[2]
-        x, y, n_seq, S_ev, seg = _step_xy(batch, lengths, rt.store.device, tok.pad_id, "validation_metrics: lengths")
-        e = _ops.embed_sum(x, rt.outer.embed)
-        hidden, _ = rt.outer.forward(e, n_seq, S_ev, self.net.rotary_emb.inv_freq, save=False, seg=seg)
-        xin = _ops.inner_input(hidden, y[:, :-1].contiguous(), rt.inner.embed)
-        hs, _ = rt.inner.forward(xin, n_seq * S_ev, T, self.net_token.rotary_emb.inv_freq, save=False)
-        del xin, hidden
-        logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)
-        targets = y.reshape(-1)
+        st = _step_rows(batch, None, lengths, rt.store.device, tok.pad_id, "validation_metrics")
+        logits, targets, *_ = self._step_forward(rt, st, save=False)
         lac, _ = _ops.ce_fwd(logits, targets, rt.V, tok.pad_id)
         hits = _ops.argmax_hits(logits, targets, rt.V, tok.pad_id)
         loss = torch.where(lac[1] > 0, lac[0], float("nan"))
         return loss, hits[0] / hits[1]
+
+    def _step_forward(self, rt: _Runtime, st: _StepRows, save: bool):
+        """A fused step's forward over the rows `st` describes: embed-sum, event-level stack, token-level input of every
+        event row or of the rows st.rows selects, token-level stack, lm_head.  Returns (logits [st.n_tok * T, pitch],
+        targets, hidden, hs, ids_in, sv_o, sv_i): both stacks' outputs and saved activations (None with save=False) and
+        the token-level input ids, for the backward; with save=False `hidden` is freed before lm_head and is None."""
+        T = st.x.shape[1]
+        e = _ops.embed_sum(st.x, rt.outer.embed)
+        hidden, sv_o = rt.outer.forward(e, st.n_seq, st.S, self.net.rotary_emb.inv_freq, save=save,
+                                        checkpoint=rt.checkpoint, seg=st.seg)
+        if st.rows is None:
+            ids_in = st.y[:, :-1].contiguous()
+            xin = _ops.inner_input(hidden, ids_in, rt.inner.embed)
+            targets = st.y.reshape(-1)
+        else:
+            xin, y_sel = _ops.inner_input_rows(hidden, st.y, st.rows, rt.inner.embed)
+            ids_in = y_sel[:, :-1].contiguous()
+            targets = y_sel.view(-1)
+        hs, sv_i = rt.inner.forward(xin, st.n_tok, T, self.net_token.rotary_emb.inv_freq, save=save,
+                                    checkpoint=rt.checkpoint)
+        del xin
+        if not save:
+            hidden = None
+        logits = _ops.linear(hs, rt.lm_head, pitch=rt.pitch)
+        return logits, targets, hidden, hs, ids_in, sv_o, sv_i
 
     def _opt_state(self, rt):
         """AdamW moments (fp32) over the trainable span of the flat parameter buffer -- everything in full training, the

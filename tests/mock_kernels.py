@@ -47,10 +47,34 @@ def inner_input(hidden, ids, table):
     return x.reshape(-1, table.shape[1]).contiguous()
 
 
+def inner_input_rows(hidden, y, rows, table):
+    y_sel = y[rows.long()]
+    return inner_input(hidden[rows.long()], y_sel[:, :-1], table), y_sel.clone()
+
+
+def inner_input_rows_bwd_hidden(dx, inv, n_events, Tin):
+    H = dx.shape[1]
+    out = torch.zeros((inv.shape[0], H), dtype=BF)
+    sel = inv >= 0
+    out[sel] = dx.view(n_events, Tin, H)[:, 0][inv[sel].long()]
+    return out
+
+
 def batch_to_xy(batch):
     b = batch.to(torch.long)
     B, S1, T = b.shape
     return b[:, :-1].reshape(B * (S1 - 1), T).contiguous(), b[:, 1:].reshape(B * (S1 - 1), T).contiguous()
+
+
+def batch_to_xy_packed(batch, src, pad_id):
+    B, S1, T = batch.shape
+    flat = batch.to(torch.long).reshape(B * S1, T)
+    idx = src.long()
+    x = torch.full((idx.numel(), T), pad_id, dtype=torch.long)
+    y = x.clone()
+    live = idx >= 0
+    x[live], y[live] = flat[idx[live]], flat[idx[live] + 1]
+    return x, y
 
 
 def embed_bwd(ids, dout, dtable, per_row, row_stride, row_inner, row_off, pad_id, accumulate):
@@ -118,6 +142,17 @@ def rope_qk_(qkv, cos, sin, S, H, D, backward=False, pos0=0, pos0_dev=None):
         qkv[:, col0:col0 + H] = _rot(blk, c, s, backward).reshape(rows, H).to(BF)
 
 
+def _segments(tiles):
+    """[(row0, rows)] of the segments a {first, last} tile table describes."""
+    firsts = sorted(set(tiles[:, 0].tolist()))
+    return [(64 * f, 64 * (int(tiles[f, 1]) + 1 - f)) for f in firsts]
+
+
+def rope_qk_seg_(qkv, cos, sin, tiles, H, D, backward=False):
+    for r0, n in _segments(tiles):
+        rope_qk_(qkv[r0:r0 + n], cos, sin, n, H, D, backward=backward)
+
+
 def _silu(g):
     return g * torch.sigmoid(g)
 
@@ -179,6 +214,12 @@ def linear_rope(x, w_qkv, cos, sin, S, D):
     return qkv
 
 
+def linear_rope_seg(x, w_qkv, cos, sin, tiles, D):
+    qkv = gemm(x, w_qkv, x.shape[0], w_qkv.shape[0], x.shape[1], lda=x.stride(0), ldb=w_qkv.stride(0))
+    rope_qk_seg_(qkv, cos, sin, tiles, w_qkv.shape[0] // 3, D)
+    return qkv
+
+
 # ------------------------------------------------------------------ attention
 def _split(qkv, n_seq, S, nh, D):
     H = nh * D
@@ -222,6 +263,20 @@ def attn_causal_bwd(qkv, out, dout, lse, B, S, n_heads, D, rope=None, impl=None)
     return _attn_bwd(qkv, dout, B, S, n_heads, D, rope)
 
 
+def attn_causal_fwd_seg(qkv, tiles, order, n_heads, D, want_lse, impl=None):
+    outs, lses = [], []
+    for r0, n in _segments(tiles):
+        o, lse = attn_causal_fwd(qkv[r0:r0 + n], 1, n, n_heads, D, True)
+        outs.append(o)
+        lses.append(lse[0])
+    return torch.cat(outs), (torch.cat(lses, 1) if want_lse else None)
+
+
+def attn_causal_bwd_seg(qkv, out, dout, lse, tiles, order, n_heads, D, rope=None, impl=None):
+    return torch.cat([attn_causal_bwd(qkv[r0:r0 + n], out[r0:r0 + n], dout[r0:r0 + n], None, 1, n, n_heads, D, rope=rope)
+                      for r0, n in _segments(tiles)])
+
+
 def attn_tiny_fwd(qkv, n_events, L, n_heads, D, rope=None):
     if rope is not None:
         rope_qk_(qkv, rope[0], rope[1], L, n_heads * D, D)          # the kernel rotates q, k in place
@@ -243,6 +298,12 @@ def ce_fwd(logits, targets, V, ignore_index):
     cnt = keep.sum().float()
     loss = (row * keep).sum() / cnt
     return torch.stack([loss, cnt]).float(), lse
+
+
+def argmax_hits(logits, targets, V, ignore_index):
+    am = logits[:, :V].float().argmax(-1)
+    live = (targets != ignore_index) & (targets >= 0) & (targets < V)
+    return torch.stack([(live & (am == targets)).sum(), live.sum()]).float()
 
 
 def ce_bwd_(logits, targets, lse, lac, V, ignore_index, grad_scale=1.0, grad_scale_dev=None):
@@ -442,13 +503,18 @@ def _query(name, *args):
     raise AssertionError(f"mock kernel layer: unexpected C-ABI query {name}")
 
 
+# the `midi_b200.ops` wrappers the host code calls, each replaced by the stand-in of the same name above
+OPS = ("embed_sum", "inner_input", "inner_input_rows", "inner_input_rows_bwd_hidden", "batch_to_xy", "batch_to_xy_packed",
+       "embed_bwd", "rmsnorm", "add_rmsnorm", "rmsnorm_bwd", "rope_table", "rope_qk_", "rope_qk_seg_", "swiglu", "swiglu_bwd",
+       "scale", "gemm", "linear_swiglu", "linear_rope", "linear_rope_seg", "attn_causal_fwd", "attn_causal_bwd",
+       "attn_causal_fwd_seg", "attn_causal_bwd_seg", "attn_tiny_fwd", "attn_tiny_bwd", "ce_fwd", "argmax_hits", "ce_bwd_")
+
+
 def install(monkeypatch):
     """Route the host code's kernel calls to the CPU stand-ins above for the duration of one test."""
     from midi_b200 import engine, lib, ops
     g = globals()
-    for name in ("embed_sum", "inner_input", "batch_to_xy", "embed_bwd", "rmsnorm", "add_rmsnorm", "rmsnorm_bwd", "rope_table",
-                 "rope_qk_", "swiglu", "swiglu_bwd", "scale", "gemm", "linear_swiglu", "linear_rope", "attn_causal_fwd",
-                 "attn_causal_bwd", "attn_tiny_fwd", "attn_tiny_bwd", "ce_fwd", "ce_bwd_"):
+    for name in OPS:
         monkeypatch.setattr(ops, name, g[name])
     monkeypatch.setattr(ops, "_ws", lambda key, nbytes, device, zero=False: torch.zeros(max(nbytes, 256), dtype=torch.uint8))
     monkeypatch.setattr(ops, "GEMM_PROFILE", None)
@@ -467,3 +533,17 @@ def install(monkeypatch):
     monkeypatch.setattr(torch.cuda, "Stream", _NoStream)
     monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: _NoStream())
     monkeypatch.setattr(torch.cuda, "stream", lambda s: contextlib.nullcontext())
+
+
+def trace(monkeypatch, fn, names=None):
+    """fn() with every wrapper of OPS and every raw C-ABI call recorded by name, in call order, into `names` (a new list
+    by default), which is returned.  Use inside a `monkeypatch.context()`: the recording stays patched in until it ends."""
+    from midi_b200 import lib, ops
+    names = [] if names is None else names
+    for name in OPS:
+        f = getattr(ops, name)
+        monkeypatch.setattr(ops, name, lambda *a, _f=f, _n=name, **k: (names.append(_n), _f(*a, **k))[1])
+    call = lib.call
+    monkeypatch.setattr(lib, "call", lambda n, *a: (names.append(n), call(n, *a))[1])
+    fn()
+    return names

@@ -7,33 +7,20 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import host_model
 import mock_kernels
-
-BF = torch.bfloat16
-TARGETS = ["q_proj", "o_proj", "k_proj", "v_proj", "gate_proj", "up_proj", "down_proj"]      # train.py:443
+from host_model import BF, TARGETS, oracle_padded as _oracle_grads
 
 
 def _tiny_model(seed=0):
     import midi_model as mm
-    torch.manual_seed(seed)
-    cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=4, n_embd=256, n_inner=512)
-    return mm, cfg, mm.MIDIModel(cfg).to(BF).train()
+    model = host_model.tiny_model(seed)
+    return mm, model.config, model
 
 
 def _batch(model, B=2, S1=6, seed=1):
     from midi_b200.synth import synth_batch
     return synth_batch(model.tokenizer, B, S1, seed=seed)
-
-
-def _oracle_grads(model, batch, lora_scale=None):
-    """Loss and gradients from the oracle (fp32 autograd over the bf16-rounded weights).  With adapters: the effective
-    weight W + scale * B A is formed differentiably, so the gradients of A and B are those of peft's unmerged forward."""
-    from oracle import midi_oracle as O
-    leaf = {n: p.detach().float().requires_grad_(True) for n, p in model.named_parameters()}
-    sd = O.lora_effective_sd(leaf, lora_scale) if lora_scale is not None else leaf
-    loss = O.train_loss(sd, O.cfg_from_hf(model.config), batch)
-    loss.backward()
-    return float(loss.detach()), {n: t.grad for n, t in leaf.items()}
 
 
 def _stream(model, **kw):
@@ -60,19 +47,10 @@ def test_engine_schedule_matches_oracle_autograd(monkeypatch):
     assert rt.store.base_numel == rt.store.numel and rt.store.train_dense and (rt.store.train_lo, rt.store.train_hi) == (0, rt.store.numel)
 
 
-def _lora_model(monkeypatch, r=8, alpha=16, seed=0):
-    from midi_b200 import lora
+def _lora_model(monkeypatch):
     mock_kernels.install(monkeypatch)
-    mm, cfg, model = _tiny_model(seed)
-    model.requires_grad_(False)                                              # train.py:440
-    model.add_adapter(lora.LoraAdapterConfig(r=r, lora_alpha=alpha, target_modules=TARGETS, lora_dropout=0, bias="none",
-                                             task_type="CAUSAL_LM"))          # train.py:441-449
-    g = torch.Generator().manual_seed(5)
-    with torch.no_grad():                                                    # B = 0 at init would zero dA: make it non-trivial
-        for n, p in model.named_parameters():
-            if ".lora_B." in n:
-                p.copy_((torch.randn(p.shape, generator=g) * 0.02).to(BF))
-    return mm, model
+    mm, cfg, model = _tiny_model()
+    return mm, host_model.add_lora(model)
 
 
 def test_lora_container_layout_and_flat_store(monkeypatch):

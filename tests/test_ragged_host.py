@@ -1,130 +1,19 @@
 """Host logic of the fused trainer's ragged batches (`training_loss(batch, lengths=...)`, `validation_metrics(batch,
-lengths)`) on CPU, over the mock kernel layer (tests/mock_kernels.py) plus stand-ins for the entry points they add,
-compared with the oracle's autograd of the padded step.  The kernels themselves are checked on the GPU
-(tests/test_gpu_ragged.py)."""
+lengths)`) on CPU, over the mock kernel layer (tests/mock_kernels.py), compared with the oracle's autograd of the padded
+step.  The kernels themselves are checked on the GPU (tests/test_gpu_ragged.py)."""
 import pytest
 import torch
 
-import mock_kernels
-
-BF = torch.bfloat16
-TARGETS = ["q_proj", "o_proj", "k_proj", "v_proj", "gate_proj", "up_proj", "down_proj"]      # train.py:443
-
-
-# ------------------------------------------------------------------ stand-ins for the new wrappers (midi_b200.ops)
-def batch_to_xy_packed(batch, src, pad_id):
-    B, S1, T = batch.shape
-    flat = batch.to(torch.long).reshape(B * S1, T)
-    idx = src.long()
-    x = torch.full((idx.numel(), T), pad_id, dtype=torch.long)
-    y = x.clone()
-    live = idx >= 0
-    x[live], y[live] = flat[idx[live]], flat[idx[live] + 1]
-    return x, y
-
-
-def _segments(tiles):
-    """[(row0, rows)] of the segments a {first, last} tile table describes."""
-    firsts = sorted(set(tiles[:, 0].tolist()))
-    return [(64 * f, 64 * (int(tiles[f, 1]) + 1 - f)) for f in firsts]
-
-
-def rope_qk_seg_(qkv, cos, sin, tiles, H, D, backward=False):
-    for r0, n in _segments(tiles):
-        blk = qkv[r0:r0 + n]
-        mock_kernels.rope_qk_(blk, cos, sin, n, H, D, backward=backward)
-
-
-def linear_rope_seg(x, w_qkv, cos, sin, tiles, D):
-    qkv = mock_kernels.gemm(x, w_qkv, x.shape[0], w_qkv.shape[0], x.shape[1], lda=x.stride(0), ldb=w_qkv.stride(0))
-    rope_qk_seg_(qkv, cos, sin, tiles, w_qkv.shape[0] // 3, D)
-    return qkv
-
-
-def attn_causal_fwd_seg(qkv, tiles, order, n_heads, D, want_lse, impl=None):
-    outs, lses = [], []
-    for r0, n in _segments(tiles):
-        o, lse = mock_kernels.attn_causal_fwd(qkv[r0:r0 + n], 1, n, n_heads, D, True)
-        outs.append(o)
-        lses.append(lse[0])
-    return torch.cat(outs), (torch.cat(lses, 1) if want_lse else None)
-
-
-def attn_causal_bwd_seg(qkv, out, dout, lse, tiles, order, n_heads, D, rope=None, impl=None):
-    return torch.cat([mock_kernels.attn_causal_bwd(qkv[r0:r0 + n], out[r0:r0 + n], dout[r0:r0 + n], None, 1, n, n_heads, D,
-                                                   rope=rope) for r0, n in _segments(tiles)])
-
-
-def argmax_hits(logits, targets, V, ignore_index):
-    am = logits[:, :V].float().argmax(-1)
-    live = (targets != ignore_index) & (targets >= 0) & (targets < V)
-    return torch.stack([(live & (am == targets)).sum(), live.sum()]).float()
-
-
-NEW = ("batch_to_xy_packed", "rope_qk_seg_", "linear_rope_seg", "attn_causal_fwd_seg", "attn_causal_bwd_seg", "argmax_hits")
-
-
-def install(monkeypatch):
-    from midi_b200 import ops
-    mock_kernels.install(monkeypatch)
-    for name in NEW:
-        monkeypatch.setattr(ops, name, globals()[name])
-
-
-# ------------------------------------------------------------------ helpers
-def _tiny_model(seed=0):
-    import midi_model as mm
-    torch.manual_seed(seed)
-    cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=4, n_embd=256, n_inner=512)
-    return mm.MIDIModel(cfg).to(BF).train()
+from host_model import BF, add_lora, global_rel as _global_rel, grads as _grads, make_batch, \
+    oracle_padded as _oracle_padded, tiny_model as _tiny_model
+from mock_kernels import install, trace as _trace
 
 
 def _batch(model, lengths, S1, seed=1):
-    """A right-padded batch (train.py:86-90 collate_fn): sample b holds lengths[b] events, then pad_id."""
-    from midi_b200.synth import synth_batch
-    b = synth_batch(model.tokenizer, len(lengths), S1, seed=seed)
-    for i, L in enumerate(lengths):
-        b[i, L:] = model.tokenizer.pad_id
-    return b
-
-
-def _grads(model):
-    return {n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None}
-
-
-def _oracle_padded(model, batch, lora_scale=None):
-    """train.py:169-185 on the padded batch under the oracle's fp32 autograd."""
-    from oracle import midi_oracle as O
-    leaf = {n: p.detach().float().requires_grad_(True) for n, p in model.named_parameters()}
-    sd = O.lora_effective_sd(leaf, lora_scale) if lora_scale is not None else leaf
-    loss = O.train_loss(sd, O.cfg_from_hf(model.config), batch)
-    loss.backward()
-    return float(loss.detach()), {n: t.grad for n, t in leaf.items() if t.grad is not None}
-
-
-def _global_rel(got, ref):
-    num = sum(float((got[n].double() - ref[n].double()).pow(2).sum()) for n in ref)
-    den = sum(float(ref[n].double().pow(2).sum()) for n in ref)
-    return (num / den) ** 0.5
+    return make_batch(model, S1=S1, seed=seed, lengths=lengths)
 
 
 LENGTHS = [70, 66, 10, 1]          # 69, 65, 9 and 0 trained rows -> segments of 128, 128 and 64 rows
-
-
-def _trace(monkeypatch, fn):
-    """Names of the kernel-layer calls `fn` issues (ops wrappers and raw C-ABI calls), in order."""
-    from midi_b200 import lib, ops
-    names = []
-    for name in ("embed_sum", "inner_input", "batch_to_xy", "embed_bwd", "rmsnorm", "add_rmsnorm", "rmsnorm_bwd",
-                 "rope_table", "rope_qk_", "swiglu", "swiglu_bwd", "scale", "gemm", "linear_swiglu", "linear_rope",
-                 "attn_causal_fwd", "attn_causal_bwd", "attn_tiny_fwd", "attn_tiny_bwd", "ce_fwd", "ce_bwd_") + NEW:
-        f = getattr(ops, name)
-        monkeypatch.setattr(ops, name, lambda *a, _f=f, _n=name, **k: (names.append(_n), _f(*a, **k))[1])
-    call = lib.call
-    monkeypatch.setattr(lib, "call", lambda n, *a: (names.append(n), call(n, *a))[1])
-    fn()
-    monkeypatch.setattr(lib, "call", call)
-    return names
 
 
 # ------------------------------------------------------------------ tests
@@ -163,17 +52,8 @@ def test_ragged_step_rope_settings(monkeypatch, fuse):
 
 
 def test_ragged_step_lora(monkeypatch):
-    from midi_b200 import lora
     install(monkeypatch)
-    model = _tiny_model()
-    model.requires_grad_(False)
-    model.add_adapter(lora.LoraAdapterConfig(r=8, lora_alpha=16, target_modules=TARGETS, lora_dropout=0, bias="none",
-                                             task_type="CAUSAL_LM"))
-    g = torch.Generator().manual_seed(5)
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if ".lora_B." in n:
-                p.copy_((torch.randn(p.shape, generator=g) * 0.02).to(BF))
+    model = add_lora(_tiny_model())
     batch = _batch(model, LENGTHS, 70)
     ref_loss, ref = _oracle_padded(model, batch, lora_scale=2.0)
     loss = model.training_loss(batch, lengths=LENGTHS)
@@ -259,7 +139,8 @@ def test_lengths_none_runs_the_default_calls(monkeypatch):
     with monkeypatch.context() as m:
         vnone = _trace(m, lambda: model.validation_metrics(batch, None))
     assert vbase == vnone
-    assert not set(NEW[:-1]) & set(base + vbase)
+    assert not {"batch_to_xy_packed", "rope_qk_seg_", "linear_rope_seg", "attn_causal_fwd_seg",
+                "attn_causal_bwd_seg"} & set(base + vbase)
 
 
 def test_validation_metrics_lengths(monkeypatch):

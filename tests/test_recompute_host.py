@@ -8,24 +8,7 @@ import torch
 import torch.nn.functional as F
 
 import mock_kernels
-from test_sample_seq_host import _batch, _grads, _tiny_model
-from test_sample_seq_host import install as _install_sample_seq
-
-BF = torch.bfloat16
-TARGETS = ["q_proj", "o_proj", "k_proj", "v_proj", "gate_proj", "up_proj", "down_proj"]      # train.py:443
-
-
-def _lora(model):
-    from midi_b200 import lora
-    model.requires_grad_(False)                                                          # train.py:440
-    model.add_adapter(lora.LoraAdapterConfig(r=8, lora_alpha=16, target_modules=TARGETS, lora_dropout=0, bias="none",
-                                             task_type="CAUSAL_LM"))
-    g = torch.Generator().manual_seed(5)
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if ".lora_B." in n:
-                p.copy_((torch.randn(p.shape, generator=g) * 0.02).to(BF))
-    return model
+from host_model import add_lora as _lora, grads as _grads, make_batch as _batch, tiny_model as _tiny_model
 
 
 def _both(model, step):
@@ -56,7 +39,7 @@ def _assert_same(out):
 
 @pytest.mark.parametrize("case", ["full", "lora", "sample_idx", "int16"])
 def test_checkpointed_step_is_exact(monkeypatch, case):
-    _install_sample_seq(monkeypatch)
+    mock_kernels.install(monkeypatch)
     model = _tiny_model()
     if case == "lora":
         _lora(model)
@@ -68,7 +51,7 @@ def test_checkpointed_step_is_exact(monkeypatch, case):
 
 
 def test_checkpointed_accumulate_is_exact(monkeypatch):
-    _install_sample_seq(monkeypatch)
+    mock_kernels.install(monkeypatch)
     model = _tiny_model()
     a, b = _batch(model, seed=1), _batch(model, seed=2)
 
@@ -118,7 +101,7 @@ def _split(names):
 
 def _traced(monkeypatch, fn):
     """Kernel-call names of fn() with the recompute markers interleaved at the point where they happen."""
-    from midi_b200 import engine, lib, ops
+    from midi_b200 import engine
     names = []
     rec = engine.StackEngine._recompute
 
@@ -128,16 +111,7 @@ def _traced(monkeypatch, fn):
         names.append("</recompute>")
         return r
     monkeypatch.setattr(engine.StackEngine, "_recompute", marked)
-    for name in ("embed_sum", "inner_input", "inner_input_rows", "inner_input_rows_bwd_hidden", "batch_to_xy", "embed_bwd",
-                 "rmsnorm", "add_rmsnorm", "rmsnorm_bwd", "rope_table", "rope_qk_", "swiglu", "swiglu_bwd", "scale", "gemm",
-                 "linear_swiglu", "linear_rope", "attn_causal_fwd", "attn_causal_bwd", "attn_tiny_fwd", "attn_tiny_bwd",
-                 "ce_fwd", "ce_bwd_", "argmax_hits"):
-        f = getattr(ops, name)
-        monkeypatch.setattr(ops, name, lambda *a, _f=f, _n=name, **k: (names.append(_n), _f(*a, **k))[1])
-    call = lib.call
-    monkeypatch.setattr(lib, "call", lambda n, *a: (names.append(n), call(n, *a))[1])
-    fn()
-    return names
+    return mock_kernels.trace(monkeypatch, fn, names)
 
 
 # the recompute of one layer, per configuration: rmsnorm(x); QKV GEMM (+ q/k/v adapters: A GEMM, scale, B GEMM into qkv)
@@ -153,7 +127,7 @@ _RECOMPUTE = {
 
 @pytest.mark.parametrize("lora", [False, True])
 def test_checkpointed_trace_is_default_plus_recompute(monkeypatch, lora):
-    _install_sample_seq(monkeypatch)
+    mock_kernels.install(monkeypatch)
     model = _tiny_model()
     if lora:
         _lora(model)
@@ -186,7 +160,7 @@ def test_checkpointed_trace_is_default_plus_recompute(monkeypatch, lora):
 def test_recompute_issues_no_down_proj_gemm(monkeypatch):
     """The GEMMs a recompute issues, by their (N, K): the QKV, o and gate|up projections, none with K = inner (down)."""
     from midi_b200 import engine, ops
-    _install_sample_seq(monkeypatch)
+    mock_kernels.install(monkeypatch)
     model = _tiny_model()
     batch = _batch(model)
     model.gradient_checkpointing_enable()

@@ -1,59 +1,13 @@
 """Host logic of the fused trainer's train.py --sample-seq path (`training_loss(sample_idx=...)`) and of its validation
-step (`validation_metrics`) on CPU, over the mock kernel layer (tests/mock_kernels.py) plus stand-ins for the three entry
-points they add, compared with the oracle's autograd.  The kernels themselves are checked on the GPU
-(tests/test_gpu_sample_seq.py)."""
+step (`validation_metrics`) on CPU, over the mock kernel layer (tests/mock_kernels.py), compared with the oracle's
+autograd.  The kernels themselves are checked on the GPU (tests/test_gpu_sample_seq.py)."""
 import pytest
 import torch
 import torch.nn.functional as F
 
-import mock_kernels
-
-BF = torch.bfloat16
-TARGETS = ["q_proj", "o_proj", "k_proj", "v_proj", "gate_proj", "up_proj", "down_proj"]      # train.py:443
-
-
-# ------------------------------------------------------------------ stand-ins for the new wrappers (midi_b200.ops)
-def inner_input_rows(hidden, y, rows, table):
-    y_sel = y[rows.long()]
-    return mock_kernels.inner_input(hidden[rows.long()], y_sel[:, :-1], table), y_sel.clone()
-
-
-def inner_input_rows_bwd_hidden(dx, inv, n_events, Tin):
-    H = dx.shape[1]
-    out = torch.zeros((inv.shape[0], H), dtype=BF)
-    sel = inv >= 0
-    out[sel] = dx.view(n_events, Tin, H)[:, 0][inv[sel].long()]
-    return out
-
-
-def argmax_hits(logits, targets, V, ignore_index):
-    am = logits[:, :V].float().argmax(-1)
-    live = (targets != ignore_index) & (targets >= 0) & (targets < V)
-    return torch.stack([(live & (am == targets)).sum(), live.sum()]).float()
-
-
-def install(monkeypatch):
-    from midi_b200 import ops
-    mock_kernels.install(monkeypatch)
-    for name in ("inner_input_rows", "inner_input_rows_bwd_hidden", "argmax_hits"):
-        monkeypatch.setattr(ops, name, globals()[name])
-
-
-# ------------------------------------------------------------------ helpers
-def _tiny_model(seed=0):
-    import midi_model as mm
-    torch.manual_seed(seed)
-    cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=4, n_embd=256, n_inner=512)
-    return mm.MIDIModel(cfg).to(BF).train()
-
-
-def _batch(model, B=2, S1=10, seed=1, pad_tail=0):
-    from midi_b200.synth import synth_batch
-    return synth_batch(model.tokenizer, B, S1, seed=seed, pad_tail=pad_tail)
-
-
-def _grads(model):
-    return {n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None}
+from host_model import BF, add_lora, global_rel as _global_rel, grads as _grads, make_batch as _batch, \
+    tiny_model as _tiny_model
+from mock_kernels import install, trace as _trace
 
 
 def _oracle_sampled(model, batch, idx, lora_scale=None):
@@ -70,12 +24,6 @@ def _oracle_sampled(model, batch, idx, lora_scale=None):
     loss = F.cross_entropy(logits.reshape(-1, tok.vocab_size), ys.reshape(-1), reduction="mean", ignore_index=tok.pad_id)
     loss.backward()
     return float(loss.detach()), {n: t.grad for n, t in leaf.items() if t.grad is not None}
-
-
-def _global_rel(got, ref):
-    num = sum(float((got[n].double() - ref[n].double()).pow(2).sum()) for n in ref)
-    den = sum(float(ref[n].double().pow(2).sum()) for n in ref)
-    return (num / den) ** 0.5
 
 
 # ------------------------------------------------------------------ tests
@@ -142,17 +90,8 @@ def test_sample_idx_accumulate_and_grad_ready(monkeypatch):
 
 
 def test_sample_idx_lora(monkeypatch):
-    from midi_b200 import lora
     install(monkeypatch)
-    model = _tiny_model()
-    model.requires_grad_(False)
-    model.add_adapter(lora.LoraAdapterConfig(r=8, lora_alpha=16, target_modules=TARGETS, lora_dropout=0, bias="none",
-                                             task_type="CAUSAL_LM"))
-    g = torch.Generator().manual_seed(5)
-    with torch.no_grad():
-        for n, p in model.named_parameters():
-            if ".lora_B." in n:
-                p.copy_((torch.randn(p.shape, generator=g) * 0.02).to(BF))
+    model = add_lora(_tiny_model())
     batch = _batch(model)
     idx = [-1, 3, 0]
     ref_loss, ref = _oracle_sampled(model, batch, idx, lora_scale=2.0)
@@ -161,23 +100,6 @@ def test_sample_idx_lora(monkeypatch):
     got = _grads(model)
     assert set(got) == {n for n in ref if ".lora_" in n}
     assert _global_rel(got, {n: ref[n] for n in got}) < 6e-2
-
-
-def _trace(monkeypatch, fn):
-    """Names of the kernel-layer calls `fn` issues (ops wrappers and raw C-ABI calls), in order."""
-    from midi_b200 import lib, ops
-    names = []
-    for name in ("embed_sum", "inner_input", "inner_input_rows", "inner_input_rows_bwd_hidden", "batch_to_xy", "embed_bwd",
-                 "rmsnorm", "add_rmsnorm", "rmsnorm_bwd", "rope_table", "rope_qk_", "swiglu", "swiglu_bwd", "scale", "gemm",
-                 "linear_swiglu", "linear_rope", "attn_causal_fwd", "attn_causal_bwd", "attn_tiny_fwd", "attn_tiny_bwd",
-                 "ce_fwd", "ce_bwd_", "argmax_hits"):
-        f = getattr(ops, name)
-        monkeypatch.setattr(ops, name, lambda *a, _f=f, _n=name, **k: (names.append(_n), _f(*a, **k))[1])
-    call = lib.call
-    monkeypatch.setattr(lib, "call", lambda n, *a: (names.append(n), call(n, *a))[1])
-    fn()
-    monkeypatch.setattr(lib, "call", call)
-    return names
 
 
 def test_sample_idx_none_runs_the_default_calls(monkeypatch):
