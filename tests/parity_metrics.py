@@ -1,5 +1,6 @@
-"""Metrics that compare a bf16 kernel result with a high-precision reference element by element or row by row, and the
-NaN sentinel / poisoned-input buffers the conformance groups of gpu_checks.py build their operands in.
+"""Metrics that compare a bf16 kernel result with a high-precision reference element by element or row by row, the
+NaN sentinel / poisoned-input buffers the conformance groups of gpu_checks.py build their operands in, the fp64
+attention references they are scored against, and the one check that judges every GPU test's metrics by its bounds.
 
 Global norms hide localized errors: a wrong 8-column group in one row of a 1000 x 1024 GEMM, or a zeroed last row of
 one attention head, moves a relative Frobenius norm by less than its usual bound.  These helpers score the worst
@@ -7,10 +8,39 @@ element or the worst row instead.  Pure PyTorch on any device, so tests/test_par
 each metric fails on the corruptions it is meant to catch."""
 from __future__ import annotations
 
+import math
+
 import torch
 
 BF = torch.bfloat16
 NAN = float("nan")
+
+
+# ------------------------------------------------------------------------------------------ bounds
+def check_bounds(metrics: dict, bounds, info=()) -> list:
+    """(name, value, bound, ok) for every metric.
+
+    bounds: (prefix, bound) pairs; the first prefix a name starts with gives its bound.  A "min:" prefix is a lower
+            bound (ok when value >= bound), any other an upper bound (ok when value <= bound and value is not NaN).
+    info  : the names reported without a bound (timings, lengths, distances kept for the record).  Any other metric
+            that matches no prefix fails, so a renamed or misspelt metric cannot drop out of the check unnoticed."""
+    rows = []
+    for k, v in metrics.items():
+        hit = next(((p, b) for p, b in bounds if k.startswith(p.removeprefix("min:"))), None)
+        if hit is None:
+            rows.append((k, v, None, k in info))
+        elif hit[0].startswith("min:"):
+            rows.append((k, v, hit[1], v >= hit[1]))
+        else:
+            rows.append((k, v, hit[1], v <= hit[1] and not math.isnan(v)))
+    return rows
+
+
+def assert_within(metrics: dict, bounds, info=()):
+    """check_bounds as a test assertion; prints the metrics."""
+    print(metrics)
+    bad = [(k, v, b) for k, v, b, ok in check_bounds(metrics, bounds, info) if not ok]
+    assert not bad, f"out of bounds or without one: {bad}"
 
 
 # ------------------------------------------------------------------------------------------ per-element exactness
@@ -113,3 +143,31 @@ def sentinel_report(buf: torch.Tensor, inside, zero=None) -> dict:
     if zero is not None:
         out["padcols_nonzero"] = float(((buf.float() != 0) & mask_zero).sum())
     return out
+
+
+# ------------------------------------------------------------------------------------------ fp64 references
+def attn_ref64(q, k, v, do, off, scale=0.125, o_in=None):
+    """fp64 causal attention (query q sees keys <= q + off) and its gradients; tensors (B, h, S, D).
+
+    The backward is written out (dS = P (dP - delta), delta = rowsum(dO o)) because the kernels take o as an input: with
+    o_in (the bf16 o handed to the backward) delta is formed from it, so the reference is the exact gradient of the
+    inputs the kernel gets.  Without o_in (o exact) this is fp64 autograd.  It matters where softmax saturates: there
+    dS cancels almost completely and the rounding of o alone moves dq, dk far more than any kernel error."""
+    q, k, v, do = (t.detach().double() for t in (q, k, v, do))
+    s = (q @ k.transpose(-1, -2)) * scale
+    Sq, Sk = q.shape[-2], k.shape[-2]
+    m = torch.arange(Sk, device=q.device)[None] > (torch.arange(Sq, device=q.device)[:, None] + off)
+    s = s.masked_fill(m, float("-inf"))
+    lse = torch.logsumexp(s, -1)
+    p = torch.softmax(s, -1)
+    o = p @ v
+    delta = (do * (o if o_in is None else o_in.double())).sum(-1, keepdim=True)
+    ds = p * (do @ v.transpose(-1, -2) - delta)
+    return o, lse, ds @ k * scale, ds.transpose(-1, -2) @ q * scale, p.transpose(-1, -2) @ do
+
+
+def rope_bwd64(g, cos, sin, pos):
+    """gradient w.r.t. the pre-rotation projection: the transpose of x' = x c + rotate_half(x) s, in fp64 at `pos`."""
+    c, s = cos.double()[pos], sin.double()[pos]
+    g1, g2 = g[..., :32], g[..., 32:]
+    return torch.cat([g1 * c + g2 * s, g2 * c - g1 * s], -1)

@@ -1,24 +1,21 @@
 """The restatements of tests/decode_reference.py and the case sets the decode conformance groups (gv_ / da_ / sm_ / pd_ in
 gpu_checks.py) feed them, on the CPU: each defect a sampler, RNG or paged-KV kernel could plausibly have changes the
-result on some case, and is judged a failure by the bounds the GPU groups use (gpu_checks.THRESH)."""
+result on some case, and is judged a failure by the bounds the GPU groups use (the tables of gpu_checks.GROUPS)."""
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import decode_reference as R  # noqa: E402
-import gpu_checks as G  # noqa: E402
-import parity_metrics as P  # noqa: E402
+import decode_reference as R
+import gpu_checks as G
+import parity_metrics as P
 
 BF = torch.bfloat16
 
 
-def _fails(metrics):
-    res = G.verdict(metrics)
+def _fails(group, metrics):
+    res = P.check_bounds(metrics, G.GROUPS[group].bounds)
     assert all(b is not None for _, _, b, _ in res), res
     return any(not ok for *_, ok in res)
 
@@ -44,12 +41,12 @@ def _topp_topk_mismatches(bf16_sem, **defect):
 def test_sampler_cases_catch_defect(bf16_sem, defect):
     n = _topp_topk_mismatches(bf16_sem, **defect)
     assert n > 0
-    assert _fails({"sm_topp_fp32_mismatch": float(n)})
+    assert _fails("sampler_exact", {"sm_topp_fp32_mismatch": float(n)})
 
 
 def test_sampler_cases_catch_unrounded_cumulative_sums():
     n = _topp_topk_mismatches(True, round_cum=False)
-    assert n > 0 and _fails({"sm_topp_bf16_mismatch": float(n)})
+    assert n > 0 and _fails("sampler_exact", {"sm_topp_bf16_mismatch": float(n)})
 
 
 def test_sampler_restatement_reference_semantics():
@@ -96,7 +93,7 @@ def test_uniform_fill_restatement():
         consts[i] ^= 1 << 17                                          # one constant changed
         bad = R.uniform_fill(1024, seed=12345, counter=7, dev_seed=99, consts=tuple(consts))
         n = float((bad != u).sum())
-        assert n > 0 and _fails({"sm_uniform_mismatch": n})
+        assert n > 0 and _fails("sampler_exact", {"sm_uniform_mismatch": n})
 
 
 def test_event_commit_restatement():
@@ -132,7 +129,7 @@ def test_pool_slot_written_one_position_late_fails():
         rep = {f"da_append_{k_}": v_ for k_, v_ in P.sentinel_report(kk, m).items()}
         got = torch.stack([R.gather_kv(kk, bt, page, b, T) for b in range(2)]).transpose(1, 2)
         rep["da_append_mismatch"] = float((got != vals).sum())
-        assert _fails(rep) == bool(late), rep
+        assert _fails("decode_attn_edges", rep) == bool(late), rep
         if late:
             assert rep["da_append_sentinels_changed"] > 0 and rep["da_append_nan_in_range"] > 0
 
@@ -149,13 +146,13 @@ def test_key_read_past_context_propagates_nan():
     ref = R.paged_attention64(q, k, v, bt, page, 0, T, 0.25)
     assert torch.isfinite(ref).all()
     # the same attention rounded to bf16 passes the per-row bound; one key past T (a NaN slot) makes the row +inf
-    assert not _fails({"da_attn_d64_o_row": P.row_worst(ref.to(BF), ref)})
+    assert not _fails("decode_attn_edges", {"da_attn_d64_o_row": P.row_worst(ref.to(BF), ref)})
     past = R.paged_attention64(q, k, v, bt, page, 0, T + 1, 0.25)[:, -1:]
     assert math.isinf(P.row_worst(past, ref[:, -1:]))
-    assert _fails({"da_attn_d64_o_row": P.row_worst(past, ref[:, -1:])})
+    assert _fails("decode_attn_edges", {"da_attn_d64_o_row": P.row_worst(past, ref[:, -1:])})
     # reading one slot early (key t-1 for key t) moves a row by far more than the bound
     k_shift = k.clone()
     for t in range(T - 1, 0, -1):
         k_shift[int(bt[0, t // page]), :, t % page] = k[int(bt[0, (t - 1) // page]), :, (t - 1) % page]
     early = R.paged_attention64(q, k_shift, v, bt, page, 0, T, 0.25)
-    assert _fails({"da_attn_d64_o_row": P.row_worst(early.to(BF), ref)})
+    assert _fails("decode_attn_edges", {"da_attn_d64_o_row": P.row_worst(early.to(BF), ref)})

@@ -1,17 +1,10 @@
 """GPU parity tests (`pytest -m gpu`).  Each group compares the sm_90a kernels / the drop-in
-MIDIModel -- called through the C ABI -- with the PyTorch composite / the oracle; see gpu_checks.py."""
-import os
-import sys
-
+MIDIModel -- called through the C ABI -- with the PyTorch composite / the oracle, judged by the bound table each check
+carries; see gpu_checks.py."""
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-GROUP_NAMES = ["gemm_fwd", "gemm_swiglu", "gemm_dgrad", "gemm_wgrad", "elementwise", "fused_rope", "attn_flash", "attn_wgmma", "attn_tiny", "loss_optim", "decode",
-               "model_forward", "model_layer_tf", "model_train", "model_generate", "model_peaked_greedy", "model_large",
-               "gemm_exact", "decode_paged", "lora_train", "model_vs_hf", "model_medium_long",
-               "gemm_matrix", "gemm_epilogues", "attn_edges", "gemv_matrix", "decode_attn_edges", "sampler_exact",
-               "persist_vs_phase"]
+import gpu_checks as G
+from parity_metrics import assert_within
 
 
 @pytest.mark.gpu
@@ -25,16 +18,11 @@ def test_native_library_is_loaded():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("group", GROUP_NAMES)
+@pytest.mark.parametrize("group", list(G.GROUPS))
 def test_gpu_group(group):
     import torch
     assert torch.cuda.is_available(), "needs an H100"
-    import gpu_checks as G
-    metrics = G.GROUPS[group]()
+    g = G.GROUPS[group]
+    metrics = g()
     torch.cuda.synchronize()
-    res = G.verdict(metrics)
-    if group in G.STRICT_GROUPS:
-        unbounded = [k for k, v, b, ok in res if b is None]
-        assert not unbounded, f"{group}: metrics without a bound in THRESH: {unbounded}"
-    bad = [(k, v, b) for k, v, b, ok in res if not ok]
-    assert not bad, f"{group}: out of tolerance: {bad}"
+    assert_within(metrics, g.bounds, g.info)

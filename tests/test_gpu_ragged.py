@@ -10,16 +10,12 @@ gradient must be bit-identical; RMSNorm-weight and embedding gradients are summe
 order and get the 1e-3 global relative bound of the other trainer tests.  With varied lengths the ragged step is scored
 against the oracle's fp32 autograd of the padded batch, and against the native padded step, whose GEMMs run plans
 chosen for a different M."""
-import math
-import os
-import sys
-
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (os.path.join(ROOT, "midi-model_b200"), ROOT, os.path.dirname(os.path.abspath(__file__))):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import gpu_checks as G
+import gpu_model as GM
+from host_model import TARGETS, global_rel as _rel, make_batch
+from parity_metrics import assert_within
 
 # metric-name prefix -> upper bound.  Every metric a test reports must match one.  Measured on an NVIDIA H100 80GB HBM3 at
 # a 700 W power limit: every exact comparison 0; attention worst row 3.4e-3 (o), 4.5e-3 / 4.6e-3 / 4.3e-3 (dq / dk / dv,
@@ -29,35 +25,21 @@ BOUNDS = [
     ("seg_mismatch", 0.0),                # segment kernels vs the unsegmented kernel on each segment alone
     ("sentinels_changed", 0.0),
     ("nan_in_range", 0.0),
-    ("lse_abs", 1e-4),                    # vs fp64: the attention conformance bounds of gpu_checks.py (ae_)
-    ("row", 1e-2),
+    ("lse_abs", G.AE_LSE_ABS),            # vs fp64: the attention conformance bounds of gpu_checks.py (ae_)
+    ("row", G.AE_ROW),
     ("pack_mismatch", 0.0),
     ("loss_mismatch", 0.0),               # ragged vs padded loss, bitwise (full lengths, garbage tail, validation)
     ("gemm_grad_mismatch", 0.0),          # differing elements of GEMM-produced gradients
     ("atomic_grad_rel", 1e-3),            # norm weights + embedding tables: global relative difference
-    ("oracle_loss_abs", 5e-2),            # vs the oracle's fp32 autograd of the padded batch: the sample-seq bounds
-    ("oracle_grad_rel", 6e-2),
+    ("oracle_loss_abs", G.SAMPLE_SEQ_LOSS_ABS),      # vs the oracle's fp32 autograd of the padded batch
+    ("oracle_grad_rel", G.SAMPLE_SEQ_GRAD_REL),
     ("native_loss_abs", 2e-6),            # vs the native padded step (GEMM plans for another M)
     ("native_grad_rel", 2.5e-4),
     ("accum_grad_rel", 1e-3),             # two accumulated micro-batches vs bf16(sum of the separate gradients)
     ("grad_ready_cover_error", 0.0),
     ("val_grad_changed", 0.0),
 ]
-TARGETS = ["q_proj", "o_proj", "k_proj", "v_proj", "gate_proj", "up_proj", "down_proj"]      # train.py:443
 D = 64
-
-
-def _assert_within(metrics):
-    bad, unbounded = [], []
-    for k, v in metrics.items():
-        b = next((b for p, b in BOUNDS if k.startswith(p)), None)
-        if b is None:
-            unbounded.append(k)
-        elif math.isnan(v) or v > b:
-            bad.append((k, v, b))
-    print(metrics)
-    assert not unbounded, unbounded
-    assert not bad, bad
 
 
 def _tables(seg_rows):
@@ -68,27 +50,6 @@ def _tables(seg_rows):
 
 
 # ------------------------------------------------------------------------------------------ kernels
-def _ref64(q, k, v, do, o_in):
-    """fp64 causal attention and its gradient given the bf16 o the backward receives; q..do [h, S, D]."""
-    import torch
-    q, k, v, do = (t.double() for t in (q, k, v, do))
-    S = q.shape[-2]
-    s = (q @ k.transpose(-1, -2)) * 0.125
-    s = s.masked_fill(torch.ones(S, S, dtype=torch.bool, device=q.device).triu(1), float("-inf"))
-    lse = torch.logsumexp(s, -1)
-    p = torch.softmax(s, -1)
-    o = p @ v
-    ds = p * (do @ v.transpose(-1, -2) - (do * o_in.double()).sum(-1, keepdim=True))
-    return o, lse, ds @ k * 0.125, ds.transpose(-1, -2) @ q * 0.125, p.transpose(-1, -2) @ do
-
-
-def _rope_bwd64(g, cos, sin, n):
-    """gradient w.r.t. the pre-rotation projection at positions 0 .. n-1, in fp64."""
-    import torch
-    c, s = cos.double()[:n], sin.double()[:n]
-    return torch.cat([g[..., :32] * c + g[..., 32:] * s, g[..., 32:] * c - g[..., :32] * s], -1)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("segs", [[64], [64, 192, 64, 1216, 128], [2048]], ids=["one_tile", "mixed", "s2048"])
 @pytest.mark.parametrize("nh", [1, 16])
@@ -155,13 +116,13 @@ def test_segment_attention_kernels(segs, nh):
             mism["dqkv_rope" if rope else "dqkv"] += int((d1[:, :3 * H] != grads[rope][r0:r0 + R, :3 * H]).sum())
         heads = lambda t, c0: t[r0:r0 + R, c0:c0 + H].view(R, nh, D).transpose(0, 1)
         qs, ks, vs, dos, os_ = heads(qkvb, 0), heads(qkvb, H), heads(qkvb, 2 * H), heads(dob, 0), heads(ob, 0)
-        o64, lse64, dq64, dk64, dv64 = _ref64(qs, ks, vs, dos, os_)
+        o64, lse64, dq64, dk64, dv64 = P.attn_ref64(qs, ks, vs, dos, 0, o_in=os_)
         atol = 1e-3 * float(dos.double().norm(dim=-1).median())
         sc = {"o": P.row_worst(os_, o64, atol=atol), "lse_abs": float((lse[:, r0:r0 + R].double() - lse64).abs().max())}
         for rope in (False, True):
             gq, gk, gv = (heads(grads[rope], c) for c in (0, H, 2 * H))
-            rq = _rope_bwd64(dq64, cos, sin, R) if rope else dq64
-            rk = _rope_bwd64(dk64, cos, sin, R) if rope else dk64
+            rq = P.rope_bwd64(dq64, cos, sin, slice(0, R)) if rope else dq64
+            rk = P.rope_bwd64(dk64, cos, sin, slice(0, R)) if rope else dk64
             sfx = "_rope" if rope else ""
             sc["dq" + sfx] = P.row_worst(gq, rq, atol=atol)
             sc["dk" + sfx] = P.row_worst(gk, rk, atol=atol)
@@ -171,7 +132,7 @@ def test_segment_attention_kernels(segs, nh):
         r0 += R
     m.update({f"seg_mismatch_{n}_{tag}": float(c) for n, c in mism.items()})
     m.update({(n if n == "lse_abs" else f"row_{n}") + f"_{tag}": val for n, val in worst.items()})
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 @pytest.mark.gpu
@@ -204,7 +165,7 @@ def test_segment_rope_kernels():
         r0 += R
     # the fused epilogue rotates exactly as the stand-alone kernel does (as in the unsegmented entries)
     m["seg_mismatch_gemm_vs_rope_kernel"] = float((fused != rot[False]).sum())
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 @pytest.mark.gpu
@@ -224,76 +185,25 @@ def test_pack_kernel_matches_torch_gather():
     m = {"pack_mismatch_x": float((x != flat[idx].masked_fill(gap, pad)).sum()),
          "pack_mismatch_y": float((y != flat[idx + 1].masked_fill(gap, pad)).sum()),
          "pack_mismatch_shape": float(x.shape != (src.numel(), T) or x.dtype != torch.long)}
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 # ------------------------------------------------------------------------------------------ model
-def _new_model():
-    import torch
-    import midi_model as mm
-    assert torch.cuda.is_available(), "needs an H100"
-    torch.manual_seed(0)
-    cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=16, n_embd=1024, n_inner=4096)
-    return mm.MIDIModel(cfg).to("cuda", dtype=torch.bfloat16).train()
-
-
 @pytest.fixture(scope="module")
 def model():
-    return _new_model()
+    return GM.cuda_model()
 
 
 def _batch(model, lengths, S1, seed):
-    from midi_b200.synth import synth_batch
-    b = synth_batch(model.tokenizer, len(lengths), S1, seed=seed)
-    for i, L in enumerate(lengths):
-        b[i, L:] = model.tokenizer.pad_id
-    return b.to("cuda")
-
-
-def _atomic(name):
-    return name.endswith("norm.weight") or name.endswith("layernorm.weight") or name.endswith("embed_tokens.weight")
-
-
-def _step(model, fn):
-    import torch
-    for p in model.parameters():
-        p.grad = None
-    calls = []
-    loss = fn(lambda lo, hi: calls.append((lo, hi)))
-    torch.cuda.synchronize()
-    return loss.detach().float().clone(), {n: p.grad.clone() for n, p in model.named_parameters() if p.grad is not None}, calls
-
-
-def _rel(got, ref, names):
-    num = sum(float((got[n].double() - ref[n].double()).pow(2).sum()) for n in names)
-    den = sum(float(ref[n].double().pow(2).sum()) for n in names)
-    return math.sqrt(num / den)
+    return make_batch(model, S1=S1, seed=seed, lengths=lengths).to("cuda")
 
 
 def _exact(a, b, tag):
-    """metrics of two steps that must agree bit for bit up to the fp32-atomic gradients."""
-    import torch
-    (l0, g0, c0), (l1, g1, c1) = a, b
-    assert g0 and g0.keys() == g1.keys()
-    gemm = [n for n in g0 if not _atomic(n)]
-    atomic = [n for n in g0 if _atomic(n)]
-    m = {f"loss_mismatch_{tag}": float(not torch.equal(l0, l1)),
-         f"gemm_grad_mismatch_{tag}": float(sum(int((g0[n] != g1[n]).sum()) for n in gemm))}
-    if atomic:
-        m[f"atomic_grad_rel_{tag}"] = _rel(g1, g0, atomic)
-    if c0 or c1:
-        m[f"grad_ready_cover_error_{tag}_calls"] = float(c0 != c1)
+    """GM.exact, and whether the two steps made the same grad_ready calls."""
+    m = GM.exact(a, b, tag)
+    if a[2] or b[2]:
+        m[f"grad_ready_cover_error_{tag}_calls"] = float(a[2] != b[2])
     return m
-
-
-def _cover(model, calls, tag):
-    import torch
-    store = model._rt().store
-    cover, want = (torch.zeros(store.numel, dtype=torch.int32) for _ in range(2))
-    want[store.train_lo:store.train_hi] = 1
-    for lo, hi in calls:
-        cover[lo:hi] += 1
-    return {f"grad_ready_cover_error_{tag}": float((cover != want).sum())}
 
 
 @pytest.mark.gpu
@@ -305,30 +215,30 @@ def test_full_lengths_are_the_padded_step(model):
         batch = _batch(model, [S1] * B, S1, seed=3)
         for dt in (torch.int64, torch.int16):
             b = batch.to(dt)
-            pad = _step(model, lambda gr: model.training_loss(b, grad_ready=gr))
-            rag = _step(model, lambda gr: model.training_loss(b, grad_ready=gr, lengths=[S1] * B))
+            pad = GM.step(model, lambda gr: model.training_loss(b, grad_ready=gr))
+            rag = GM.step(model, lambda gr: model.training_loss(b, grad_ready=gr, lengths=[S1] * B))
             m.update(_exact(pad, rag, f"S{S1 - 1}_{str(dt)[6:]}"))
-            m.update(_cover(model, rag[2], f"S{S1 - 1}_{str(dt)[6:]}"))
+            m.update(GM.cover(model, rag[2], f"S{S1 - 1}_{str(dt)[6:]}"))
     # the other RoPE settings: QKV GEMM epilogue in the forward, stand-alone RoPE kernel in the backward
     batch = _batch(model, [129] * 3, 129, seed=4)
     for flag, val in (("FUSE_ROPE_FWD", True), ("FUSE_ROPE", False)):
         old = getattr(engine, flag)
         setattr(engine, flag, val)
         try:
-            pad = _step(model, lambda gr: model.training_loss(batch))
-            rag = _step(model, lambda gr: model.training_loss(batch, lengths=[129] * 3))
+            pad = GM.step(model, lambda gr: model.training_loss(batch))
+            rag = GM.step(model, lambda gr: model.training_loss(batch, lengths=[129] * 3))
         finally:
             setattr(engine, flag, old)
         m.update(_exact(pad, rag, f"S128_{flag}_{int(val)}"))
     # activation checkpointing: the checkpointed ragged step against the padded one
     model.gradient_checkpointing_enable()
     try:
-        pad = _step(model, lambda gr: model.training_loss(batch))
-        rag = _step(model, lambda gr: model.training_loss(batch, lengths=[129] * 3))
+        pad = GM.step(model, lambda gr: model.training_loss(batch))
+        rag = GM.step(model, lambda gr: model.training_loss(batch, lengths=[129] * 3))
     finally:
         model.gradient_checkpointing_disable()
     m.update(_exact(pad, rag, "S128_checkpoint"))
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 VARIED = [2049, 1300, 700, 65]
@@ -340,11 +250,11 @@ def test_varied_lengths_against_oracle_and_padded_step(model):
     import torch.nn.functional as F
     from oracle import midi_oracle as O
     batch = _batch(model, VARIED, 2049, seed=5)
-    rag = _step(model, lambda gr: model.training_loss(batch, lengths=VARIED, grad_ready=gr))
-    pad = _step(model, lambda gr: model.training_loss(batch))
+    rag = GM.step(model, lambda gr: model.training_loss(batch, lengths=VARIED, grad_ready=gr))
+    pad = GM.step(model, lambda gr: model.training_loss(batch))
     names = list(rag[1])
-    m = {"native_loss_abs": float((rag[0] - pad[0]).abs()), "native_grad_rel": _rel(rag[1], pad[1], names)}
-    m.update(_cover(model, rag[2], "varied"))
+    m = {"native_loss_abs": float((rag[0] - pad[0]).abs()), "native_grad_rel": _rel(rag[1], pad[1])}
+    m.update(GM.cover(model, rag[2], "varied"))
     # events past each length are never read: garbage there changes nothing
     junk = _batch(model, [2049] * 4, 2049, seed=9)
     dirty = batch.clone()
@@ -352,7 +262,7 @@ def test_varied_lengths_against_oracle_and_padded_step(model):
         dirty[i, L:] = junk[i, L:]
     for dt in (torch.int64, torch.int16):
         b = dirty.to(dt)
-        m.update(_exact(rag, _step(model, lambda gr: model.training_loss(b, lengths=VARIED, grad_ready=gr)),
+        m.update(_exact(rag, GM.step(model, lambda gr: model.training_loss(b, lengths=VARIED, grad_ready=gr)),
                         f"garbage_{str(dt)[6:]}"))
     # the oracle's fp32 autograd of the padded batch (train.py:169-185)
     ocfg = O.cfg_from_hf(model.config)
@@ -360,11 +270,11 @@ def test_varied_lengths_against_oracle_and_padded_step(model):
     lo = O.train_loss(sd, ocfg, batch)
     lo.backward()
     m["oracle_loss_abs"] = float((rag[0] - lo.detach()).abs())
-    m["oracle_grad_rel"] = _rel(rag[1], {n: sd[n].grad for n in names}, names)
+    m["oracle_grad_rel"] = _rel(rag[1], {n: sd[n].grad for n in names})
     print("ragged loss", float(rag[0]), "padded", float(pad[0]), "oracle", float(lo))
     del sd, lo
     torch.cuda.empty_cache()
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 @pytest.mark.gpu
@@ -372,25 +282,25 @@ def test_varied_lengths_checkpoint_accumulate_validation(model):
     import torch
     m = {}
     batch = _batch(model, VARIED, 2049, seed=5)
-    plain = _step(model, lambda gr: model.training_loss(batch, lengths=VARIED))
+    plain = GM.step(model, lambda gr: model.training_loss(batch, lengths=VARIED))
     model.gradient_checkpointing_enable()
     try:
-        ck = _step(model, lambda gr: model.training_loss(batch, lengths=VARIED))
+        ck = GM.step(model, lambda gr: model.training_loss(batch, lengths=VARIED))
     finally:
         model.gradient_checkpointing_disable()
     m.update(_exact(plain, ck, "checkpoint"))
     # two accumulated micro-batches
     la, lb = [130, 2, 77, 129], [64, 130, 0, 100]
     a, b = _batch(model, la, 130, seed=21), _batch(model, lb, 130, seed=22)
-    _, ga, _ = _step(model, lambda gr: model.training_loss(a, lengths=la))
-    _, gb, _ = _step(model, lambda gr: model.training_loss(b, lengths=lb))
+    _, ga, _ = GM.step(model, lambda gr: model.training_loss(a, lengths=la))
+    _, gb, _ = GM.step(model, lambda gr: model.training_loss(b, lengths=lb))
     calls = []
     model.training_loss(a, lengths=la)
     model.training_loss(b, lengths=torch.tensor(lb), accumulate=True, grad_ready=lambda lo, hi: calls.append((lo, hi)))
     got = {n: p.grad.clone() for n, p in model.named_parameters()}
     gsum = {n: (ga[n].float() + gb[n].float()).to(torch.bfloat16) for n in ga}
-    m["accum_grad_rel"] = _rel(got, gsum, list(ga))
-    m.update(_cover(model, calls, "accum"))
+    m["accum_grad_rel"] = _rel(got, gsum)
+    m.update(GM.cover(model, calls, "accum"))
     # validation: the loss training_loss(backward=False) returns, gradient buffer untouched
     gflat = model._rt().store.gflat
     g0 = gflat.clone()
@@ -398,14 +308,14 @@ def test_varied_lengths_checkpoint_accumulate_validation(model):
     m["val_grad_changed"] = float((gflat != g0).sum())
     m["loss_mismatch_val"] = float(not torch.equal(loss, model.training_loss(batch, lengths=VARIED, backward=False)))
     print("val loss", float(loss), "acc", float(acc))
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 @pytest.mark.gpu
 def test_lora_ragged_step():
     import torch
     from midi_b200 import lora
-    lm = _new_model()
+    lm = GM.cuda_model()
     lm.requires_grad_(False)
     lm.add_adapter(lora.LoraAdapterConfig(r=16, lora_alpha=32, target_modules=TARGETS, lora_dropout=0, bias="none",
                                           task_type="CAUSAL_LM"))
@@ -416,16 +326,16 @@ def test_lora_ragged_step():
                 p.copy_((torch.randn(p.shape, generator=g, device="cuda") * 0.02).to(torch.bfloat16))
     m = {}
     batch = _batch(lm, [129] * 3, 129, seed=6)
-    pad = _step(lm, lambda gr: lm.training_loss(batch, grad_ready=gr))
-    rag = _step(lm, lambda gr: lm.training_loss(batch, lengths=[129] * 3, grad_ready=gr))
+    pad = GM.step(lm, lambda gr: lm.training_loss(batch, grad_ready=gr))
+    rag = GM.step(lm, lambda gr: lm.training_loss(batch, lengths=[129] * 3, grad_ready=gr))
     m.update(_exact(pad, rag, "lora_full"))
-    m.update(_cover(lm, rag[2], "lora"))
+    m.update(GM.cover(lm, rag[2], "lora"))
     vb = _batch(lm, VARIED, 2049, seed=7)
     lm.gradient_checkpointing_enable()
-    ck = _step(lm, lambda gr: lm.training_loss(vb, lengths=VARIED))
+    ck = GM.step(lm, lambda gr: lm.training_loss(vb, lengths=VARIED))
     lm.gradient_checkpointing_disable()
-    plain = _step(lm, lambda gr: lm.training_loss(vb, lengths=VARIED))
+    plain = GM.step(lm, lambda gr: lm.training_loss(vb, lengths=VARIED))
     m.update(_exact(plain, ck, "lora_checkpoint"))
     del lm
     torch.cuda.empty_cache()
-    _assert_within(m)
+    assert_within(m, BOUNDS)

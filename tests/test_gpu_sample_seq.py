@@ -6,24 +6,19 @@ The reference for the sampled step is the drop-in autograd path running train.py
 same kernels, so the loss must agree bit for bit (the drop-in loss is bf16, the dtype of the logits: the fused fp32 loss
 rounded to bf16 must equal it) and the gradients within the spread of the backward's non-deterministic fp32 reductions.
 The oracle's fp32 autograd bounds the error itself."""
-import math
-import os
-import random
-import sys
-
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for _p in (os.path.join(ROOT, "midi-model_b200"), ROOT):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+import gpu_checks as G
+import gpu_model as GM
+from host_model import BF, global_rel as _rel, grads as _grads, make_batch
+from parity_metrics import assert_within
 
 # metric-name prefix -> upper bound.  Every metric a test reports must match one.
 BOUNDS = [
     ("dropin_loss_mismatch", 0.0),        # fused loss (rounded to bf16) vs the drop-in --sample-seq loss
-    ("dropin_grad_rel", 1e-3),            # global relative gradient error: the int16_path_grad_rel bound
-    ("oracle_loss_abs", 5e-2),            # vs the oracle's fp32 autograd: the drop-in sample_seq_* bounds
-    ("oracle_grad_rel", 6e-2),
+    ("dropin_grad_rel", G.INT16_PATH_GRAD_REL),      # global relative gradient error
+    ("oracle_loss_abs", G.SAMPLE_SEQ_LOSS_ABS),      # vs the oracle's fp32 autograd
+    ("oracle_grad_rel", G.SAMPLE_SEQ_GRAD_REL),
     ("full_range_loss_mismatch", 0.0),    # sample_idx = range(S) vs training_loss(batch)
     ("full_range_grad_rel", 1e-3),
     ("accum_grad_rel", 1e-3),             # two accumulated micro-batches vs bf16(sum of the separate gradients)
@@ -36,47 +31,13 @@ BOUNDS = [
 ]
 
 
-def _assert_within(metrics):
-    bad, unbounded = [], []
-    for k, v in metrics.items():
-        b = next((b for p, b in BOUNDS if k.startswith(p)), None)
-        if b is None:
-            unbounded.append(k)
-        elif math.isnan(v) or v > b:
-            bad.append((k, v, b))
-    print(metrics)
-    assert not unbounded, unbounded
-    assert not bad, bad
-
-
 @pytest.fixture(scope="module")
 def model():
-    import torch
-    import midi_model as mm
-    assert torch.cuda.is_available(), "needs an H100"
-    torch.manual_seed(0)
-    cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=16, n_embd=1024, n_inner=4096)
-    return mm.MIDIModel(cfg).to("cuda", dtype=torch.bfloat16).train()
+    return GM.cuda_model()
 
 
 def _batch(model, S1, seed, pad_tail=0):
-    from midi_b200.synth import synth_batch
-    return synth_batch(model.tokenizer, 2, S1, seed=seed, pad_tail=pad_tail).to("cuda")
-
-
-def _rand_idx(S, seed=0):
-    random.seed(seed)
-    return [-1] + random.sample(list(range(S - 2)), min(127, (S - 2) // 2))      # train.py:173
-
-
-def _grads(model):
-    return {n: p.grad.float().clone() for n, p in model.named_parameters()}
-
-
-def _rel(got, ref):
-    num = sum(float((got[n].double() - ref[n].double()).pow(2).sum()) for n in ref)
-    den = sum(float(ref[n].double().pow(2).sum()) for n in ref)
-    return math.sqrt(num / den)
+    return make_batch(model, 2, S1, seed=seed, pad_tail=pad_tail).to("cuda")
 
 
 def _fused(model, batch, idx, **kw):
@@ -112,8 +73,8 @@ def _vs_dropin(model, batch, idx, tag):
 def test_sampled_step_matches_the_dropin_expression(model):
     m = {}
     for S1 in (130, 2049):
-        m.update(_vs_dropin(model, _batch(model, S1, seed=5), _rand_idx(S1 - 1), f"S{S1 - 1}"))
-    _assert_within(m)
+        m.update(_vs_dropin(model, _batch(model, S1, seed=5), GM.rand_idx(S1 - 1), f"S{S1 - 1}"))
+    assert_within(m, BOUNDS)
 
 
 @pytest.mark.gpu
@@ -123,7 +84,7 @@ def test_sampled_step_matches_oracle_autograd(model):
     from oracle import midi_oracle as O
     tok = model.tokenizer
     batch = _batch(model, 130, seed=5)
-    idx = _rand_idx(129)
+    idx = GM.rand_idx(129)
     lf, gf = _fused(model, batch, idx)
     ocfg = O.cfg_from_hf(model.config)
     sd = {k: v.detach().float().requires_grad_(True) for k, v in model.state_dict().items()}
@@ -133,8 +94,8 @@ def test_sampled_step_matches_oracle_autograd(model):
     lg = O.forward_token(sd, ocfg, h.reshape(-1, h.shape[-1]), ys[:, :-1], inv_freq=model.net_token.rotary_emb.inv_freq)
     lo = F.cross_entropy(lg.view(-1, tok.vocab_size), ys.reshape(-1), reduction="mean", ignore_index=tok.pad_id)
     lo.backward()
-    _assert_within({"oracle_loss_abs": float((lf - lo.detach()).abs()),
-                    "oracle_grad_rel": _rel(gf, {n: sd[n].grad for n in gf})})
+    assert_within({"oracle_loss_abs": float((lf - lo.detach()).abs()),
+                   "oracle_grad_rel": _rel(gf, {n: sd[n].grad for n in gf})}, BOUNDS)
     del sd, lg, h
     torch.cuda.empty_cache()
 
@@ -145,7 +106,7 @@ def test_full_range_is_the_default_step(model):
     l0 = model.training_loss(batch).detach().clone()
     g0 = _grads(model)
     l1, g1 = _fused(model, batch, range(129))
-    _assert_within({"full_range_loss_mismatch": float(l0 != l1), "full_range_grad_rel": _rel(g1, g0)})
+    assert_within({"full_range_loss_mismatch": float(l0 != l1), "full_range_grad_rel": _rel(g1, g0)}, BOUNDS)
 
 
 @pytest.mark.gpu
@@ -154,24 +115,24 @@ def test_sampled_step_edge_cases(model):
     m = {}
     # unsorted and negative positions; a batch whose last 20 events are padding (-1 selects a pad event); S = 3 (K = 1)
     m.update(_vs_dropin(model, _batch(model, 130, seed=7), [5, -1, 0, -7, 3, 100, -128], "unsorted"))
-    m.update(_vs_dropin(model, _batch(model, 130, seed=8, pad_tail=20), _rand_idx(129, seed=3), "padtail"))
-    m.update(_vs_dropin(model, _batch(model, 4, seed=9), _rand_idx(3), "S3"))
+    m.update(_vs_dropin(model, _batch(model, 130, seed=8, pad_tail=20), GM.rand_idx(129, seed=3), "padtail"))
+    m.update(_vs_dropin(model, _batch(model, 4, seed=9), GM.rand_idx(3), "S3"))
     # two accumulated micro-batches with different indices == the sum of their separate gradients
     a, b = _batch(model, 130, seed=21), _batch(model, 130, seed=22)
-    ia, ib = _rand_idx(129, seed=1), _rand_idx(129, seed=2)
+    ia, ib = GM.rand_idx(129, seed=1), GM.rand_idx(129, seed=2)
     _, ga = _fused(model, a, ia)
     _, gb = _fused(model, b, ib)
     calls = []
     model.training_loss(a, sample_idx=ia)
     model.training_loss(b, sample_idx=ib, accumulate=True, grad_ready=lambda lo, hi: calls.append((lo, hi)))
-    gsum = {n: (ga[n] + gb[n]).to(torch.bfloat16).float() for n in ga}
+    gsum = {n: (ga[n].float() + gb[n].float()).to(BF) for n in ga}
     m["accum_grad_rel"] = _rel(_grads(model), gsum)
     # grad_ready hands over [0, numel) exactly once
     cover = torch.zeros(model._rt().store.numel, dtype=torch.int32)
     for lo, hi in calls:
         cover[lo:hi] += 1
     m["grad_ready_cover_error"] = float((cover != 1).sum())
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 @pytest.mark.gpu
@@ -212,7 +173,7 @@ def test_argmax_hits_kernel_matches_torch_argmax():
             got = ops.argmax_hits(L[:n], tt, V, pad)
             m[f"argmax_mismatch_{tag}_{n}"] = float((got != want).sum())
     m["argmax_mismatch_empty"] = float((ops.argmax_hits(L[:0], ref[:0], V, pad) != 0).sum())
-    _assert_within(m)
+    assert_within(m, BOUNDS)
 
 
 @pytest.mark.gpu
@@ -239,4 +200,4 @@ def test_validation_metrics(model):
     l_e, a_e = model.validation_metrics(torch.full_like(batch, tok.pad_id))
     m["val_empty_not_nan"] = float(not (torch.isnan(l_e) and torch.isnan(a_e)))
     print("val loss", float(loss), "acc", float(acc))
-    _assert_within(m)
+    assert_within(m, BOUNDS)
