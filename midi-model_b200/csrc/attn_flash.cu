@@ -8,6 +8,7 @@
 // XOR-swizzled shared memory.  q/k/v are addressed through (batch, row, head) strides so the same
 // kernels read the packed [rows, 3*hidden] qkv activation of training and the KV cache of prefill.
 #include "common.cuh"
+#include "rope.cuh"
 
 namespace {
 
@@ -261,8 +262,8 @@ flash_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const b
 // ============================================================================================
 // backward
 // ============================================================================================
-// Optional fused RoPE backward: the gradient w.r.t. the *pre-rotation* q / k is R^T applied to the accumulators
-// (dx1 = d1*c + d2*s, dx2 = d2*c - d1*s on the (d, d+32) pairs = accumulator blocks (nb, nb+4) of the same thread).
+// Optional fused RoPE backward: the gradient w.r.t. the *pre-rotation* q / k, on the accumulators; the (d, d+32) pairs
+// are accumulator blocks (nb, nb+4) of the same thread.
 __device__ __forceinline__ void rope_bwd_acc(float acc[8][4], int r, const bf16* __restrict__ cos_t,
                                              const bf16* __restrict__ sin_t, int pos, int t) {
 #pragma unroll
@@ -271,10 +272,10 @@ __device__ __forceinline__ void rope_bwd_acc(float acc[8][4], int r, const bf16*
         const float2 sn = __bfloat1622float2(*reinterpret_cast<const bf162*>(sin_t + (size_t)pos * 32 + nb * 8 + 2 * t));
         const float a0 = acc[nb][2 * r], a1 = acc[nb][2 * r + 1];
         const float b0 = acc[nb + 4][2 * r], b1 = acc[nb + 4][2 * r + 1];
-        acc[nb][2 * r] = a0 * c.x + b0 * sn.x;
-        acc[nb][2 * r + 1] = a1 * c.y + b1 * sn.y;
-        acc[nb + 4][2 * r] = b0 * c.x - a0 * sn.x;
-        acc[nb + 4][2 * r + 1] = b1 * c.y - a1 * sn.y;
+        acc[nb][2 * r] = rope_bwd_elem(a0, b0, c.x, sn.x, false);
+        acc[nb][2 * r + 1] = rope_bwd_elem(a1, b1, c.y, sn.y, false);
+        acc[nb + 4][2 * r] = rope_bwd_elem(b0, a0, c.x, sn.x, true);
+        acc[nb + 4][2 * r + 1] = rope_bwd_elem(b1, a1, c.y, sn.y, true);
     }
 }
 

@@ -5,6 +5,7 @@
 // shuffles, softmax is fp32, P is rounded to bf16 before P.V (flash semantics, DESIGN.md 3.3).
 // HBM-bound: reads the packed qkv rows once, writes the output once.
 #include "common.cuh"
+#include "rope.cuh"
 
 namespace {
 
@@ -33,35 +34,22 @@ __device__ __forceinline__ void axpy8(float* acc, float a, const uint4& x) {
     }
 }
 
-// Fused RoPE backward (d = 256): lane l holds d = 8l..8l+7; the rotation pairs (d, d+128) live in lanes l and l^16.
-// dx1 = d1*c + d2*s (first half), dx2 = d2*c - d1*s (second half); tables are [pos][128].
-__device__ __forceinline__ void rope_bwd_lane(float* acc, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
-                                              int pos, int lane) {
+// RoPE backward / forward on the lane's slice of head_dim 256 at position pos (tables are [pos][128])
+__device__ __forceinline__ void rope_bwd_slice(float* acc, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                                               int pos, int lane) {
     float c[8], sn[8];
     unpack8(*reinterpret_cast<const uint4*>(cos_t + (size_t)pos * (TD / 2) + (lane & 15) * 8), c);
     unpack8(*reinterpret_cast<const uint4*>(sin_t + (size_t)pos * (TD / 2) + (lane & 15) * 8), sn);
-    const bool first = lane < 16;
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-        const float other = __shfl_xor_sync(0xffffffffu, acc[j], 16);
-        acc[j] = first ? acc[j] * c[j] + other * sn[j] : acc[j] * c[j] - other * sn[j];
-    }
+    rope_bwd_lane(acc, c, sn, lane);
 }
-
-// forward RoPE on one 8-wide slice: lanes l and l^16 hold the (d, d+128) pairs
-__device__ __forceinline__ uint4 rope_fwd_lane(const uint4& x, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
-                                               int pos, int lane) {
-    float v[8], c[8], sn[8], o[8];
+__device__ __forceinline__ uint4 rope_fwd_slice(const uint4& x, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                                                int pos, int lane) {
+    float v[8], c[8], sn[8];
     unpack8(x, v);
     unpack8(*reinterpret_cast<const uint4*>(cos_t + (size_t)pos * (TD / 2) + (lane & 15) * 8), c);
     unpack8(*reinterpret_cast<const uint4*>(sin_t + (size_t)pos * (TD / 2) + (lane & 15) * 8), sn);
-    const bool lo = lane < 16;
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-        const float other = __shfl_xor_sync(0xffffffffu, v[j], 16);
-        o[j] = bf16_round(v[j] * c[j]) + bf16_round((lo ? -other : other) * sn[j]);
-    }
-    return pack8(o);
+    rope_fwd_lane(v, c, sn, lane);
+    return pack8(v);
 }
 
 // causal softmax over s[i][0..i] (scaled scores); returns fp32 probabilities in place
@@ -102,12 +90,12 @@ tiny_attn_fwd_kernel(bf16* __restrict__ qkv, bf16* __restrict__ out, int n_event
         k[i] = *reinterpret_cast<const uint4*>(base + (size_t)i * ld_qkv + H);
     }
     if (rope_cos) {
-        // fused RoPE (hf :146-168, three roundings): this warp owns the (event, head) slice, so q and k are rotated in
-        // registers and written back in place -- the saved activation is post-RoPE, as the backward pass expects
+        // fused RoPE: this warp owns the (event, head) slice, so q and k are rotated in registers and written back in
+        // place -- the saved activation is post-RoPE, as the backward pass expects
 #pragma unroll
         for (int i = 0; i < L; i++) {
-            q[i] = rope_fwd_lane(q[i], rope_cos, rope_sin, i, lane);
-            k[i] = rope_fwd_lane(k[i], rope_cos, rope_sin, i, lane);
+            q[i] = rope_fwd_slice(q[i], rope_cos, rope_sin, i, lane);
+            k[i] = rope_fwd_slice(k[i], rope_cos, rope_sin, i, lane);
             *reinterpret_cast<uint4*>(base + (size_t)i * ld_qkv) = q[i];
             *reinterpret_cast<uint4*>(base + (size_t)i * ld_qkv + H) = k[i];
         }
@@ -199,7 +187,7 @@ tiny_attn_bwd_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ d_ou
             float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 #pragma unroll
             for (int j = 0; j <= i; j++) axpy8(acc, ds[i][j], k[j]);
-            if (rope_cos) rope_bwd_lane(acc, rope_cos, rope_sin, i, lane);
+            if (rope_cos) rope_bwd_slice(acc, rope_cos, rope_sin, i, lane);
             *reinterpret_cast<uint4*>(dbase + (size_t)i * ld_qkv) = pack8(acc);
         }
     }
@@ -212,7 +200,7 @@ tiny_attn_bwd_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ d_ou
             float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 #pragma unroll
             for (int i = j; i < L; i++) axpy8(acc, ds[i][j], q[i]);
-            if (rope_cos) rope_bwd_lane(acc, rope_cos, rope_sin, j, lane);
+            if (rope_cos) rope_bwd_slice(acc, rope_cos, rope_sin, j, lane);
             *reinterpret_cast<uint4*>(dbase + (size_t)j * ld_qkv + H) = pack8(acc);
         }
     }

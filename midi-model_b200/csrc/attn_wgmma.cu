@@ -13,16 +13,18 @@
 // Segment mode (SEG = true): one packed "batch" of N rows holding several sequences, each a segment of whole 64-row
 // tiles.  seg[2 t] / seg[2 t + 1] = first / last tile of tile t's segment: a query tile's key loop starts at its
 // segment's first tile, a key tile's query loop ends at its segment's last tile, so no tile mixes sequences and the
-// causal mask inside a tile is the unsegmented one.  RoPE positions are in-segment (row - 64 * first).  `order` lists
+// causal mask inside a tile is the unsegmented one.  RoPE positions are in-segment (rope.cuh).  `order` lists
 // the tiles by descending loop length (longest first, as the unsegmented grids run them).
 // Same semantics as the mma.sync kernels of attn_flash.cu, which the tests use as the second implementation.
 #include "hopper.cuh"
+#include "rope.cuh"
 
 namespace {
 using namespace hopper;
 
 constexpr int D = 64;
 constexpr int T = 64;                  // rows per tile (queries or keys)
+static_assert(T == SEG_TILE, "segments are whole tiles");
 constexpr int NT = 128;                // one warpgroup
 constexpr int TILE_BYTES = T * D * 2;  // 8 KB
 constexpr float LOG2E = 1.4426950408889634f;
@@ -75,10 +77,10 @@ __device__ __forceinline__ void rope_bwd(float* acc, int h, const bf16* __restri
         float* a = acc + 4 * nb + 2 * h;
         float* b = acc + 4 * (nb + 4) + 2 * h;
         const float a0 = a[0], a1 = a[1], b0 = b[0], b1 = b[1];
-        a[0] = a0 * c.x + b0 * sn.x;
-        a[1] = a1 * c.y + b1 * sn.y;
-        b[0] = b0 * c.x - a0 * sn.x;
-        b[1] = b1 * c.y - a1 * sn.y;
+        a[0] = rope_bwd_elem(a0, b0, c.x, sn.x, false);
+        a[1] = rope_bwd_elem(a1, b1, c.y, sn.y, false);
+        b[0] = rope_bwd_elem(b0, a0, c.x, sn.x, true);
+        b[1] = rope_bwd_elem(b1, a1, c.y, sn.y, true);
     }
 }
 
@@ -208,7 +210,7 @@ attn_bwd_dkv_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_
     const int k0 = k_blk * T;
     const int q_first = max(0, k0 - p.off) / T;
     const int q_end = SEG ? seg[2 * k_blk + 1] + 1 : (p.Sq + T - 1) / T;
-    const int pos0 = SEG ? seg[2 * k_blk] * T : 0;                  // RoPE position of row r: r - pos0
+    const int pos0 = SEG ? seg_first_row(seg, k_blk) : 0;           // RoPE position of row r: r - pos0
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, cq = 2 * (lane & 3);
     const float* lse_g = lse + (long long)bh * p.Sq;
     const float* del_g = delta + (long long)bh * p.Sq;
@@ -364,7 +366,7 @@ attn_bwd_dq_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_c
     for (int hh = 0; hh < 2; hh++) {
         const int q = q0 + r0 + 8 * hh;
         if (q < p.Sq) {
-            if (rope_cos) rope_bwd(dqacc, hh, rope_cos, rope_sin, q + p.off - (SEG ? seg[2 * q_blk] * T : 0), cq);
+            if (rope_cos) rope_bwd(dqacc, hh, rope_cos, rope_sin, q + p.off - (SEG ? seg_first_row(seg, q_blk) : 0), cq);
             bf16* dst = dq + b * sdq.b + (long long)q * sdq.r + h * sdq.h + cq;
 #pragma unroll
             for (int g = 0; g < 8; g++)

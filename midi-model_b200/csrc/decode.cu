@@ -7,6 +7,7 @@
 //  * fused sampler: temperature, full-vocab softmax, grammar range / mask, top-p, top-k, draw
 //    (midi_model.py:222-223 + 152-165), one CTA per row, bitonic sort of the non-zero entries only.
 #include "common.cuh"
+#include "rope.cuh"
 #include "sampler.cuh"
 
 namespace {
@@ -345,7 +346,7 @@ decode_attn_kernel(const bf16* __restrict__ q, KVLayout L, float* __restrict__ p
     attend_chunk<D>(s_q_sh, CacheRows{L, b, h}, t0, t1, scale, pout, false, [] { return (bf16*)nullptr; });
 }
 
-// Fused single-token attention step: RoPE on the new q and k (hf :146-168, same three roundings as rope_kernel), append
+// Fused single-token attention step: RoPE on the new q and k (rope.cuh, as rope_kernel), append
 // k / v to the paged cache (hf cache_utils.py:119-120) and attend over positions 0 .. pos -- one launch instead of
 // rope + kv_append + attention (+ combine when n_split == 1).  qkv: [batch, 3*H] pre-RoPE rows of the new token.
 template <int D>
@@ -371,13 +372,13 @@ decode_attn_fused_kernel(const bf16* __restrict__ qkv, KVLayout L, const bf16* _
         const float c = __bfloat162float(cos_t[(size_t)pos * (D / 2) + i]), sn = __bfloat162float(sin_t[(size_t)pos * (D / 2) + i]);
         {
             const float x1 = __bfloat162float(row[h * D + i]), x2 = __bfloat162float(row[h * D + i + D / 2]);
-            s_q[i] = __float2bfloat16_rn(bf16_round(x1 * c) + bf16_round(-x2 * sn));
-            s_q[i + D / 2] = __float2bfloat16_rn(bf16_round(x2 * c) + bf16_round(x1 * sn));
+            s_q[i] = __float2bfloat16_rn(rope_fwd_elem(x1, x2, c, sn, false));
+            s_q[i + D / 2] = __float2bfloat16_rn(rope_fwd_elem(x2, x1, c, sn, true));
         }
         if (owns_new) {
             const float x1 = __bfloat162float(row[H + h * D + i]), x2 = __bfloat162float(row[H + h * D + i + D / 2]);
-            s_k[i] = __float2bfloat16_rn(bf16_round(x1 * c) + bf16_round(-x2 * sn));
-            s_k[i + D / 2] = __float2bfloat16_rn(bf16_round(x2 * c) + bf16_round(x1 * sn));
+            s_k[i] = __float2bfloat16_rn(rope_fwd_elem(x1, x2, c, sn, false));
+            s_k[i + D / 2] = __float2bfloat16_rn(rope_fwd_elem(x2, x1, c, sn, true));
             s_v[i] = row[2 * H + h * D + i];
             s_v[i + D / 2] = row[2 * H + h * D + i + D / 2];
         }
@@ -416,20 +417,19 @@ decode_attn_small_kernel(const bf16* __restrict__ qkv, KVLayout L, const bf16* _
     const int pos = (pos_dev ? *pos_dev : 0) + pos0;
     const int H = L.n_heads * D;
     const bf16* row = qkv + (size_t)b * ldq + h * D;
-    // RoPE pairs (d, d + D/2) live in lanes l and l ^ 16
+    // RoPE pairs (d, d + D/2) live in lanes l and l ^ 16.  q and k are rotated in one loop rather than by two calls of
+    // rope_fwd_lane: the compiler schedules the shuffles of both together
     float qv[8], kv_[8], cs[8], sn[8];
     unpack8(*reinterpret_cast<const uint4*>(row + lane * 8), qv);
     unpack8(*reinterpret_cast<const uint4*>(row + H + lane * 8), kv_);
     unpack8(*reinterpret_cast<const uint4*>(cos_t + (size_t)pos * (D / 2) + (lane & 15) * 8), cs);
     unpack8(*reinterpret_cast<const uint4*>(sin_t + (size_t)pos * (D / 2) + (lane & 15) * 8), sn);
-    const bool lo = lane < 16;
     float qr[8], kr[8];
 #pragma unroll
     for (int j = 0; j < 8; j++) {
         const float qo = __shfl_xor_sync(0xffffffffu, qv[j], 16), ko = __shfl_xor_sync(0xffffffffu, kv_[j], 16);
-        // first half: x1*c + (-x2)*s ; second half: x2*c + x1*s   (other = the partner element)
-        qr[j] = bf16_round(bf16_round(qv[j] * cs[j]) + bf16_round((lo ? -qo : qo) * sn[j]));
-        kr[j] = bf16_round(bf16_round(kv_[j] * cs[j]) + bf16_round((lo ? -ko : ko) * sn[j]));
+        qr[j] = bf16_round(rope_fwd_elem(qv[j], qo, cs[j], sn[j], lane >= 16));
+        kr[j] = bf16_round(rope_fwd_elem(kv_[j], ko, cs[j], sn[j], lane >= 16));
     }
     const uint4 k_new = pack8(kr);
     const uint4 v_new = *reinterpret_cast<const uint4*>(row + 2 * H + lane * 8);

@@ -18,6 +18,7 @@
 #include <cooperative_groups.h>
 
 #include "common.cuh"
+#include "rope.cuh"
 #include "sampler.cuh"
 #include "../../include/midi_b200.h"
 
@@ -343,15 +344,15 @@ __device__ __noinline__ void outer_attention(const PD& p, int layer, int pos, in
         {
             const float x1 = __bfloat162float(__ushort_as_bfloat16(__ldcg(reinterpret_cast<const unsigned short*>(row + h * D + lane))));
             const float x2 = __bfloat162float(__ushort_as_bfloat16(__ldcg(reinterpret_cast<const unsigned short*>(row + h * D + lane + 32))));
-            q_s[lane] = bf16_round(bf16_round(x1 * cs) + bf16_round(-x2 * sn));
-            q_s[lane + 32] = bf16_round(bf16_round(x2 * cs) + bf16_round(x1 * sn));
+            q_s[lane] = bf16_round(rope_fwd_elem(x1, x2, cs, sn, false));
+            q_s[lane + 32] = bf16_round(rope_fwd_elem(x2, x1, cs, sn, true));
         }
         const bool owns_new = (t0 <= pos && pos < t1);
         if (owns_new) {   // RoPE(k), v of the new position: used from shared memory here and appended to the cache
             const float x1 = __bfloat162float(__ushort_as_bfloat16(__ldcg(reinterpret_cast<const unsigned short*>(row + H + h * D + lane))));
             const float x2 = __bfloat162float(__ushort_as_bfloat16(__ldcg(reinterpret_cast<const unsigned short*>(row + H + h * D + lane + 32))));
-            kn_s[lane] = __float2bfloat16_rn(bf16_round(x1 * cs) + bf16_round(-x2 * sn));
-            kn_s[lane + 32] = __float2bfloat16_rn(bf16_round(x2 * cs) + bf16_round(x1 * sn));
+            kn_s[lane] = __float2bfloat16_rn(rope_fwd_elem(x1, x2, cs, sn, false));
+            kn_s[lane + 32] = __float2bfloat16_rn(rope_fwd_elem(x2, x1, cs, sn, true));
             vn_s[lane] = __ushort_as_bfloat16(__ldcg(reinterpret_cast<const unsigned short*>(row + 2 * H + h * D + lane)));
             vn_s[lane + 32] = __ushort_as_bfloat16(__ldcg(reinterpret_cast<const unsigned short*>(row + 2 * H + h * D + lane + 32)));
         }
@@ -484,13 +485,13 @@ __device__ __noinline__ void inner_attention(const PD& p, int layer, int step, i
         unpack8(ldcg16(row + H + lane * 8), kv_);
         unpack8(*reinterpret_cast<const uint4*>(d.cos_inner + (size_t)step * (D / 2) + (lane & 15) * 8), cs);
         unpack8(*reinterpret_cast<const uint4*>(d.sin_inner + (size_t)step * (D / 2) + (lane & 15) * 8), sn);
-        const bool lo = lane < 16;
+        // q and k rotated in one loop, as in decode_attn_small_kernel: two calls of rope_fwd_lane spill 16 more bytes here
         float qr[8], kr[8];
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             const float qo = __shfl_xor_sync(0xffffffffu, qv[j], 16), ko = __shfl_xor_sync(0xffffffffu, kv_[j], 16);
-            qr[j] = bf16_round(bf16_round(qv[j] * cs[j]) + bf16_round((lo ? -qo : qo) * sn[j]));
-            kr[j] = bf16_round(bf16_round(kv_[j] * cs[j]) + bf16_round((lo ? -ko : ko) * sn[j]));
+            qr[j] = bf16_round(rope_fwd_elem(qv[j], qo, cs[j], sn[j], lane >= 16));
+            kr[j] = bf16_round(rope_fwd_elem(kv_[j], ko, cs[j], sn[j], lane >= 16));
         }
         const uint4 k_new = pack8(kr);
         const uint4 v_new = ldcg16(row + 2 * H + lane * 8);

@@ -4,6 +4,7 @@
 // bf16 storage with the reference's rounding points (DESIGN.md 3.3).  16-byte vector
 // accesses, one 128-thread CTA per row (rows are 2 KB at hidden=1024), grids sized in rows.
 #include "common.cuh"
+#include "rope.cuh"
 
 namespace {
 
@@ -501,15 +502,13 @@ __global__ void rope_table_kernel(const float* __restrict__ inv_freq, int half, 
 }
 
 // In place on the q and k thirds of packed qkv rows [rows, 3*H]; position of row r = pos0 (+ *pos0_dev) + r % S
-// (the tables cover absolute positions), or with a segment table r - 64 * seg[2 * (r / 64)] (first row of r's segment).
-// forward : o1 = bf16(bf16(x1*c) + bf16(-x2*s)), o2 = bf16(bf16(x2*c) + bf16(x1*s))   (three roundings, A.4)
-// backward: dx1 = do1*c + do2*s, dx2 = do2*c - do1*s  (one rounding)
+// (the tables cover absolute positions), or its in-segment position with a segment table (rope.cuh).
 template <bool BWD>
 __global__ void rope_kernel(bf16* __restrict__ qkv, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
                             int rows, int S, int H, int D, int ld, int pos0, const int* __restrict__ pos0_dev,
                             const int* __restrict__ seg) {
     const int r = blockIdx.x;
-    const int s = seg ? r - 64 * seg[2 * (r >> 6)] : pos0 + (pos0_dev ? *pos0_dev : 0) + r % S;
+    const int s = seg ? seg_pos(seg, r) : pos0 + (pos0_dev ? *pos0_dev : 0) + r % S;
     const int half = D / 2;
     const int vec_per_head = half / 8;
     const int heads2 = 2 * (H / D);   // q heads then k heads (k third starts at column H)
@@ -527,11 +526,11 @@ __global__ void rope_kernel(bf16* __restrict__ qkv, const bf16* __restrict__ cos
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             if (!BWD) {
-                o1[j] = bf16_round(x1[j] * c[j]) + bf16_round(-x2[j] * sn[j]);
-                o2[j] = bf16_round(x2[j] * c[j]) + bf16_round(x1[j] * sn[j]);
+                o1[j] = rope_fwd_elem(x1[j], x2[j], c[j], sn[j], false);
+                o2[j] = rope_fwd_elem(x2[j], x1[j], c[j], sn[j], true);
             } else {
-                o1[j] = x1[j] * c[j] + x2[j] * sn[j];
-                o2[j] = x2[j] * c[j] - x1[j] * sn[j];
+                o1[j] = rope_bwd_elem(x1[j], x2[j], c[j], sn[j], false);
+                o2[j] = rope_bwd_elem(x2[j], x1[j], c[j], sn[j], true);
             }
         }
         *reinterpret_cast<uint4*>(p1) = pack8(o1);
@@ -867,7 +866,7 @@ extern "C" int b200_rope_qk(void* qkv, const void* cos_t, const void* sin_t, int
 extern "C" int b200_rope_qk_seg(void* qkv, const void* cos_t, const void* sin_t, int rows, const int* seg, int H, int D,
                                 int ld, int backward, cudaStream_t stream) {
     B200_CHECK_ARG(D % 16 == 0 && H % D == 0 && ld % 8 == 0, "rope_seg: head_dim must be a multiple of 16");
-    B200_CHECK_ARG(rows % 64 == 0 && (rows == 0 || seg), "rope_seg: rows (%d) must be whole 64-row tiles of a segment table",
+    B200_CHECK_ARG(rows % SEG_TILE == 0 && (rows == 0 || seg), "rope_seg: rows (%d) must be whole 64-row tiles of a segment table",
                    rows);
     if (rows == 0) return B200_OK;
     if (backward)

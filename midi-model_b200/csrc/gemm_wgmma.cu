@@ -12,6 +12,7 @@
 #include <math.h>
 
 #include "hopper.cuh"
+#include "rope.cuh"
 
 namespace {
 
@@ -23,6 +24,17 @@ constexpr int NUM_THREADS = CONSUMERS * 128 + 32;       // + the producer warp
 constexpr int EPI_BOX_BYTES = 64 * 64 * 2;              // one 64-row x 64-column bf16 box of the TMA store
 
 enum { EPI_STORE = 0, EPI_RESIDUAL = 1, EPI_PARTIAL_F32 = 2, EPI_ROPE = 3, EPI_SWIGLU = 4 };
+
+// EPI_ROPE: rotary embedding applied to columns [0, cols) (the q and k thirds of a packed QKV row) in heads of D columns;
+// row r sits at position r % S, or at its in-segment position with a segment table
+struct RopeOperands { const bf16 *cos, *sin; const int* seg; int S, D, cols; };
+// EPI_SWIGLU: B = [gate | up] weight rows; tile n covers gate rows [128n, 128n+128) and up rows [I + 128n, ...), and
+// act[M, I] (pitch ld_act) is written besides gate|up
+struct SwigluOperands { bf16* act; int I, ld_act; };
+
+// The epilogue a GEMM call asks for: EPI_STORE (plain, residual or split-K, as its other arguments say), EPI_ROPE or
+// EPI_SWIGLU, with the operands of the last two
+struct Epilogue { int kind = EPI_STORE; RopeOperands rope = {}; SwigluOperands swiglu = {}; };
 
 struct GemmParams {
     bf16* C;
@@ -37,15 +49,8 @@ struct GemmParams {
     int tail_tile0, tail_splits, tail_kb, total_items;
     float* tail_ws;
     int m_tiles, n_tiles;
-    // EPI_ROPE: rotary embedding applied to columns [0, rope_cols) (the q and k thirds of a packed QKV row); row r sits at
-    // position r % rope_S, or r - 64 * rope_seg[2 * (r / 64)] with a segment table (segments of whole 64-row tiles)
-    const bf16* rope_cos;
-    const bf16* rope_sin;
-    const int* rope_seg;
-    int rope_S, rope_D, rope_cols;
-    // EPI_SWIGLU: B = [gate | up] weight rows; tile n covers gate rows [128n, 128n+128) and up rows [I + 128n, ...)
-    bf16* act;
-    int swiglu_I, ld_act;
+    RopeOperands rope;
+    SwigluOperands swiglu;
 };
 
 using namespace hopper;
@@ -99,29 +104,28 @@ __device__ __forceinline__ void wgmma_tile(float* acc, uint64_t da, uint64_t db,
 // Accumulator fragment of wgmma m64nN (fp32): thread (warp w of the warpgroup, lane l) holds, for every 8-column group
 // j, acc[4j + h] at row 16w + l/4 + 8 * (h >> 1), column 8j + 2 * (l % 4) + (h & 1).
 
-// RoPE on the fragment: x = bf16(acc) (the Linear's rounding), then o1 = bf16(bf16(x1*c) + bf16(-x2*s)),
-// o2 = bf16(bf16(x2*c) + bf16(x1*s)) on (d, d + D/2) pairs (hf modeling_llama.py:262-268).  A head of D <= BLOCK_N
-// columns never straddles a tile, so both halves of a pair sit in the same thread (groups j and j + HALF8).
+// RoPE on the fragment, of x = bf16(acc) (the Linear's rounding).  A head of D <= BLOCK_N columns never straddles a
+// tile, so both halves of a (d, d + D/2) pair sit in the same thread (groups j and j + HALF8).
 template <int BLOCK_N, int HALF8>
 __device__ __forceinline__ void rope_fragment(float* acc, const GemmParams& p, int n_blk, int row, int h, int cq) {
     if (row >= p.M) return;
-    const int pos = p.rope_seg ? row - 64 * p.rope_seg[2 * (row >> 6)] : row % p.rope_S;
+    const int pos = p.rope.seg ? seg_pos(p.rope.seg, row) : row % p.rope.S;
     const int half = HALF8 * 8;
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; j++) {
         if ((j / HALF8) & 1) continue;                          // second half of a head: done with its partner
         const int col = n_blk * BLOCK_N + 8 * j + cq;
-        if (col >= p.rope_cols) continue;
+        if (col >= p.rope.cols) continue;
         const int d = (8 * j) % half + cq;
-        const float2 cc = __bfloat1622float2(*reinterpret_cast<const bf162*>(p.rope_cos + (size_t)pos * half + d));
-        const float2 ss = __bfloat1622float2(*reinterpret_cast<const bf162*>(p.rope_sin + (size_t)pos * half + d));
+        const float2 cc = __bfloat1622float2(*reinterpret_cast<const bf162*>(p.rope.cos + (size_t)pos * half + d));
+        const float2 ss = __bfloat1622float2(*reinterpret_cast<const bf162*>(p.rope.sin + (size_t)pos * half + d));
 #pragma unroll
         for (int e = 0; e < 2; e++) {
             const float c = e ? cc.y : cc.x, s = e ? ss.y : ss.x;
             const float x1 = bf16_round(acc[4 * j + 2 * h + e]);
             const float x2 = bf16_round(acc[4 * (j + HALF8) + 2 * h + e]);
-            acc[4 * j + 2 * h + e] = bf16_round(x1 * c) + bf16_round(-x2 * s);
-            acc[4 * (j + HALF8) + 2 * h + e] = bf16_round(x2 * c) + bf16_round(x1 * s);
+            acc[4 * j + 2 * h + e] = rope_fwd_elem(x1, x2, c, s, false);
+            acc[4 * (j + HALF8) + 2 * h + e] = rope_fwd_elem(x2, x1, c, s, true);
         }
     }
 }
@@ -221,7 +225,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     if (!B_MN) {
                         if (BLOCK_N == 256 && p.epilogue == EPI_SWIGLU) {   // gate half | up half (tensor map box = 128 rows)
                             tma_load_2d(sB, &tmB, &full_bar[stage], kb * BLOCK_K, wi.n_blk * 128);
-                            tma_load_2d(sB + 128 * BLOCK_K * 2, &tmB, &full_bar[stage], kb * BLOCK_K, p.swiglu_I + wi.n_blk * 128);
+                            tma_load_2d(sB + 128 * BLOCK_K * 2, &tmB, &full_bar[stage], kb * BLOCK_K, p.swiglu.I + wi.n_blk * 128);
                         } else {
                             tma_load_2d(sB, &tmB, &full_bar[stage], kb * BLOCK_K, wi.n_blk * BLOCK_N);
                         }
@@ -312,8 +316,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 const int row = row0 + r_lo + 8 * h;
-                if (p.rope_D == 64) rope_fragment<BLOCK_N, 4>(acc, p, wi.n_blk, row, h, cq);
-                else if (p.rope_D == 128) rope_fragment<BLOCK_N, 8>(acc, p, wi.n_blk, row, h, cq);
+                if (p.rope.D == 64) rope_fragment<BLOCK_N, 4>(acc, p, wi.n_blk, row, h, cq);
+                else if (p.rope.D == 128) rope_fragment<BLOCK_N, 8>(acc, p, wi.n_blk, row, h, cq);
                 else rope_fragment<BLOCK_N, 16>(acc, p, wi.n_blk, row, h, cq);
             }
         }
@@ -332,7 +336,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
 #pragma unroll
             for (int q = 0; q < 2; q++) {
-                store_box(staging, boxes, &tmC, p.swiglu_I + f0 + 64 * q, row0, wg, r_lo, lane, elected, nullptr, 0, 0, 0,
+                store_box(staging, boxes, &tmC, p.swiglu.I + f0 + 64 * q, row0, wg, r_lo, lane, elected, nullptr, 0, 0, 0,
                           [&](int jj, int h, uint32_t) {
                     const int j = 16 + 8 * q + jj;
                     return pack2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
@@ -612,14 +616,13 @@ extern "C" int b200_gemm_suggest_splits(int M, int N, int K, int block_n) {
 
 static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda, int ldb, int ldc,
                      int ldr, int a_mn_major, int b_mn_major, int accumulate, int block_n, int splits, void* workspace,
-                     size_t workspace_bytes, const bf16* rope_cos, const bf16* rope_sin, int rope_S, int rope_D,
-                     int rope_cols, cudaStream_t stream, const int* rope_seg = nullptr);
+                     size_t workspace_bytes, const Epilogue& epi, cudaStream_t stream);
 
 extern "C" int b200_gemm_bf16(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda, int ldb,
                               int ldc, int ldr, int a_mn_major, int b_mn_major, int accumulate, int block_n, int splits,
                               void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     return gemm_impl(A, B, C, R, M, N, K, lda, ldb, ldc, ldr, a_mn_major, b_mn_major, accumulate, block_n, splits, workspace,
-                     workspace_bytes, nullptr, nullptr, 0, 0, 0, stream);
+                     workspace_bytes, Epilogue{}, stream);
 }
 
 // Fused QKV projection + RoPE: C[M,N] = rope(A . B^T) with both operands K-major; rows are positions r % S of their
@@ -630,20 +633,20 @@ extern "C" int b200_gemm_bf16_rope(const void* A, const void* B, void* C, int M,
     B200_CHECK_ARG(head_dim == 64 || head_dim == 128 || head_dim == 256, "gemm_rope: head_dim %d unsupported", head_dim);
     B200_CHECK_ARG(N % 256 == 0 && rope_cols % 256 == 0, "gemm_rope: N and rope_cols must be multiples of 256");
     B200_CHECK_ARG(S > 0 && rope_cos && rope_sin, "gemm_rope: missing tables");
-    return gemm_impl(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, 256, 1, nullptr, 0, (const bf16*)rope_cos,
-                     (const bf16*)rope_sin, S, head_dim, rope_cols, stream);
+    const Epilogue epi{EPI_ROPE, {(const bf16*)rope_cos, (const bf16*)rope_sin, nullptr, S, head_dim, rope_cols}};
+    return gemm_impl(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, 256, 1, nullptr, 0, epi, stream);
 }
 
-// The same with in-segment positions: row r sits at r - 64 * seg[2 * (r / 64)] (segments of whole 64-row tiles).
+// The same with in-segment positions (segments of whole 64-row tiles, rope.cuh).
 extern "C" int b200_gemm_bf16_rope_seg(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                                        const void* rope_cos, const void* rope_sin, const int* seg, int head_dim,
                                        int rope_cols, cudaStream_t stream) {
     B200_CHECK_ARG(head_dim == 64 || head_dim == 128 || head_dim == 256, "gemm_rope_seg: head_dim %d unsupported", head_dim);
     B200_CHECK_ARG(N % 256 == 0 && rope_cols % 256 == 0, "gemm_rope_seg: N and rope_cols must be multiples of 256");
-    B200_CHECK_ARG(M % 64 == 0 && seg && rope_cos && rope_sin, "gemm_rope_seg: M (%d) must be whole 64-row tiles; tables "
-                   "required", M);
-    return gemm_impl(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, 256, 1, nullptr, 0, (const bf16*)rope_cos,
-                     (const bf16*)rope_sin, 1, head_dim, rope_cols, stream, seg);
+    B200_CHECK_ARG(M % SEG_TILE == 0 && seg && rope_cos && rope_sin, "gemm_rope_seg: M (%d) must be whole 64-row tiles; "
+                   "tables required", M);
+    const Epilogue epi{EPI_ROPE, {(const bf16*)rope_cos, (const bf16*)rope_sin, seg, 1, head_dim, rope_cols}};
+    return gemm_impl(A, B, C, nullptr, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, 256, 1, nullptr, 0, epi, stream);
 }
 
 // Fused gate|up projection + SwiGLU: gu[M, 2I] = A . Wgu^T (stored, the backward pass needs g and u) and
@@ -652,15 +655,14 @@ extern "C" int b200_gemm_bf16_swiglu(const void* A, const void* Wgu, void* gu, v
                                      int ldw, int ld_gu, int ld_act, cudaStream_t stream) {
     B200_CHECK_ARG(I % 128 == 0, "gemm_swiglu: intermediate size %d must be a multiple of 128", I);
     B200_CHECK_ARG(ld_act % 8 == 0 && (uintptr_t)act % 16 == 0, "gemm_swiglu: act must be 16-byte aligned");
-    return gemm_impl(A, Wgu, gu, nullptr, M, 2 * I, K, lda, ldw, ld_gu, 0, 0, 0, 0, 256, 1, act, (size_t)I | ((size_t)ld_act << 32),
-                     nullptr, nullptr, -1, 0, 0, stream);
+    const Epilogue epi{EPI_SWIGLU, {}, {(bf16*)act, I, ld_act}};
+    return gemm_impl(A, Wgu, gu, nullptr, M, 2 * I, K, lda, ldw, ld_gu, 0, 0, 0, 0, 256, 1, nullptr, 0, epi, stream);
 }
 
 static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda, int ldb, int ldc,
                      int ldr, int a_mn_major, int b_mn_major, int accumulate, int block_n, int splits, void* workspace,
-                     size_t workspace_bytes, const bf16* rope_cos, const bf16* rope_sin, int rope_S, int rope_D,
-                     int rope_cols, cudaStream_t stream, const int* rope_seg) {
-    const bool swiglu = (rope_S == -1);      // internal marker set by b200_gemm_bf16_swiglu (workspace = act, bytes = I | ld<<32)
+                     size_t workspace_bytes, const Epilogue& epi, cudaStream_t stream) {
+    const bool swiglu = epi.kind == EPI_SWIGLU;
     B200_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
     // N need not be a multiple of 8: B rows >= N are out of bounds for the tensor map (zero-filled), so the
     // epilogue may store whole 16-byte vectors up to roundup8(N) (zeros) as long as the row pitch covers them.
@@ -696,16 +698,10 @@ static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M
     } else {
         p.epilogue = R ? EPI_RESIDUAL : EPI_STORE;
     }
-    p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.rope_seg = rope_seg; p.rope_S = rope_S; p.rope_D = rope_D; p.rope_cols = rope_cols;
-    if (rope_cos) p.epilogue = EPI_ROPE;
-    p.act = nullptr; p.swiglu_I = 0; p.ld_act = 0;
-    if (swiglu) {
-        p.epilogue = EPI_SWIGLU;
-        p.act = (bf16*)workspace;
-        p.swiglu_I = (int)(workspace_bytes & 0xffffffffu);
-        p.ld_act = (int)(workspace_bytes >> 32);
-        p.n_tiles = p.swiglu_I / 128;         // one tile = 128 gate + 128 up features
-    }
+    if (epi.kind != EPI_STORE) p.epilogue = epi.kind;
+    p.rope = epi.rope;
+    p.swiglu = epi.swiglu;
+    if (swiglu) p.n_tiles = p.swiglu.I / 128;   // one tile = 128 gate + 128 up features
 
     CUtensorMap tmA, tmB;
     int rc;
@@ -741,7 +737,7 @@ static int gemm_impl(const void* A, const void* B, void* C, const void* R, int M
         if (rc) return rc;
     }
     if (swiglu) {
-        rc = hopper::make_tmap_2d(&tmAct, p.act, p.swiglu_I, M, p.ld_act, 64, 64);
+        rc = hopper::make_tmap_2d(&tmAct, p.swiglu.act, p.swiglu.I, M, p.swiglu.ld_act, 64, 64);
         if (rc) return rc;
     }
 

@@ -197,7 +197,7 @@ def host_to_device(t: torch.Tensor, device) -> torch.Tensor:
     return t.pin_memory().to(device, non_blocking=True) if device.type == "cuda" else t
 
 
-SEG_TILE = 64   # rows per segment tile: the event-level attention's tile height (csrc/attn_wgmma.cu T)
+SEG_TILE = 64   # rows per segment tile: the event-level attention's tile height (csrc/rope.cuh SEG_TILE)
 
 
 @dataclass
@@ -432,8 +432,8 @@ class StackEngine:
         """Packed QKV projection of n1, the q/k/v adapters added BEFORE the rotation, and RoPE on the q and k thirds.
         rotate=False leaves the rotation to the token-level attention kernel (fused RoPE, the forward's default there);
         with `seg` rows sit at in-segment positions instead of r % S;
-        the stand-alone RoPE kernel performs the same three roundings (csrc/attn_tiny.cu rope_fwd_lane, csrc/elementwise.cu
-        rope_kernel), so a recompute that does not run attention gets the rotated q, k the forward's kernel wrote back."""
+        the stand-alone RoPE kernel performs the same three roundings (both use csrc/rope.cuh), so a recompute that does
+        not run attention gets the rotated q, k the forward's kernel wrote back."""
         H, D = self.cfg.hidden, self.cfg.head_dim
         lo = w.lora
         if FUSE_ROPE_FWD and not any(k in lo for k in ("q", "k", "v")):
