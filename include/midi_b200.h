@@ -92,6 +92,10 @@ int b200_rope_qk(void* qkv, const void* cos_t, const void* sin_t, int rows, int 
    row r sits at position r - 64 * seg[2 * (r / 64)] */
 int b200_rope_qk_seg(void* qkv, const void* cos_t, const void* sin_t, int rows, const int* seg, int H, int D, int ld,
                      int backward, cudaStream_t s);
+/* ragged generate (forward only): row r sits at pos0 (+ *pos0_dev) + row_off[r / S] + r % S; row_off device int32 [rows / S].
+   Precondition: every such position is >= 0 and inside the tables */
+int b200_rope_qk_ragged(void* qkv, const void* cos_t, const void* sin_t, int rows, int S, int H, int D, int ld, int pos0,
+                        const int* pos0_dev /*may be NULL*/, const int* row_off, cudaStream_t s);
 
 /* ---- SwiGLU (hf modeling_llama.py:183) on packed [rows, 2I] = [gate | up] ------------------------- */
 int b200_swiglu_fwd(const void* gu, void* act, long long rows, int I, cudaStream_t s);
@@ -236,6 +240,28 @@ int b200_uniform_fill(float* u, int n, unsigned long long seed, unsigned long lo
 /* graph-captured generate loop: commit the event sampled into ev_t [T][B] to seq[:, *pos+1] and ev_next; (*pos)++ */
 int b200_event_commit(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T, int max_len,
                       cudaStream_t s);
+/*      ragged generate: the entries above with a per-row position offset row_off (device int32 [batch], row_off[b] <= 0).
+ *      Row b's position is the shared position plus row_off[b]: its RoPE position, its KV slot, its attention length
+ *      (that position + 1) and its commit slot.  Preconditions (the caller's): pos + row_off[b] >= 0 and within row b's
+ *      pages and the RoPE tables.  The split grid (max_T, n_split) is the counterpart's; splits of a short row that hold no
+ *      key drop out of the combine pass.  row_off = all zeros gives the counterpart's results bit for bit.
+ *        kv_append_ragged:        row b's i-th new row goes to slot pos0 (+ *pos0_dev) + row_off[b] + i
+ *        attn_decode_ragged:      query row b*s_q + i attends keys 0 .. past (+ *past_dev) + row_off[b] + i
+ *        attn_decode_fused_ragged: RoPE, append and attention at row b's own position
+ *        event_commit_ragged:     writes seq[b, *pos + row_off[b] + 1]; *pos still advances by one */
+int b200_kv_append_ragged(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages, int page,
+                          int n_heads, int head_dim, int batch, int s_new, int pos0, const int* pos0_dev, int ld,
+                          const int* row_off, cudaStream_t s);
+int b200_attn_decode_ragged(const void* q, const void* k_pool, const void* v_pool, const int* block_table, int max_pages,
+                            int page, void* out, int batch, int s_q, int n_heads, int head_dim, int past,
+                            const int* past_dev, int max_T, int ldq, int ldo, float scale, int n_split, void* workspace,
+                            size_t workspace_bytes, const int* row_off, cudaStream_t s);
+int b200_attn_decode_fused_ragged(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages,
+                                  int page, const void* cos_t, const void* sin_t, void* out, int batch, int n_heads,
+                                  int head_dim, int pos0, const int* pos_dev, int max_T, int ldq, int ldo, float scale,
+                                  int n_split, void* workspace, size_t workspace_bytes, const int* row_off, cudaStream_t s);
+int b200_event_commit_ragged(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T,
+                             int max_len, const int* row_off, cudaStream_t s);
 
 
 /* ---- persistent generate kernel (midi_model.py:192-248: one generated event = event-level decode step + up to 8
@@ -277,6 +303,12 @@ size_t b200_decode_desc_bytes(void);            /* sizeof(b200_decode_desc): let
 size_t b200_decode_events_workspace_bytes(const b200_decode_desc* d);
 int b200_decode_events(const b200_decode_desc* d, int n_events, void* workspace /*256-byte aligned*/,
                        size_t workspace_bytes, cudaStream_t s);
+/*      ragged generate: as b200_decode_events, with row b at position *pos + row_off[b] (device int32 [batch], <= 0; see
+ *      b200_kv_append_ragged for the preconditions).  The shared *pos, its `*pos + 1 >= max_len` exit and the attention's
+ *      chunk grid (on *pos + 1) stay uniform across the grid; a short row's trailing chunks are empty and drop out of the
+ *      combine.  Row b commits to seq[b, *pos + row_off[b] + 1].  Same descriptor and workspace. */
+int b200_decode_events_ragged(const b200_decode_desc* d, const int* row_off, int n_events, void* workspace,
+                              size_t workspace_bytes, cudaStream_t s);
 
 #ifdef __cplusplus
 }

@@ -201,10 +201,14 @@ __device__ __forceinline__ size_t kv_off(const KVLayout& L, int b, int h, int t)
 }
 
 // copy the k / v thirds of packed qkv rows [batch*s_new, 3H] into the cache at positions pos0 .. pos0+s_new-1
-__global__ void kv_append_kernel(const bf16* __restrict__ qkv, KVLayout L, int s_new, int pos0, const int* pos0_dev, int ld) {
+// (RAGGED: row b's at pos0 + row_off[b] ..)
+template <bool RAGGED>
+__global__ void kv_append_kernel(const bf16* __restrict__ qkv, KVLayout L, int s_new, int pos0, const int* pos0_dev, int ld,
+                                 const int* __restrict__ row_off) {
     const int r = blockIdx.x;
     const int b = r / s_new, i = r % s_new;
-    const int t = (pos0_dev ? *pos0_dev : pos0) + i;
+    int t = (pos0_dev ? *pos0_dev : pos0) + i;
+    if constexpr (RAGGED) t += row_off[b];
     const int H = L.n_heads * L.D;
     const int vec_per_head = L.D / 8;
     for (int c = threadIdx.x; c < H / 8; c += blockDim.x) {
@@ -321,17 +325,18 @@ __device__ __forceinline__ void attend_chunk(const bf16* s_q, const Rows& rows, 
     }
 }
 
-// single-query attention over the cache.  Row r = b * s_q + i attends to keys 0 .. past + i.
+// single-query attention over the cache.  Row r = b * s_q + i attends to keys 0 .. past + i (RAGGED: past + row_off[b] + i).
 // grid (rows * n_heads, n_split); partial: [rows*n_heads][n_split][D + 2] = (m, l, o[D])
-template <int D>
+template <int D, bool RAGGED>
 __global__ void __launch_bounds__(128)
 decode_attn_kernel(const bf16* __restrict__ q, KVLayout L, float* __restrict__ partial, int s_q, int past,
-                   const int* past_dev, int ldq, float scale, int n_split) {
+                   const int* past_dev, int ldq, float scale, int n_split, const int* __restrict__ row_off) {
     __shared__ __align__(16) bf16 s_q_sh[D];
     const int rh = blockIdx.x;
     const int r = rh / L.n_heads, h = rh % L.n_heads;
     const int b = r / s_q, i = r % s_q;
-    const int T = (past_dev ? *past_dev : past) + i + 1;
+    int T = (past_dev ? *past_dev : past) + i + 1;
+    if constexpr (RAGGED) T += row_off[b];
     const int chunk = (T + n_split - 1) / n_split;
     const int t0 = blockIdx.y * chunk;
     const int t1 = min(T, t0 + chunk);
@@ -349,17 +354,19 @@ decode_attn_kernel(const bf16* __restrict__ q, KVLayout L, float* __restrict__ p
 // Fused single-token attention step: RoPE on the new q and k (rope.cuh, as rope_kernel), append
 // k / v to the paged cache (hf cache_utils.py:119-120) and attend over positions 0 .. pos -- one launch instead of
 // rope + kv_append + attention (+ combine when n_split == 1).  qkv: [batch, 3*H] pre-RoPE rows of the new token.
-template <int D>
+// RAGGED: row b's new token is at pos0 (+ *pos_dev) + row_off[b].
+template <int D, bool RAGGED>
 __global__ void __launch_bounds__(128)
 decode_attn_fused_kernel(const bf16* __restrict__ qkv, KVLayout L, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
                          float* __restrict__ partial, bf16* __restrict__ out, int pos0, const int* pos_dev, int ldq, int ldo,
-                         float scale, int n_split) {
+                         float scale, int n_split, const int* __restrict__ row_off) {
     __shared__ __align__(16) bf16 s_q[D];
     __shared__ __align__(16) bf16 s_k[D];
     __shared__ __align__(16) bf16 s_v[D];
     const int rh = blockIdx.x;
     const int b = rh / L.n_heads, h = rh % L.n_heads;
-    const int pos = (pos_dev ? *pos_dev : 0) + pos0;     // position of the new token
+    int pos = (pos_dev ? *pos_dev : 0) + pos0;           // position of the new token
+    if constexpr (RAGGED) pos += row_off[b];
     const int T = pos + 1;
     const int chunk = (T + n_split - 1) / n_split;
     const int t0 = blockIdx.y * chunk;
@@ -404,17 +411,19 @@ decode_attn_fused_kernel(const bf16* __restrict__ qkv, KVLayout L, const bf16* _
 // Token-level stack variant (context <= 32 positions): one WARP per (batch row, head); each lane owns D/32 consecutive
 // elements of q / k / v, scores are warp reductions, softmax lives in registers.  Same math and rounding points as
 // decode_attn_fused_kernel (RoPE three roundings, P rounded to bf16 before P.V).
-template <int D>
+template <int D, bool RAGGED>
 __global__ void __launch_bounds__(128)
 decode_attn_small_kernel(const bf16* __restrict__ qkv, KVLayout L, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
-                         bf16* __restrict__ out, int n_rows_heads, int pos0, const int* pos_dev, int ldq, int ldo, float scale) {
+                         bf16* __restrict__ out, int n_rows_heads, int pos0, const int* pos_dev, int ldq, int ldo, float scale,
+                         const int* __restrict__ row_off) {
     constexpr int E = D / 32;          // elements per lane (8 for D = 256)
     static_assert(E == 8, "one 16-byte vector per lane");
     const int wid = blockIdx.x * 4 + (threadIdx.x >> 5);
     if (wid >= n_rows_heads) return;
     const int lane = threadIdx.x & 31;
     const int b = wid / L.n_heads, h = wid % L.n_heads;
-    const int pos = (pos_dev ? *pos_dev : 0) + pos0;
+    int pos = (pos_dev ? *pos_dev : 0) + pos0;
+    if constexpr (RAGGED) pos += row_off[b];
     const int H = L.n_heads * D;
     const bf16* row = qkv + (size_t)b * ldq + h * D;
     // RoPE pairs (d, d + D/2) live in lanes l and l ^ 16.  q and k are rotated in one loop rather than by two calls of
@@ -571,14 +580,19 @@ __global__ void philox_uniform_kernel(float* __restrict__ u, int n, unsigned lon
 }
 
 // End of one generated event (graph-captured loop): ev_t [T][B] (token-major scratch written by the sampler)
-// -> seq[b, *pos + 1, :] and ev_next[b, :] (input of the next outer step); then (*pos)++.
+// -> seq[b, *pos + 1, :] (RAGGED: seq[b, *pos + row_off[b] + 1, :]) and ev_next[b, :] (input of the next outer step);
+// then (*pos)++.
+template <bool RAGGED>
 __global__ void event_commit_kernel(const long long* __restrict__ ev_t, long long* __restrict__ seq,
-                                    long long* __restrict__ ev_next, int* __restrict__ pos, int B, int T, int max_len) {
+                                    long long* __restrict__ ev_next, int* __restrict__ pos, int B, int T, int max_len,
+                                    const int* __restrict__ row_off) {
     const int p = *pos;
     for (int i = threadIdx.x; i < B * T; i += blockDim.x) {
         const int b = i / T, t = i % T;
         const long long v = ev_t[(size_t)t * B + b];
-        if (p + 1 < max_len) seq[((size_t)b * max_len + p + 1) * T + t] = v;
+        int q = p;
+        if constexpr (RAGGED) q += row_off[b];
+        if (q + 1 < max_len) seq[((size_t)b * max_len + q + 1) * T + t] = v;
         ev_next[(size_t)b * T + t] = v;
     }
     __syncthreads();
@@ -680,13 +694,16 @@ extern "C" int b200_gemv_fused(const void* x, const long long* ids, int ids_stri
     return B200_OK;
 }
 
-// one new token per batch row: RoPE(q,k) + KV append + attention over the cache (+ combine pass when n_split > 1)
-extern "C" int b200_attn_decode_fused(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages,
-                                      int page, const void* cos_t, const void* sin_t, void* out, int batch, int n_heads,
-                                      int head_dim, int pos0, const int* pos_dev, int max_T, int ldq, int ldo, float scale,
-                                      int n_split, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+namespace {
+
+template <bool RAGGED>
+int attn_decode_fused(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages, int page,
+                      const void* cos_t, const void* sin_t, void* out, int batch, int n_heads, int head_dim, int pos0,
+                      const int* pos_dev, int max_T, int ldq, int ldo, float scale, int n_split, void* workspace,
+                      size_t workspace_bytes, const int* row_off, cudaStream_t stream) {
     B200_CHECK_ARG(head_dim == 64 || head_dim == 256, "attn_decode_fused: head_dim %d unsupported", head_dim);
     if (batch == 0) return B200_OK;
+    B200_CHECK_ARG(!RAGGED || row_off, "attn_decode_fused_ragged: row_off required");
     if (n_split < 1) n_split = 1;
     B200_CHECK_ARG((max_T + n_split - 1) / n_split <= 1024, "attn_decode_fused: chunk per split exceeds 1024 keys");
     B200_CHECK_ARG(workspace_bytes >= b200_attn_decode_workspace_bytes(batch, n_heads, head_dim, n_split),
@@ -694,22 +711,22 @@ extern "C" int b200_attn_decode_fused(const void* qkv, void* k_pool, void* v_poo
     KVLayout L{(bf16*)k_pool, (bf16*)v_pool, block_table, max_pages, page, n_heads, head_dim};
     if (head_dim == 256 && max_T <= 32) {      // token-level stack: warp-per-head kernel
         const int n = batch * n_heads;
-        decode_attn_small_kernel<256><<<(n + 3) / 4, 128, 0, stream>>>((const bf16*)qkv, L, (const bf16*)cos_t, (const bf16*)sin_t,
-                                                                      (bf16*)out, n, pos0, pos_dev, ldq, ldo, scale);
+        decode_attn_small_kernel<256, RAGGED><<<(n + 3) / 4, 128, 0, stream>>>((const bf16*)qkv, L, (const bf16*)cos_t,
+            (const bf16*)sin_t, (bf16*)out, n, pos0, pos_dev, ldq, ldo, scale, row_off);
         B200_CHECK_LAUNCH("attn_decode_small");
         return B200_OK;
     }
     dim3 grid(batch * n_heads, n_split);
     if (head_dim == 64) {
-        decode_attn_fused_kernel<64><<<grid, 128, 0, stream>>>((const bf16*)qkv, L, (const bf16*)cos_t, (const bf16*)sin_t,
-            (float*)workspace, (bf16*)out, pos0, pos_dev, ldq, ldo, scale, n_split);
+        decode_attn_fused_kernel<64, RAGGED><<<grid, 128, 0, stream>>>((const bf16*)qkv, L, (const bf16*)cos_t, (const bf16*)sin_t,
+            (float*)workspace, (bf16*)out, pos0, pos_dev, ldq, ldo, scale, n_split, row_off);
         if (n_split > 1) {
             decode_attn_combine_kernel<64><<<batch * n_heads, 64, 0, stream>>>((const float*)workspace, (bf16*)out, n_heads, n_split, ldo);
             B200_COUNT_EXTRA(1);
         }
     } else {
-        decode_attn_fused_kernel<256><<<grid, 128, 0, stream>>>((const bf16*)qkv, L, (const bf16*)cos_t, (const bf16*)sin_t,
-            (float*)workspace, (bf16*)out, pos0, pos_dev, ldq, ldo, scale, n_split);
+        decode_attn_fused_kernel<256, RAGGED><<<grid, 128, 0, stream>>>((const bf16*)qkv, L, (const bf16*)cos_t, (const bf16*)sin_t,
+            (float*)workspace, (bf16*)out, pos0, pos_dev, ldq, ldo, scale, n_split, row_off);
         if (n_split > 1) {
             decode_attn_combine_kernel<256><<<batch * n_heads, 128, 0, stream>>>((const float*)workspace, (bf16*)out, n_heads, n_split, ldo);
             B200_COUNT_EXTRA(1);
@@ -719,15 +736,82 @@ extern "C" int b200_attn_decode_fused(const void* qkv, void* k_pool, void* v_poo
     return B200_OK;
 }
 
+template <bool RAGGED>
+int kv_append(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages, int page, int n_heads,
+              int head_dim, int batch, int s_new, int pos0, const int* pos0_dev, int ld, const int* row_off,
+              cudaStream_t stream) {
+    B200_CHECK_ARG(head_dim % 8 == 0, "kv_append: head_dim must be a multiple of 8");
+    if (batch * s_new == 0) return B200_OK;
+    B200_CHECK_ARG(!RAGGED || row_off, "kv_append_ragged: row_off required");
+    KVLayout L{(bf16*)k_pool, (bf16*)v_pool, block_table, max_pages, page, n_heads, head_dim};
+    kv_append_kernel<RAGGED><<<batch * s_new, 128, 0, stream>>>((const bf16*)qkv, L, s_new, pos0, pos0_dev, ld, row_off);
+    B200_CHECK_LAUNCH("kv_append");
+    return B200_OK;
+}
+
+template <bool RAGGED>
+int attn_decode(const void* q, const void* k_pool, const void* v_pool, const int* block_table, int max_pages, int page,
+                void* out, int batch, int s_q, int n_heads, int head_dim, int past, const int* past_dev, int max_T, int ldq,
+                int ldo, float scale, int n_split, void* workspace, size_t workspace_bytes, const int* row_off,
+                cudaStream_t stream) {
+    B200_CHECK_ARG(head_dim == 64 || head_dim == 256, "attn_decode: head_dim %d unsupported", head_dim);
+    const int rows = batch * s_q;
+    if (rows == 0) return B200_OK;
+    B200_CHECK_ARG(!RAGGED || row_off, "attn_decode_ragged: row_off required");
+    if (n_split < 1) n_split = 1;
+    B200_CHECK_ARG((max_T + n_split - 1) / n_split <= 1024, "attn_decode: chunk per split exceeds 1024 keys (raise n_split)");
+    B200_CHECK_ARG(workspace_bytes >= b200_attn_decode_workspace_bytes(rows, n_heads, head_dim, n_split),
+                   "attn_decode: workspace too small");
+    KVLayout L{(bf16*)k_pool, (bf16*)v_pool, block_table, max_pages, page, n_heads, head_dim};
+    dim3 grid(rows * n_heads, n_split);
+    if (head_dim == 64) {
+        decode_attn_kernel<64, RAGGED><<<grid, 128, 0, stream>>>((const bf16*)q, L, (float*)workspace, s_q, past, past_dev, ldq,
+                                                                 scale, n_split, row_off);
+        decode_attn_combine_kernel<64><<<rows * n_heads, 64, 0, stream>>>((const float*)workspace, (bf16*)out, n_heads, n_split, ldo);
+    } else {
+        decode_attn_kernel<256, RAGGED><<<grid, 128, 0, stream>>>((const bf16*)q, L, (float*)workspace, s_q, past, past_dev, ldq,
+                                                                  scale, n_split, row_off);
+        decode_attn_combine_kernel<256><<<rows * n_heads, 128, 0, stream>>>((const float*)workspace, (bf16*)out, n_heads, n_split, ldo);
+    }
+    B200_COUNT_EXTRA(1);
+    B200_CHECK_LAUNCH("attn_decode");
+    return B200_OK;
+}
+
+}   // namespace
+
+// one new token per batch row: RoPE(q,k) + KV append + attention over the cache (+ combine pass when n_split > 1)
+extern "C" int b200_attn_decode_fused(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages,
+                                      int page, const void* cos_t, const void* sin_t, void* out, int batch, int n_heads,
+                                      int head_dim, int pos0, const int* pos_dev, int max_T, int ldq, int ldo, float scale,
+                                      int n_split, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+    return attn_decode_fused<false>(qkv, k_pool, v_pool, block_table, max_pages, page, cos_t, sin_t, out, batch, n_heads,
+                                    head_dim, pos0, pos_dev, max_T, ldq, ldo, scale, n_split, workspace, workspace_bytes,
+                                    nullptr, stream);
+}
+
+extern "C" int b200_attn_decode_fused_ragged(const void* qkv, void* k_pool, void* v_pool, const int* block_table,
+                                             int max_pages, int page, const void* cos_t, const void* sin_t, void* out,
+                                             int batch, int n_heads, int head_dim, int pos0, const int* pos_dev, int max_T,
+                                             int ldq, int ldo, float scale, int n_split, void* workspace,
+                                             size_t workspace_bytes, const int* row_off, cudaStream_t stream) {
+    return attn_decode_fused<true>(qkv, k_pool, v_pool, block_table, max_pages, page, cos_t, sin_t, out, batch, n_heads,
+                                   head_dim, pos0, pos_dev, max_T, ldq, ldo, scale, n_split, workspace, workspace_bytes,
+                                   row_off, stream);
+}
+
 extern "C" int b200_kv_append(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages, int page,
                               int n_heads, int head_dim, int batch, int s_new, int pos0, const int* pos0_dev, int ld,
                               cudaStream_t stream) {
-    B200_CHECK_ARG(head_dim % 8 == 0, "kv_append: head_dim must be a multiple of 8");
-    if (batch * s_new == 0) return B200_OK;
-    KVLayout L{(bf16*)k_pool, (bf16*)v_pool, block_table, max_pages, page, n_heads, head_dim};
-    kv_append_kernel<<<batch * s_new, 128, 0, stream>>>((const bf16*)qkv, L, s_new, pos0, pos0_dev, ld);
-    B200_CHECK_LAUNCH("kv_append");
-    return B200_OK;
+    return kv_append<false>(qkv, k_pool, v_pool, block_table, max_pages, page, n_heads, head_dim, batch, s_new, pos0,
+                            pos0_dev, ld, nullptr, stream);
+}
+
+extern "C" int b200_kv_append_ragged(const void* qkv, void* k_pool, void* v_pool, const int* block_table, int max_pages,
+                                     int page, int n_heads, int head_dim, int batch, int s_new, int pos0,
+                                     const int* pos0_dev, int ld, const int* row_off, cudaStream_t stream) {
+    return kv_append<true>(qkv, k_pool, v_pool, block_table, max_pages, page, n_heads, head_dim, batch, s_new, pos0,
+                           pos0_dev, ld, row_off, stream);
 }
 
 extern "C" size_t b200_attn_decode_workspace_bytes(int rows, int n_heads, int head_dim, int n_split) {
@@ -739,25 +823,16 @@ extern "C" int b200_attn_decode(const void* q, const void* k_pool, const void* v
                                 int page, void* out, int batch, int s_q, int n_heads, int head_dim, int past,
                                 const int* past_dev, int max_T, int ldq, int ldo, float scale, int n_split, void* workspace,
                                 size_t workspace_bytes, cudaStream_t stream) {
-    B200_CHECK_ARG(head_dim == 64 || head_dim == 256, "attn_decode: head_dim %d unsupported", head_dim);
-    const int rows = batch * s_q;
-    if (rows == 0) return B200_OK;
-    if (n_split < 1) n_split = 1;
-    B200_CHECK_ARG((max_T + n_split - 1) / n_split <= 1024, "attn_decode: chunk per split exceeds 1024 keys (raise n_split)");
-    B200_CHECK_ARG(workspace_bytes >= b200_attn_decode_workspace_bytes(rows, n_heads, head_dim, n_split),
-                   "attn_decode: workspace too small");
-    KVLayout L{(bf16*)k_pool, (bf16*)v_pool, block_table, max_pages, page, n_heads, head_dim};
-    dim3 grid(rows * n_heads, n_split);
-    if (head_dim == 64) {
-        decode_attn_kernel<64><<<grid, 128, 0, stream>>>((const bf16*)q, L, (float*)workspace, s_q, past, past_dev, ldq, scale, n_split);
-        decode_attn_combine_kernel<64><<<rows * n_heads, 64, 0, stream>>>((const float*)workspace, (bf16*)out, n_heads, n_split, ldo);
-    } else {
-        decode_attn_kernel<256><<<grid, 128, 0, stream>>>((const bf16*)q, L, (float*)workspace, s_q, past, past_dev, ldq, scale, n_split);
-        decode_attn_combine_kernel<256><<<rows * n_heads, 128, 0, stream>>>((const float*)workspace, (bf16*)out, n_heads, n_split, ldo);
-    }
-    B200_COUNT_EXTRA(1);
-    B200_CHECK_LAUNCH("attn_decode");
-    return B200_OK;
+    return attn_decode<false>(q, k_pool, v_pool, block_table, max_pages, page, out, batch, s_q, n_heads, head_dim, past,
+                              past_dev, max_T, ldq, ldo, scale, n_split, workspace, workspace_bytes, nullptr, stream);
+}
+
+extern "C" int b200_attn_decode_ragged(const void* q, const void* k_pool, const void* v_pool, const int* block_table,
+                                       int max_pages, int page, void* out, int batch, int s_q, int n_heads, int head_dim,
+                                       int past, const int* past_dev, int max_T, int ldq, int ldo, float scale, int n_split,
+                                       void* workspace, size_t workspace_bytes, const int* row_off, cudaStream_t stream) {
+    return attn_decode<true>(q, k_pool, v_pool, block_table, max_pages, page, out, batch, s_q, n_heads, head_dim, past,
+                             past_dev, max_T, ldq, ldo, scale, n_split, workspace, workspace_bytes, row_off, stream);
 }
 
 extern "C" int b200_sample_topp_topk(const void* probs, int is_bf16, int rows, int V, int ld, float top_p, int top_k,
@@ -798,7 +873,15 @@ extern "C" int b200_uniform_fill(float* u, int n, unsigned long long seed, unsig
 
 extern "C" int b200_event_commit(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T,
                                  int max_len, cudaStream_t stream) {
-    event_commit_kernel<<<1, 256, 0, stream>>>(ev_t, seq, ev_next, pos_dev, B, T, max_len);
+    event_commit_kernel<false><<<1, 256, 0, stream>>>(ev_t, seq, ev_next, pos_dev, B, T, max_len, nullptr);
+    B200_CHECK_LAUNCH("event_commit");
+    return B200_OK;
+}
+
+extern "C" int b200_event_commit_ragged(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B,
+                                        int T, int max_len, const int* row_off, cudaStream_t stream) {
+    B200_CHECK_ARG(row_off != nullptr, "event_commit_ragged: row_off required");
+    event_commit_kernel<true><<<1, 256, 0, stream>>>(ev_t, seq, ev_next, pos_dev, B, T, max_len, row_off);
     B200_CHECK_LAUNCH("event_commit");
     return B200_OK;
 }

@@ -16,6 +16,7 @@
 // Arithmetic and rounding points are those of the launch-per-phase kernels in decode.cu (same per-row accumulation
 // order in the projections; attention differs only in how the context is cut into chunks).
 #include <cooperative_groups.h>
+#include <type_traits>
 
 #include "common.cuh"
 #include "rope.cuh"
@@ -62,6 +63,13 @@ struct PD {                              // kernel parameters (device pointers r
     int n_events;
     int k_max;
 };
+// parameters of the ragged kernel (b200_decode_events_ragged): PD plus the per-row position offsets.  A derived struct
+// rather than a new PD field, so that the kernel without RAGGED keeps its parameter block (and its stack copy of it).
+struct PDRagged : PD {
+    const int* row_off;                  // [B]: row b's position is pos + row_off[b] <= pos
+};
+template <bool RAGGED>
+using PDArg = std::conditional_t<RAGGED, PDRagged, PD>;
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
     unsigned v;
@@ -318,12 +326,16 @@ __device__ __forceinline__ size_t kv_base(const int* bt, int max_pages, int page
     return (((size_t)pg * nh + h) * page + (t % page)) * D;
 }
 
-__device__ __noinline__ void outer_attention(const PD& p, int layer, int pos, int B, int gw, int ngw, int lane,
+// RAGGED: row b's new position is pos + row_off[b] <= pos.  The chunk grid stays on the shared length pos + 1 (uniform
+// across the grid), so the trailing chunks of a shorter row can be empty: their key loop does not run and they write the
+// neutral partial (m = -inf, l = 0, o = 0), which the combine pass weights by exp(-inf - mx) = 0.  Chunk 0 is never empty.
+template <bool RAGGED>
+__device__ __noinline__ void outer_attention(const PDArg<RAGGED>& p, int layer, int pos_shared, int B, int gw, int ngw, int lane,
                                                 float* q_s, bf16* kn_s, bf16* vn_s, int& n_chunks_out) {
     const DD& d = p.d;
     constexpr int D = 64;
     const int nh = d.nh_outer, H = d.H;
-    const int T = pos + 1;
+    const int T = pos_shared + 1;
     const int items = B * nh;
     int target = ngw / items;
     if (target < 1) target = 1;
@@ -338,7 +350,9 @@ __device__ __noinline__ void outer_attention(const PD& p, int layer, int pos, in
     for (int it = gw; it < items * n_chunks; it += ngw) {
         const int bh = it / n_chunks, c = it % n_chunks;
         const int b = bh / nh, h = bh % nh;
-        const int t0 = c * chunk, t1 = min(T, t0 + chunk);
+        int pos = pos_shared;
+        if constexpr (RAGGED) pos += p.row_off[b];
+        const int t0 = c * chunk, t1 = min(pos + 1, t0 + chunk);
         const bf16* row = p.qkv + (size_t)b * 3 * H;
         const float cs = __bfloat162float(d.cos_outer[(size_t)pos * 32 + lane]), sn = __bfloat162float(d.sin_outer[(size_t)pos * 32 + lane]);
         {
@@ -575,8 +589,8 @@ __device__ __forceinline__ float rng_uniform(unsigned long long seed, unsigned l
 }
 
 // =================================================================================================================
-template <int BM>
-__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PD p) {
+template <int BM, bool RAGGED>
+__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED> p) {
     extern __shared__ __align__(16) uint8_t pd_smem[];
     const DD& d = p.d;
     const int B = d.batch, H = d.H;
@@ -655,7 +669,7 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PD p
             grid_sync(gb);
             prof.mark(PH_QKV_O);
             int n_chunks;
-            outer_attention(p, l, pos, B, gw, ngw, lane, q_s, kn_s, vn_s, n_chunks);
+            outer_attention<RAGGED>(p, l, pos, B, gw, ngw, lane, q_s, kn_s, vn_s, n_chunks);
             prof.sub(PH_ATT_O, 1);
             if (n_chunks > 1) {
                 grid_sync(gb);
@@ -814,7 +828,9 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PD p
             const long long v = (t < n_steps) ? __ldcg(p.ev_t + (size_t)t * B + b) : (long long)d.pad_id;
             cur_ev[k] = (int)v;
             if (blockIdx.x == 0) {
-                d.seq[((size_t)b * d.max_len + pos + 1) * PD_T + t] = v;
+                int row_pos = pos;                        // RAGGED: row b commits at its own position
+                if constexpr (RAGGED) row_pos += p.row_off[b];
+                d.seq[((size_t)b * d.max_len + row_pos + 1) * PD_T + t] = v;
                 d.ev_in[k] = v;
             }
         }
@@ -857,9 +873,13 @@ WsLayout ws_layout(const b200_decode_desc& d) {
 extern "C" size_t b200_decode_events_workspace_bytes(const b200_decode_desc* d) { return ws_layout(*d).total; }
 extern "C" size_t b200_decode_desc_bytes(void) { return sizeof(b200_decode_desc); }
 
-extern "C" int b200_decode_events(const b200_decode_desc* desc, int n_events, void* workspace, size_t workspace_bytes,
-                                  cudaStream_t stream) {
+namespace {
+
+template <bool RAGGED>
+int decode_events(const b200_decode_desc* desc, const int* row_off, int n_events, void* workspace, size_t workspace_bytes,
+                  cudaStream_t stream) {
     const b200_decode_desc& d = *desc;
+    B200_CHECK_ARG(!RAGGED || row_off != nullptr, "decode_events_ragged: row_off required");
     B200_CHECK_ARG(d.batch >= 1 && d.batch <= 16, "decode_events: batch %d outside 1..16", d.batch);
     B200_CHECK_ARG(d.H == 1024 && d.nh_outer * 64 == d.H && d.nh_inner * 256 == d.H,
                    "decode_events: built for hidden 1024 (16 x 64 event-level heads, 4 x 256 token-level heads)");
@@ -897,17 +917,20 @@ extern "C" int b200_decode_events(const b200_decode_desc* desc, int n_events, vo
     p.k_max = d.I_outer > d.I_inner ? d.I_outer : d.I_inner;
     if (p.k_max < d.H) p.k_max = d.H;
     B200_CUDA(cudaMemsetAsync(p.bar, 0, 256, stream), "decode_events: barrier reset");
+    PDArg<RAGGED> pk;
+    static_cast<PD&>(pk) = p;
+    if constexpr (RAGGED) pk.row_off = row_off;
     const int bm = d.batch <= 1 ? 1 : d.batch <= 2 ? 2 : d.batch <= 4 ? 4 : d.batch <= 8 ? 8 : 16;
     const size_t smem = (size_t)bm * p.k_max * 2 + (size_t)smp::SMP_MAXV * 8 + (PD_THREADS + 8) * 4 + 64 * 4 +
                         PD_WARPS * 64 * (4 + 2 + 2) + (size_t)bm * PD_T * 4 + 64;
-    void* args[] = {(void*)&p};
+    void* args[] = {(void*)&pk};
     const void* fn = nullptr;
     switch (bm) {
-        case 1: fn = (const void*)decode_events_kernel<1>; break;
-        case 2: fn = (const void*)decode_events_kernel<2>; break;
-        case 4: fn = (const void*)decode_events_kernel<4>; break;
-        case 8: fn = (const void*)decode_events_kernel<8>; break;
-        default: fn = (const void*)decode_events_kernel<16>; break;
+        case 1: fn = (const void*)decode_events_kernel<1, RAGGED>; break;
+        case 2: fn = (const void*)decode_events_kernel<2, RAGGED>; break;
+        case 4: fn = (const void*)decode_events_kernel<4, RAGGED>; break;
+        case 8: fn = (const void*)decode_events_kernel<8, RAGGED>; break;
+        default: fn = (const void*)decode_events_kernel<16, RAGGED>; break;
     }
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "decode_events smem attr");
     int per_sm = 0;
@@ -917,4 +940,16 @@ extern "C" int b200_decode_events(const b200_decode_desc* desc, int n_events, vo
     B200_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(PD_THREADS), args, smem, stream), "decode_events launch");
     b200_count_launches(1);
     return B200_OK;
+}
+
+}   // namespace
+
+extern "C" int b200_decode_events(const b200_decode_desc* desc, int n_events, void* workspace, size_t workspace_bytes,
+                                  cudaStream_t stream) {
+    return decode_events<false>(desc, nullptr, n_events, workspace, workspace_bytes, stream);
+}
+
+extern "C" int b200_decode_events_ragged(const b200_decode_desc* desc, const int* row_off, int n_events, void* workspace,
+                                         size_t workspace_bytes, cudaStream_t stream) {
+    return decode_events<true>(desc, row_off, n_events, workspace, workspace_bytes, stream);
 }

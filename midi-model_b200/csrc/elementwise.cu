@@ -502,13 +502,16 @@ __global__ void rope_table_kernel(const float* __restrict__ inv_freq, int half, 
 }
 
 // In place on the q and k thirds of packed qkv rows [rows, 3*H]; position of row r = pos0 (+ *pos0_dev) + r % S
-// (the tables cover absolute positions), or its in-segment position with a segment table (rope.cuh).
-template <bool BWD>
+// (the tables cover absolute positions), or its in-segment position with a segment table (rope.cuh).  RAGGED: row r of
+// sequence r / S is at pos0 (+ *pos0_dev) + row_off[r / S] + r % S.
+template <bool BWD, bool RAGGED = false>
 __global__ void rope_kernel(bf16* __restrict__ qkv, const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
                             int rows, int S, int H, int D, int ld, int pos0, const int* __restrict__ pos0_dev,
-                            const int* __restrict__ seg) {
+                            const int* __restrict__ seg, const int* __restrict__ row_off) {
     const int r = blockIdx.x;
-    const int s = seg ? seg_pos(seg, r) : pos0 + (pos0_dev ? *pos0_dev : 0) + r % S;
+    int s;
+    if constexpr (RAGGED) s = pos0 + (pos0_dev ? *pos0_dev : 0) + row_off[r / S] + r % S;
+    else s = seg ? seg_pos(seg, r) : pos0 + (pos0_dev ? *pos0_dev : 0) + r % S;
     const int half = D / 2;
     const int vec_per_head = half / 8;
     const int heads2 = 2 * (H / D);   // q heads then k heads (k third starts at column H)
@@ -856,9 +859,9 @@ extern "C" int b200_rope_qk(void* qkv, const void* cos_t, const void* sin_t, int
     B200_CHECK_ARG(D % 16 == 0 && H % D == 0 && ld % 8 == 0, "rope: head_dim must be a multiple of 16");
     if (rows == 0) return B200_OK;
     if (backward)
-        rope_kernel<true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev, nullptr);
+        rope_kernel<true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev, nullptr, nullptr);
     else
-        rope_kernel<false><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev, nullptr);
+        rope_kernel<false><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H, D, ld, pos0, pos0_dev, nullptr, nullptr);
     B200_CHECK_LAUNCH("rope");
     return B200_OK;
 }
@@ -870,10 +873,21 @@ extern "C" int b200_rope_qk_seg(void* qkv, const void* cos_t, const void* sin_t,
                    rows);
     if (rows == 0) return B200_OK;
     if (backward)
-        rope_kernel<true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, 1, H, D, ld, 0, nullptr, seg);
+        rope_kernel<true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, 1, H, D, ld, 0, nullptr, seg, nullptr);
     else
-        rope_kernel<false><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, 1, H, D, ld, 0, nullptr, seg);
+        rope_kernel<false><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, 1, H, D, ld, 0, nullptr, seg, nullptr);
     B200_CHECK_LAUNCH("rope_seg");
+    return B200_OK;
+}
+
+extern "C" int b200_rope_qk_ragged(void* qkv, const void* cos_t, const void* sin_t, int rows, int S, int H, int D, int ld,
+                                   int pos0, const int* pos0_dev, const int* row_off, cudaStream_t stream) {
+    B200_CHECK_ARG(D % 16 == 0 && H % D == 0 && ld % 8 == 0, "rope_ragged: head_dim must be a multiple of 16");
+    B200_CHECK_ARG(S >= 1 && row_off != nullptr, "rope_ragged: S >= 1 and row_off required");
+    if (rows == 0) return B200_OK;
+    rope_kernel<false, true><<<rows, ROW_THREADS, 0, stream>>>((bf16*)qkv, (const bf16*)cos_t, (const bf16*)sin_t, rows, S, H,
+                                                              D, ld, pos0, pos0_dev, nullptr, row_off);
+    B200_CHECK_LAUNCH("rope_ragged");
     return B200_OK;
 }
 

@@ -118,10 +118,11 @@ class CachedStack:
         return True
 
     def step(self, x: torch.Tensor, kv: PagedKV, s_new: int, pos_dev: Optional[torch.Tensor] = None,
-             max_T: Optional[int] = None, final_norm: bool = True) -> torch.Tensor:
+             max_T: Optional[int] = None, final_norm: bool = True, row_off: Optional[torch.Tensor] = None) -> torch.Tensor:
         """x: [batch * s_new, H] new inputs_embeds; appends to kv; returns final-normed hidden for the new rows.
         With `pos_dev` (int32[1] on the device) the number of cached positions is read by the kernels themselves
-        (CUDA-graph replay); `max_T` then bounds the context for the split-T decode attention."""
+        (CUDA-graph replay); `max_T` then bounds the context for the split-T decode attention.  `row_off` (int32 [batch]
+        on the device, with `pos_dev` only): row b sits at *pos_dev + row_off[b] (ragged generate, the `_ragged` entries)."""
         c = self.eng.cfg
         H, D, nh = c.hidden, c.head_dim, c.n_head
         B = kv.batch
@@ -139,17 +140,25 @@ class CachedStack:
         n_split = max(1, min(32, (T + 255) // 256)) if D == 64 else 1
         pd = lib.ptr(pos_dev)
         ws_bytes = lib.query("b200_attn_decode_workspace_bytes", B * s_new, nh, D, n_split)
+        if row_off is not None and not dev_pos:
+            raise lib.B200Error("row_off needs device-side positions (pos_dev)")
         if FUSED_DECODE and s_new == 1 and B <= 16:
-            return self._step_fused(x, kv, past, pos_dev, T, n_split, ws_bytes, final_norm)
+            return self._step_fused(x, kv, past, pos_dev, T, n_split, ws_bytes, final_norm, row_off)
         if not final_norm:
             raise lib.B200Error("final_norm=False is only available on the fused single-token path")
         prefill = not dev_pos and past == 0 and s_new > 1        # prompt into an empty cache: causal attention kernels
         for li, w in enumerate(self.eng.layers):
             n1 = ops.rmsnorm(x, w.ln1, c.eps)
             qkv = _linear(n1, w.qkv)
-            ops.rope_qk_(qkv, self.cos, self.sin, s_new, H, D, pos0=past, pos0_dev=pos_dev)
-            lib.call("b200_kv_append", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(), kv.block_table.data_ptr(),
-                     kv.max_pages, kv.page, nh, D, B, s_new, past, pd, qkv.stride(0), lib.stream())
+            if row_off is not None:
+                ops.rope_qk_ragged_(qkv, self.cos, self.sin, s_new, H, D, row_off, pos0=past, pos0_dev=pos_dev)
+                lib.call("b200_kv_append_ragged", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
+                         kv.block_table.data_ptr(), kv.max_pages, kv.page, nh, D, B, s_new, past, pd, qkv.stride(0),
+                         row_off.data_ptr(), lib.stream())
+            else:
+                ops.rope_qk_(qkv, self.cos, self.sin, s_new, H, D, pos0=past, pos0_dev=pos_dev)
+                lib.call("b200_kv_append", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(), kv.block_table.data_ptr(),
+                         kv.max_pages, kv.page, nh, D, B, s_new, past, pd, qkv.stride(0), lib.stream())
             if prefill and D == 64:
                 attn, _ = ops.attn_causal_fwd(qkv, B, s_new, nh, D, want_lse=False)
             elif prefill and D == 256 and s_new <= 8:
@@ -158,9 +167,14 @@ class CachedStack:
                 # the cached length is `past` (host) or *pos_dev (graph replay, past = 0)
                 attn = torch.empty((B * s_new, H), dtype=BF16, device=x.device)
                 ws = ops._ws("attn_decode", ws_bytes, x.device)
-                lib.call("b200_attn_decode", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
-                         kv.block_table.data_ptr(), kv.max_pages, kv.page, attn.data_ptr(), B, s_new, nh, D, past, pd, T,
-                         qkv.stride(0), H, scale, n_split, ws.data_ptr(), ws.numel(), lib.stream())
+                if row_off is not None:
+                    lib.call("b200_attn_decode_ragged", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
+                             kv.block_table.data_ptr(), kv.max_pages, kv.page, attn.data_ptr(), B, s_new, nh, D, past, pd, T,
+                             qkv.stride(0), H, scale, n_split, ws.data_ptr(), ws.numel(), row_off.data_ptr(), lib.stream())
+                else:
+                    lib.call("b200_attn_decode", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
+                             kv.block_table.data_ptr(), kv.max_pages, kv.page, attn.data_ptr(), B, s_new, nh, D, past, pd, T,
+                             qkv.stride(0), H, scale, n_split, ws.data_ptr(), ws.numel(), lib.stream())
             h = _linear(attn, w.o, residual=x)
             n2 = ops.rmsnorm(h, w.ln2, c.eps)
             gu = _linear(n2, w.gu)
@@ -171,7 +185,7 @@ class CachedStack:
         return ops.rmsnorm(x, self.eng.norm, c.eps)
 
 
-    def _step_fused(self, x, kv, past, pos_dev, T, n_split, ws_bytes, final_norm=True):
+    def _step_fused(self, x, kv, past, pos_dev, T, n_split, ws_bytes, final_norm=True, row_off=None):
         """Single-token step with 5 launches per layer: norm+QKV, RoPE+append+attention, o_proj+residual,
         norm+gate/up+SwiGLU, down+residual.  Same rounding points as the unfused kernels (bit-identical)."""
         c = self.eng.cfg
@@ -183,10 +197,16 @@ class CachedStack:
         for li, w in enumerate(self.eng.layers):
             qkv = _gemv_fused(x, w.qkv, 3 * H, norm_w=w.ln1, eps=c.eps)
             attn = torch.empty((B, H), dtype=BF16, device=qkv.device)
-            lib.call("b200_attn_decode_fused", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
-                     kv.block_table.data_ptr(), kv.max_pages, kv.page, self.cos.data_ptr(), self.sin.data_ptr(),
-                     attn.data_ptr(), B, nh, D, past, pd, T, qkv.stride(0), H, scale, n_split, ws.data_ptr(), ws.numel(),
-                     lib.stream())
+            if row_off is not None:
+                lib.call("b200_attn_decode_fused_ragged", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
+                         kv.block_table.data_ptr(), kv.max_pages, kv.page, self.cos.data_ptr(), self.sin.data_ptr(),
+                         attn.data_ptr(), B, nh, D, past, pd, T, qkv.stride(0), H, scale, n_split, ws.data_ptr(),
+                         ws.numel(), row_off.data_ptr(), lib.stream())
+            else:
+                lib.call("b200_attn_decode_fused", qkv.data_ptr(), kv.k[li].data_ptr(), kv.v[li].data_ptr(),
+                         kv.block_table.data_ptr(), kv.max_pages, kv.page, self.cos.data_ptr(), self.sin.data_ptr(),
+                         attn.data_ptr(), B, nh, D, past, pd, T, qkv.stride(0), H, scale, n_split, ws.data_ptr(), ws.numel(),
+                         lib.stream())
             h = _gemv_fused(attn, w.o, H, residual=x)
             act = _gemv_fused(h, w.gu, c.inner, norm_w=w.ln2, eps=c.eps, swiglu=True)
             x = _gemv_fused(act, w.down, H, residual=h)
@@ -238,6 +258,10 @@ class GraphGenerator:
     parameter are forced to pad by the grammar, exactly what the reference pads with, midi_model.py:239-241), so
     no host decision is needed inside an event; the reference's stop rule -- all rows emitted EOS in the same
     event (midi_model.py:248) -- is applied on the host every `check_every` events and the output truncated there.
+
+    Ragged prompts (`lengths`, set per call): row b continues its own first L_b events.  The shared `pos` stays the loop's
+    counter (its exit, the attention's chunk grid and the events per launch stay uniform) and row b sits at
+    pos + row_off[b], row_off[b] = L_b - max(L) <= 0, through the `_ragged` kernel entries; that mode has its own graph.
     """
 
     def __init__(self, outer: CachedStack, inner: CachedStack, lm_head: torch.Tensor, pitch: int, V: int, tok,
@@ -260,7 +284,10 @@ class GraphGenerator:
         # extra sampling mask ANDed with the grammar ranges (app.py:27-34,73-87: disable_patch_change /
         # disable_control_change / disable_channels); its address is baked into the graph, its contents are not
         self.mask = torch.ones((batch, V), dtype=torch.uint8, device=dev)
+        self.row_off = torch.zeros(batch, dtype=torch.int32, device=dev)    # ragged mode: row b at pos + row_off[b]
+        self.lengths = None             # ragged mode of the current call: int64 [B] prompt lengths on the device, else None
         self.graph = None
+        self.graph_ragged = None
         self.stream = torch.cuda.Stream(device=dev)
         self._persist = None            # (descriptor, pointer tables, workspace) of the persistent kernel, built on first use
 
@@ -314,7 +341,11 @@ class GraphGenerator:
         """Run `n` generated events in one launch (stops early inside the kernel at max_len)."""
         import ctypes
         d, ws, _ = self._persistent()
-        lib.call("b200_decode_events", ctypes.byref(d), int(n), ws.data_ptr(), ws.numel(), lib.stream())
+        if self.lengths is not None:
+            lib.call("b200_decode_events_ragged", ctypes.byref(d), self.row_off.data_ptr(), int(n), ws.data_ptr(), ws.numel(),
+                     lib.stream())
+        else:
+            lib.call("b200_decode_events", ctypes.byref(d), int(n), ws.data_ptr(), ws.numel(), lib.stream())
 
     def set_deny(self, ids) -> None:
         """Token ids that may never be sampled (empty = plain grammar)."""
@@ -326,8 +357,10 @@ class GraphGenerator:
     def _event(self):
         B, T = self.B, self.T
         emb_o, emb_i = self.outer.eng.embed, self.inner.eng.embed
+        ragged = self.lengths is not None
         e = ops.embed_sum(self.ev_in, emb_o)
-        hidden = self.outer.step(e, self.kv1, 1, pos_dev=self.pos, max_T=self.max_len)
+        hidden = self.outer.step(e, self.kv1, 1, pos_dev=self.pos, max_T=self.max_len,
+                                 row_off=self.row_off if ragged else None)
         self.kv2.reset()
         for i in range(T):
             if i == 0:
@@ -345,12 +378,22 @@ class GraphGenerator:
             lib.call("b200_sample_from_logits", logits.data_ptr(), B, self.V, logits.stride(0), self.temp, self.top_p,
                      self.top_k, i, self.ev_t.data_ptr(), self.g.lut.data_ptr(), self.g.n_event_types, self.g.eos, self.g.pad,
                      self.mask.data_ptr(), self.u.data_ptr(), self.ev_t.data_ptr() + 8 * B * i, 1, lib.stream())
-        lib.call("b200_event_commit", self.ev_t.data_ptr(), self.seq.data_ptr(), self.ev_in.data_ptr(), self.pos.data_ptr(),
-                 B, T, self.max_len, lib.stream())
+        if ragged:
+            lib.call("b200_event_commit_ragged", self.ev_t.data_ptr(), self.seq.data_ptr(), self.ev_in.data_ptr(),
+                     self.pos.data_ptr(), B, T, self.max_len, self.row_off.data_ptr(), lib.stream())
+        else:
+            lib.call("b200_event_commit", self.ev_t.data_ptr(), self.seq.data_ptr(), self.ev_in.data_ptr(),
+                     self.pos.data_ptr(), B, T, self.max_len, lib.stream())
 
     def _set_state(self, prompt: torch.Tensor):
-        """prompt [B, P, T]: events 0..P-2 are prefilled into the KV cache; event P-1 is fed by the first replay."""
+        """prompt [B, P, T]: events 0..P-2 are prefilled into the KV cache; event P-1 is fed by the first replay.
+        Ragged mode (P = max(L)): events >= L_b of row b are set to pad first; the rectangular prefill is still exact, since
+        attention is causal (no real event reads a later pad event) and the slot a pad event fills in row b is >= L_b - 1,
+        which the decode step writes before it first reads it.  Row b's first fed event is its event L_b - 1."""
         P = prompt.shape[1]
+        if self.lengths is not None:
+            past = torch.arange(P, device=prompt.device)[None, :] >= self.lengths[:, None]
+            prompt = prompt.masked_fill(past[:, :, None], self.tok.pad_id)
         self.seq.fill_(self.tok.pad_id)
         self.seq[:, :P] = prompt
         self.kv1.reset()
@@ -358,23 +401,45 @@ class GraphGenerator:
             e = ops.embed_sum(prompt[:, :P - 1].reshape(self.B * (P - 1), self.T).contiguous(), self.outer.eng.embed)
             self.outer.step(e, self.kv1, P - 1)
         self.pos.fill_(P - 1)
-        self.ev_in.copy_(prompt[:, P - 1])
+        if self.lengths is not None:
+            self.ev_in.copy_(prompt[torch.arange(self.B, device=prompt.device), self.lengths - 1])
+            self.row_off.copy_(self.lengths - P)
+        else:
+            self.ev_in.copy_(prompt[:, P - 1])
         self.counter.copy_(torch.tensor([0, self.seed], dtype=torch.int64))
 
-    def _prepare(self, prompt: torch.Tensor, use_graph) -> None:
-        """Load the prompt into the device state; capture the per-event graph on first use (current stream = self.stream)."""
+    def _set_lengths(self, prompt: torch.Tensor, lengths) -> None:
+        """Ragged mode for this call (`lengths`: B ints in [1, P], max(lengths) == P, checked by the caller) or not (None)."""
+        if lengths is None:
+            self.lengths = None
+            return
+        if len(lengths) != self.B or max(lengths) != prompt.shape[1] or min(lengths) < 1:
+            raise lib.B200Error(f"lengths {list(lengths)} do not fit a prompt of {prompt.shape[1]} events and {self.B} rows")
+        self.lengths = torch.tensor(list(lengths), dtype=torch.int64).to(self.seq.device)
+
+    def _graph(self):
+        return self.graph_ragged if self.lengths is not None else self.graph
+
+    def _prepare(self, prompt: torch.Tensor, use_graph, lengths=None) -> None:
+        """Load the prompt into the device state; capture the per-event graph of this mode (rectangular or ragged) on first
+        use (current stream = self.stream)."""
+        self._set_lengths(prompt, lengths)
         self._set_state(prompt)
         if self.table_version != self.outer.version:    # RoPE tables were re-created: the captured addresses are stale
             self.graph, self.table_version = None, self.outer.version
+            self.graph_ragged = None
         if use_graph == "persist":
             return
-        if use_graph and self.graph is None:
+        if use_graph and self._graph() is None:
             self._event()                       # warm-up (allocations, function attributes) outside capture
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, stream=self.stream):
                 self._event()
-            self.graph = g
+            if self.lengths is not None:
+                self.graph_ragged = g
+            else:
+                self.graph = g
             self._set_state(prompt)             # undo the warm-up's state changes
 
     def _mode(self, use_graph):
@@ -384,34 +449,42 @@ class GraphGenerator:
             return True
         return use_graph
 
-    def events(self, prompt: torch.Tensor, use_graph=True):
+    def events(self, prompt: torch.Tensor, use_graph=True, lengths=None):
         """Generator form (app.py:27-120): yields each new event as an int64 [B, T] CPU tensor right after its graph
         replay / kernel -- one device->host copy per EVENT, none per token -- and stops after the event in which every row
-        emitted EOS (app.py:119) or at max_len."""
+        emitted EOS (app.py:119) or at max_len.  `lengths`: ragged prompt (see run); row b's i-th new event is its event
+        L_b + i."""
         use_graph = self._mode(use_graph)
         P = prompt.shape[1]
         cur = torch.cuda.current_stream()
         self.stream.wait_stream(cur)
         with torch.cuda.stream(self.stream):
-            self._prepare(prompt, use_graph)
+            self._prepare(prompt, use_graph, lengths)
+            rows = torch.arange(self.B, device=self.seq.device) if self.lengths is not None else None
         for i in range(self.max_len - P):
             with torch.cuda.stream(self.stream):          # not held across the yield
                 if use_graph == "persist":
                     self._events_persistent(1)
                 elif use_graph:
-                    self.graph.replay()
+                    self._graph().replay()
                 else:
                     self._event()
-                ev = self.seq[:, P + i].cpu()              # synchronises on this event only
+                if self.lengths is not None:
+                    ev = self.seq[rows, self.lengths + i].cpu()
+                else:
+                    ev = self.seq[:, P + i].cpu()          # synchronises on this event only
             yield ev
             if bool((ev[:, 0] == self.tok.eos_id).all()):
                 break
         cur.wait_stream(self.stream)
 
     def run(self, prompt: torch.Tensor, use_graph=True, check_every: int = 32, progress=None,
-            stop_on_eos: bool = True, max_new: Optional[int] = None) -> torch.Tensor:
+            stop_on_eos: bool = True, max_new: Optional[int] = None, lengths=None) -> torch.Tensor:
         """`max_new` stops after that many generated events although the pools (and the split-T attention) are sized for
-        max_len: a serving process keeps ONE loop with full-context pools and cuts individual requests short."""
+        max_len: a serving process keeps ONE loop with full-context pools and cuts individual requests short.
+        `lengths` (B ints, max(lengths) == P): ragged prompt, row b being its first L_b events.  Every row gets the same
+        number n of new events; the result is the data.collate layout [B, P + n, T]: row b's L_b prompt events, its n new
+        events, then pad events."""
         P = prompt.shape[1]
         n_new = self.max_len - P
         if max_new is not None:
@@ -422,7 +495,8 @@ class GraphGenerator:
         cur = torch.cuda.current_stream()
         self.stream.wait_stream(cur)
         with torch.cuda.stream(self.stream):
-            self._prepare(prompt, use_graph)
+            self._prepare(prompt, use_graph, lengths)
+            graph = self._graph()
             done = 0
             stop_at = None
             while done < n_new:
@@ -432,7 +506,7 @@ class GraphGenerator:
                 else:
                     for _ in range(n):
                         if use_graph:
-                            self.graph.replay()
+                            graph.replay()
                         else:
                             self._event()
                 done += n
@@ -440,12 +514,25 @@ class GraphGenerator:
                     progress(n)
                 if not stop_on_eos:
                     continue
-                first = self.seq[:, P:P + done, 0]                       # event-type token of every generated event
+                if self.lengths is not None:                             # row b's generated events are at L_b + j
+                    idx = self.lengths[:, None] + torch.arange(done, device=self.seq.device)[None, :]
+                    first = self.seq[:, :, 0].gather(1, idx)
+                else:
+                    first = self.seq[:, P:P + done, 0]                   # event-type token of every generated event
                 all_eos = (first == self.tok.eos_id).all(dim=0)          # one small D2H sync per `check_every` events
                 hit = torch.nonzero(all_eos)
                 if hit.numel() > 0:
                     stop_at = P + int(hit[0].item()) + 1                 # the all-EOS event itself is kept
                     break
             out = self.seq[:, :(stop_at if stop_at is not None else P + done)].clone()
+            if self.lengths is not None:
+                # rows end at L_b + n_done: events a row generated past the stop point (same check_every block) become pad
+                pad_past(out, self.lengths + (out.shape[1] - P), self.tok.pad_id)
         cur.wait_stream(self.stream)
         return out
+
+
+def pad_past(x: torch.Tensor, ends: torch.Tensor, pad_id: int) -> torch.Tensor:
+    """In place on [B, S, T] events: row b's events >= ends[b] become pad events (the data.collate layout)."""
+    past = torch.arange(x.shape[1], device=x.device)[None, :] >= ends.to(x.device)[:, None]
+    return x.masked_fill_(past[:, :, None], pad_id)

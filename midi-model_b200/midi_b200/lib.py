@@ -39,6 +39,7 @@ SIGNATURES = {
     "b200_rope_table": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
     "b200_rope_qk": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp]),
     "b200_rope_qk_seg": (i32, [vp, vp, vp, i32, vp, i32, i32, i32, i32, vp]),
+    "b200_rope_qk_ragged": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
     "b200_swiglu_fwd": (i32, [vp, vp, i64, i32, vp]),
     "b200_swiglu_bwd": (i32, [vp, vp, vp, i64, i32, vp]),
     "b200_scale_bf16": (i32, [vp, vp, i64, f32, vp]),
@@ -75,9 +76,16 @@ SIGNATURES = {
     "b200_sample_from_logits": (i32, [vp, i32, i32, i32, f32, f32, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, i32, vp]),
     "b200_uniform_fill": (i32, [vp, i32, u64, vp, vp]),
     "b200_event_commit": (i32, [vp, vp, vp, vp, i32, i32, i32, vp]),
+    "b200_kv_append_ragged": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp, vp]),
+    "b200_attn_decode_ragged": (i32, [vp, vp, vp, vp, i32, i32, vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, f32, i32, vp, sz,
+                                      vp, vp]),
+    "b200_attn_decode_fused_ragged": (i32, [vp, vp, vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp, i32, i32, i32, f32, i32,
+                                            vp, sz, vp, vp]),
+    "b200_event_commit_ragged": (i32, [vp, vp, vp, vp, i32, i32, i32, vp, vp]),
     "b200_decode_desc_bytes": (sz, []),
     "b200_decode_events_workspace_bytes": (sz, [vp]),
     "b200_decode_events": (i32, [vp, i32, vp, sz, vp]),
+    "b200_decode_events_ragged": (i32, [vp, vp, i32, vp, sz, vp]),
 }
 
 

@@ -184,6 +184,15 @@ def rope_qk_seg_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, tiles:
              int(backward), lib.stream())
 
 
+def rope_qk_ragged_(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, S: int, H: int, D: int, row_off: torch.Tensor,
+                    pos0: int = 0, pos0_dev: Optional[torch.Tensor] = None):
+    """Forward rope_qk_ of a ragged generate batch: row r sits at pos0 (+ *pos0_dev) + row_off[r // S] + r % S (row_off:
+    int32 device [rows // S])."""
+    rows, ld = qkv.shape
+    lib.call("b200_rope_qk_ragged", qkv.data_ptr(), cos.data_ptr(), sin.data_ptr(), rows, S, H, D, ld, pos0,
+             lib.ptr(pos0_dev), row_off.data_ptr(), lib.stream())
+
+
 def swiglu(gu: torch.Tensor) -> torch.Tensor:
     rows, two_i = gu.shape
     act = torch.empty((rows, two_i // 2), dtype=BF16, device=gu.device)

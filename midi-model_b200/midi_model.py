@@ -400,6 +400,17 @@ def _ragged_rows(lengths, B: int, S: int, what: str) -> list:
     return rows
 
 
+def _prompt_lengths(lengths, B: int, P: int, what: str) -> list:
+    """Events of each prompt row (`generate_ragged`): B ints in [1, P], row b being its first L_b events."""
+    vals = _host_ints(lengths, what)
+    if len(vals) != B:
+        raise _lib.B200Error(f"{what} has {len(vals)} entries for a prompt of {B} rows")
+    out_of_range = [v for v in vals if not 1 <= v <= P]
+    if out_of_range:
+        raise _lib.B200Error(f"{what}: length {out_of_range[0]} is outside [1, {P}] (the prompt holds {P} events)")
+    return vals
+
+
 _ragged_layout = _engine.Segments.pack      # (src, Segments) of a ragged batch's packed rows (DESIGN.md 1)
 
 
@@ -808,6 +819,17 @@ class MIDIModel(PreTrainedModel):
             if len(idle) < 2:                                      # keep at most two idle loops per setting
                 idle.append(gg)
 
+    def _ragged_prompt(self, prompt, batch_size: int, lengths, dev, what: str):
+        """(prompt tensor [B, max(L), T], lengths) of a `generate_ragged` / `generate_stream_ragged` call, checked."""
+        if prompt is None:
+            raise _lib.B200Error(f"{what}: a ragged call needs a prompt")
+        if os.environ.get("B200_GENERATE", "persist") == "eager":
+            raise _lib.B200Error(f"{what}: ragged prompts need the device-resident loop (B200_GENERATE=eager is "
+                                 "rectangular only)")
+        inp = self._prompt_tensor(prompt, batch_size, dev)
+        lens = _prompt_lengths(lengths, inp.shape[0], inp.shape[1], f"{what}: lengths")
+        return inp, lens
+
     @torch.inference_mode()
     def generate_stream(self, prompt=None, batch_size=1, max_len=512, temp=1.0, top_p=0.98, top_k=20,
                         disable_patch_change=False, disable_control_change=False, disable_channels=None, generator=None):
@@ -815,17 +837,10 @@ class MIDIModel(PreTrainedModel):
         yields every new event as an int64 numpy array [batch, max_token_seq], with the app's extra grammar options
         (`disable_patch_change`, `disable_control_change`, `disable_channels` = channel numbers) applied as a device-side
         mask, the app's 4096-event context window (app.py:55) and its stop rule (all rows EOS in the same event).
-        One device->host copy per event, no sync per token."""
-        tok = self.tokenizer
+        One device->host copy per event, no sync per token.  Prompts of different lengths: generate_stream_ragged."""
         rt = self._rt()
         dev = rt.store.device
-        deny = []
-        if disable_patch_change:
-            deny.append(tok.event_ids["patch_change"])
-        if disable_control_change:
-            deny.append(tok.event_ids["control_change"])
-        for c in (disable_channels or []):
-            deny.append(tok.parameter_ids["channel"][c])
+        deny = self._deny_ids(disable_patch_change, disable_control_change, disable_channels)
         inp = self._prompt_tensor(prompt, batch_size, dev)[:, -4096:]
         if inp.shape[1] >= max_len:
             return
@@ -840,8 +855,50 @@ class MIDIModel(PreTrainedModel):
             gg.set_deny(())
             self._return_generator(key, gg)
 
+    def _deny_ids(self, disable_patch_change, disable_control_change, disable_channels) -> list:
+        tok = self.tokenizer
+        deny = []
+        if disable_patch_change:
+            deny.append(tok.event_ids["patch_change"])
+        if disable_control_change:
+            deny.append(tok.event_ids["control_change"])
+        for c in (disable_channels or []):
+            deny.append(tok.parameter_ids["channel"][c])
+        return deny
+
+    @torch.inference_mode()
+    def generate_stream_ragged(self, prompt, lengths, batch_size=1, max_len=512, temp=1.0, top_p=0.98, top_k=20,
+                               disable_patch_change=False, disable_control_change=False, disable_channels=None,
+                               generator=None):
+        """generate_stream on a ragged prompt (see generate_ragged): yields the new event of every row, [batch, 8] int64
+        per iteration.  The 4096-event context window applies per row: row b keeps its last min(L_b, 4096) events."""
+        rt = self._rt()
+        dev = rt.store.device
+        deny = self._deny_ids(disable_patch_change, disable_control_change, disable_channels)
+        inp, lens = self._ragged_prompt(prompt, batch_size, lengths, dev, "generate_stream_ragged")
+        window = 4096                                               # app.py:55, per row
+        if max(lens) > window:
+            rows = [inp[b, L - min(L, window):L] for b, L in enumerate(lens)]
+            lens = [r.shape[0] for r in rows]
+            inp = torch.full((len(rows), window, inp.shape[2]), self.tokenizer.pad_id, dtype=inp.dtype, device=dev)
+            for b, r in enumerate(rows):
+                inp[b, :r.shape[0]] = r
+        inp = inp[:, :max(lens)]
+        if inp.shape[1] >= max_len:
+            return
+        mode = os.environ.get("B200_GENERATE", "persist")
+        key, gg = self._checkout_generator(batch_size, max_len, temp, top_p, top_k, generator)
+        try:
+            gg.set_deny(deny)
+            for ev in gg.events(inp, use_graph=_loop_mode(mode), lengths=lens):
+                yield ev.numpy()
+        finally:
+            gg.set_deny(())
+            self._return_generator(key, gg)
+
     def generate(self, prompt=None, batch_size=1, max_len=512, temp=1.0, top_p=0.98, top_k=20, generator=None):
-        """midi_model.py:167-250 with the per-token work on the device (see midi_b200/decode.py)."""
+        """midi_model.py:167-250 with the per-token work on the device (see midi_b200/decode.py).  Prompts of different
+        lengths: generate_ragged."""
         tok = self.tokenizer
         T = tok.max_token_seq
         rt = self._rt()
@@ -915,6 +972,34 @@ class MIDIModel(PreTrainedModel):
                 if all(end):
                     break
         return seq[:, :cur_len].cpu().numpy()
+
+    def generate_ragged(self, prompt, lengths, batch_size=1, max_len=512, temp=1.0, top_p=0.98, top_k=20, generator=None):
+        """generate on a ragged, right-padded prompt [B, P, T] (data.collate layout) whose row b is its first L_b events;
+        the padding is never read.  `lengths`: a Python sequence or a CPU integer tensor of B values in [1, P].
+
+        Lockstep: every row gets the same n = max_len - max(L) new events at most, with generate's stop rule (after the
+        event in which every row emitted EOS).  Returns the data.collate layout [B, max(L) + n_done, T]: row b's prompt,
+        its n_done new events, then pad events.  A greedy row (top_k=1) equals generating its prompt alone; sampled rows
+        draw from their row index as in a rectangular batch.  Runs on the device-resident loop (B200_GENERATE persist,
+        graph or nograph) even for fewer than 4 new events; B200_GENERATE=eager raises B200Error."""
+        rt = self._rt()
+        dev = rt.store.device
+        inp, lens = self._ragged_prompt(prompt, batch_size, lengths, dev, "generate_ragged")
+        inp = inp[:, :max(lens)]
+        if inp.shape[1] >= max_len:
+            return _dec.pad_past(inp.clone(), torch.tensor(lens), self.tokenizer.pad_id).cpu().numpy()
+        if rt.grammar is None:
+            rt.grammar = _dec.GrammarLUT(self.tokenizer, dev)
+        mode = os.environ.get("B200_GENERATE", "persist")
+        key, gg = self._checkout_generator(batch_size, max_len, temp, top_p, top_k, generator)
+        try:
+            gg.set_deny(())
+            bar = tqdm.tqdm(desc="generating", total=max_len - inp.shape[1])
+            with bar:
+                out = gg.run(inp, use_graph=_loop_mode(mode), progress=bar.update, lengths=lens)
+        finally:
+            self._return_generator(key, gg)
+        return out.cpu().numpy()
 
     # ------------------------------------------------------------------ fused training path (non-reference API)
     def training_loss(self, batch: torch.Tensor, backward: bool = True, accumulate: bool = False, grad_ready=None,
