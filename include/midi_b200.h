@@ -262,6 +262,13 @@ int b200_attn_decode_fused_ragged(const void* qkv, void* k_pool, void* v_pool, c
                                   int n_split, void* workspace, size_t workspace_bytes, const int* row_off, cudaStream_t s);
 int b200_event_commit_ragged(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T,
                              int max_len, const int* row_off, cudaStream_t s);
+/*      request queue (continuous batching): event_commit_ragged for the live rows only, plus a per-row stop.  row_end
+ *      (device int32 [B]): seq index of row b's last allowed event.  row_last (device int32 [B]): -1 while row b is live,
+ *      else the seq index of its last committed event (the caller writes -2 for an empty slot).  A live row finishes when
+ *      its committed event's type token is eos_id or its seq index reaches row_end[b]; row_last[b] then gets that index.
+ *      A row that is not live writes nothing.  *pos still advances by one. */
+int b200_event_commit_queue(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T,
+                            int max_len, const int* row_off, const int* row_end, int* row_last, int eos_id, cudaStream_t s);
 
 
 /* ---- persistent generate kernel (midi_model.py:192-248: one generated event = event-level decode step + up to 8
@@ -309,6 +316,13 @@ int b200_decode_events(const b200_decode_desc* d, int n_events, void* workspace 
  *      combine.  Row b commits to seq[b, *pos + row_off[b] + 1].  Same descriptor and workspace. */
 int b200_decode_events_ragged(const b200_decode_desc* d, const int* row_off, int n_events, void* workspace,
                               size_t workspace_bytes, cudaStream_t s);
+/*      request queue: b200_decode_events_ragged with the per-row stop of b200_event_commit_queue (row_end, row_last as
+ *      there).  A row that is not live commits nothing, is left out of the token-step count, draws nothing and skips its
+ *      attention, so none of its values reach a live row.  The launch ends after n_events events, at *pos + 1 >= max_len,
+ *      when no live row is left, or -- with exit_on_done -- after the event in which any row finished.  Every CTA derives
+ *      the finish flags from the same values, so that exit needs no extra grid barrier. */
+int b200_decode_events_queue(const b200_decode_desc* d, const int* row_off, const int* row_end, int* row_last,
+                             int exit_on_done, int n_events, void* workspace, size_t workspace_bytes, cudaStream_t s);
 
 #ifdef __cplusplus
 }

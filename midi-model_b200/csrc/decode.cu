@@ -599,6 +599,31 @@ __global__ void event_commit_kernel(const long long* __restrict__ ev_t, long lon
     if (threadIdx.x == 0) *pos = p + 1;
 }
 
+// event_commit_kernel<true> of the request-queue loop, with the persistent queue kernel's per-row finish rule: only a live
+// row (row_last[b] == -1) commits, and it finishes when its committed event is EOS or lands on row_end[b], its seq index
+// then going to row_last[b].
+__global__ void event_commit_queue_kernel(const long long* __restrict__ ev_t, long long* __restrict__ seq,
+                                          long long* __restrict__ ev_next, int* __restrict__ pos, int B, int T, int max_len,
+                                          const int* __restrict__ row_off, const int* __restrict__ row_end,
+                                          int* __restrict__ row_last, int eos_id) {
+    const int p = *pos;
+    for (int i = threadIdx.x; i < B * T; i += blockDim.x) {
+        const int b = i / T, t = i % T;
+        if (row_last[b] != -1) continue;
+        const long long v = ev_t[(size_t)t * B + b];
+        const int q = p + row_off[b];
+        if (q + 1 < max_len) seq[((size_t)b * max_len + q + 1) * T + t] = v;
+        ev_next[(size_t)b * T + t] = v;
+    }
+    __syncthreads();                                     // every read of row_last above precedes its writes below
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        if (row_last[b] != -1) continue;
+        const int last = p + row_off[b] + 1;
+        if (ev_t[b] == eos_id || last >= row_end[b]) row_last[b] = last;
+    }
+    if (threadIdx.x == 0) *pos = p + 1;
+}
+
 }   // namespace
 
 // =============================================================================================
@@ -883,5 +908,16 @@ extern "C" int b200_event_commit_ragged(const long long* ev_t, long long* seq, l
     B200_CHECK_ARG(row_off != nullptr, "event_commit_ragged: row_off required");
     event_commit_kernel<true><<<1, 256, 0, stream>>>(ev_t, seq, ev_next, pos_dev, B, T, max_len, row_off);
     B200_CHECK_LAUNCH("event_commit");
+    return B200_OK;
+}
+
+extern "C" int b200_event_commit_queue(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T,
+                                       int max_len, const int* row_off, const int* row_end, int* row_last, int eos_id,
+                                       cudaStream_t stream) {
+    B200_CHECK_ARG(row_off != nullptr && row_end != nullptr && row_last != nullptr,
+                   "event_commit_queue: row_off, row_end and row_last required");
+    event_commit_queue_kernel<<<1, 256, 0, stream>>>(ev_t, seq, ev_next, pos_dev, B, T, max_len, row_off, row_end, row_last,
+                                                     eos_id);
+    B200_CHECK_LAUNCH("event_commit_queue");
     return B200_OK;
 }

@@ -68,8 +68,14 @@ struct PD {                              // kernel parameters (device pointers r
 struct PDRagged : PD {
     const int* row_off;                  // [B]: row b's position is pos + row_off[b] <= pos
 };
-template <bool RAGGED>
-using PDArg = std::conditional_t<RAGGED, PDRagged, PD>;
+// parameters of the request-queue kernel (b200_decode_events_queue): the ragged ones plus each row's budget and state
+struct PDQueue : PDRagged {
+    const int* row_end;                  // [B]: seq index of row b's last allowed event
+    int* row_last;                       // [B]: -1 while row b is live, else the seq index of its last event (-2: empty)
+    int exit_on_done;                    // leave after the event in which a row finished
+};
+template <bool RAGGED, bool QUEUE = false>
+using PDArg = std::conditional_t<QUEUE, PDQueue, std::conditional_t<RAGGED, PDRagged, PD>>;
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
     unsigned v;
@@ -329,9 +335,11 @@ __device__ __forceinline__ size_t kv_base(const int* bt, int max_pages, int page
 // RAGGED: row b's new position is pos + row_off[b] <= pos.  The chunk grid stays on the shared length pos + 1 (uniform
 // across the grid), so the trailing chunks of a shorter row can be empty: their key loop does not run and they write the
 // neutral partial (m = -inf, l = 0, o = 0), which the combine pass weights by exp(-inf - mx) = 0.  Chunk 0 is never empty.
-template <bool RAGGED>
-__device__ __noinline__ void outer_attention(const PDArg<RAGGED>& p, int layer, int pos_shared, int B, int gw, int ngw, int lane,
-                                                float* q_s, bf16* kn_s, bf16* vn_s, int& n_chunks_out) {
+// QUEUE: a row that is not live (row_last[b] != -1, written by CTA 0 at the last commit and read after a grid barrier)
+// skips its items: it appends nothing and reads none of its pages.
+template <bool RAGGED, bool QUEUE = false>
+__device__ __noinline__ void outer_attention(const PDArg<RAGGED, QUEUE>& p, int layer, int pos_shared, int B, int gw, int ngw,
+                                                int lane, float* q_s, bf16* kn_s, bf16* vn_s, int& n_chunks_out) {
     const DD& d = p.d;
     constexpr int D = 64;
     const int nh = d.nh_outer, H = d.H;
@@ -350,6 +358,9 @@ __device__ __noinline__ void outer_attention(const PDArg<RAGGED>& p, int layer, 
     for (int it = gw; it < items * n_chunks; it += ngw) {
         const int bh = it / n_chunks, c = it % n_chunks;
         const int b = bh / nh, h = bh % nh;
+        if constexpr (QUEUE) {
+            if (__ldcg(p.row_last + b) != -1) continue;
+        }
         int pos = pos_shared;
         if constexpr (RAGGED) pos += p.row_off[b];
         const int t0 = c * chunk, t1 = min(pos + 1, t0 + chunk);
@@ -589,8 +600,11 @@ __device__ __forceinline__ float rng_uniform(unsigned long long seed, unsigned l
 }
 
 // =================================================================================================================
-template <int BM, bool RAGGED>
-__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED> p) {
+// QUEUE (implies RAGGED): each row stops on its own.  A live row finishes at the commit of an event that is EOS or lands on
+// row_end[b]; a row that is not live commits nothing, takes no part in the token-step count and skips its attention items.
+template <int BM, bool RAGGED, bool QUEUE = false>
+__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED, QUEUE> p) {
+    static_assert(!QUEUE || RAGGED, "the queue kernel positions its rows through row_off");
     extern __shared__ __align__(16) uint8_t pd_smem[];
     const DD& d = p.d;
     const int B = d.batch, H = d.H;
@@ -618,6 +632,11 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
     int pos = __ldcg(d.pos);
     for (int i = threadIdx.x; i < B * PD_T; i += PD_THREADS) cur_ev[i] = (int)__ldcg(d.ev_in + i);
     const unsigned long long rng_c0 = d.rng_state[0], rng_seed = d.rng_state[1];
+    unsigned live = 0;                                  // QUEUE: bit b set while row b is live, the same in every thread
+    if constexpr (QUEUE) {
+        for (int b = 0; b < B; b++)
+            if (__ldcg(p.row_last + b) == -1) live |= 1u << b;
+    }
     __syncthreads();
 
     int events_done = 0;
@@ -669,7 +688,7 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
             grid_sync(gb);
             prof.mark(PH_QKV_O);
             int n_chunks;
-            outer_attention<RAGGED>(p, l, pos, B, gw, ngw, lane, q_s, kn_s, vn_s, n_chunks);
+            outer_attention<RAGGED, QUEUE>(p, l, pos, B, gw, ngw, lane, q_s, kn_s, vn_s, n_chunks);
             prof.sub(PH_ATT_O, 1);
             if (n_chunks > 1) {
                 grid_sync(gb);
@@ -727,6 +746,9 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
                     // parameters; two steps at least, like the reference's loop)
                     int need = 2;
                     for (int b = 0; b < B; b++) {
+                        if constexpr (QUEUE) {
+                            if (!((live >> b) & 1u)) continue;
+                        }
                         const long long ev = __ldcg(p.ev_t + b);
                         const int et = (int)ev - (d.eos_id + 1);
                         if (ev == d.eos_id || et < 0 || et >= d.n_event_types) continue;
@@ -812,10 +834,16 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
             prof.mark(PH_LMHEAD);
             if ((int)blockIdx.x < B) {
                 const int b = blockIdx.x;
-                const long long ev0 = (i == 0) ? 0 : __ldcg(p.ev_t + b);
-                const float u = rng_uniform(rng_seed, rng_c0 + (unsigned long long)(events_done * PD_T + i), b);
-                const int id = sample_row(p, b, i, ev0, u, s_p, s_i, s_cnt, s_red);
-                if (threadIdx.x == 0) p.ev_t[(size_t)i * B + b] = id;
+                bool sample = true;
+                if constexpr (QUEUE) sample = (live >> b) & 1u;
+                if (sample) {
+                    const long long ev0 = (i == 0) ? 0 : __ldcg(p.ev_t + b);
+                    const float u = rng_uniform(rng_seed, rng_c0 + (unsigned long long)(events_done * PD_T + i), b);
+                    const int id = sample_row(p, b, i, ev0, u, s_p, s_i, s_cnt, s_red);
+                    if (threadIdx.x == 0) p.ev_t[(size_t)i * B + b] = id;
+                } else if (threadIdx.x == 0) {
+                    p.ev_t[(size_t)i * B + b] = d.pad_id;     // a row that is not live draws nothing
+                }
             }
             prof.sub(PH_SAMPLE, 1);
         }
@@ -827,7 +855,9 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
             const int b = k / PD_T, t = k % PD_T;
             const long long v = (t < n_steps) ? __ldcg(p.ev_t + (size_t)t * B + b) : (long long)d.pad_id;
             cur_ev[k] = (int)v;
-            if (blockIdx.x == 0) {
+            bool commit = blockIdx.x == 0;
+            if constexpr (QUEUE) commit = commit && ((live >> b) & 1u);
+            if (commit) {
                 int row_pos = pos;                        // RAGGED: row b commits at its own position
                 if constexpr (RAGGED) row_pos += p.row_off[b];
                 d.seq[((size_t)b * d.max_len + row_pos + 1) * PD_T + t] = v;
@@ -836,8 +866,25 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
         }
         __syncthreads();
         prof.mark(PH_COMMIT);
+        unsigned fin = 0;                                 // QUEUE: rows that finished in this event
+        if constexpr (QUEUE) {
+            // Every thread of the grid derives the same finish flags from the same values (the event types, visible since
+            // the barrier above, row_off and row_end), so the decision to leave is uniform without another barrier.
+            for (int b = 0; b < B; b++) {
+                if (!((live >> b) & 1u)) continue;
+                const int last = pos + p.row_off[b] + 1;  // seq index of the event row b just committed
+                if (cur_ev[b * PD_T] == d.eos_id || last >= p.row_end[b]) {
+                    fin |= 1u << b;
+                    if (blockIdx.x == 0 && threadIdx.x == 0) p.row_last[b] = last;
+                }
+            }
+            live &= ~fin;
+        }
         pos++;
         events_done++;
+        if constexpr (QUEUE) {
+            if (live == 0 || (fin != 0 && p.exit_on_done)) break;
+        }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         *d.pos = pos;
@@ -875,11 +922,12 @@ extern "C" size_t b200_decode_desc_bytes(void) { return sizeof(b200_decode_desc)
 
 namespace {
 
-template <bool RAGGED>
-int decode_events(const b200_decode_desc* desc, const int* row_off, int n_events, void* workspace, size_t workspace_bytes,
-                  cudaStream_t stream) {
+template <bool RAGGED, bool QUEUE = false>
+int decode_events(const b200_decode_desc* desc, const int* row_off, const int* row_end, int* row_last, int exit_on_done,
+                  int n_events, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     const b200_decode_desc& d = *desc;
     B200_CHECK_ARG(!RAGGED || row_off != nullptr, "decode_events_ragged: row_off required");
+    B200_CHECK_ARG(!QUEUE || (row_end != nullptr && row_last != nullptr), "decode_events_queue: row_end and row_last required");
     B200_CHECK_ARG(d.batch >= 1 && d.batch <= 16, "decode_events: batch %d outside 1..16", d.batch);
     B200_CHECK_ARG(d.H == 1024 && d.nh_outer * 64 == d.H && d.nh_inner * 256 == d.H,
                    "decode_events: built for hidden 1024 (16 x 64 event-level heads, 4 x 256 token-level heads)");
@@ -917,20 +965,25 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, int n_events
     p.k_max = d.I_outer > d.I_inner ? d.I_outer : d.I_inner;
     if (p.k_max < d.H) p.k_max = d.H;
     B200_CUDA(cudaMemsetAsync(p.bar, 0, 256, stream), "decode_events: barrier reset");
-    PDArg<RAGGED> pk;
+    PDArg<RAGGED, QUEUE> pk;
     static_cast<PD&>(pk) = p;
     if constexpr (RAGGED) pk.row_off = row_off;
+    if constexpr (QUEUE) {
+        pk.row_end = row_end;
+        pk.row_last = row_last;
+        pk.exit_on_done = exit_on_done;
+    }
     const int bm = d.batch <= 1 ? 1 : d.batch <= 2 ? 2 : d.batch <= 4 ? 4 : d.batch <= 8 ? 8 : 16;
     const size_t smem = (size_t)bm * p.k_max * 2 + (size_t)smp::SMP_MAXV * 8 + (PD_THREADS + 8) * 4 + 64 * 4 +
                         PD_WARPS * 64 * (4 + 2 + 2) + (size_t)bm * PD_T * 4 + 64;
     void* args[] = {(void*)&pk};
     const void* fn = nullptr;
     switch (bm) {
-        case 1: fn = (const void*)decode_events_kernel<1, RAGGED>; break;
-        case 2: fn = (const void*)decode_events_kernel<2, RAGGED>; break;
-        case 4: fn = (const void*)decode_events_kernel<4, RAGGED>; break;
-        case 8: fn = (const void*)decode_events_kernel<8, RAGGED>; break;
-        default: fn = (const void*)decode_events_kernel<16, RAGGED>; break;
+        case 1: fn = (const void*)decode_events_kernel<1, RAGGED, QUEUE>; break;
+        case 2: fn = (const void*)decode_events_kernel<2, RAGGED, QUEUE>; break;
+        case 4: fn = (const void*)decode_events_kernel<4, RAGGED, QUEUE>; break;
+        case 8: fn = (const void*)decode_events_kernel<8, RAGGED, QUEUE>; break;
+        default: fn = (const void*)decode_events_kernel<16, RAGGED, QUEUE>; break;
     }
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "decode_events smem attr");
     int per_sm = 0;
@@ -946,10 +999,17 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, int n_events
 
 extern "C" int b200_decode_events(const b200_decode_desc* desc, int n_events, void* workspace, size_t workspace_bytes,
                                   cudaStream_t stream) {
-    return decode_events<false>(desc, nullptr, n_events, workspace, workspace_bytes, stream);
+    return decode_events<false>(desc, nullptr, nullptr, nullptr, 0, n_events, workspace, workspace_bytes, stream);
 }
 
 extern "C" int b200_decode_events_ragged(const b200_decode_desc* desc, const int* row_off, int n_events, void* workspace,
                                          size_t workspace_bytes, cudaStream_t stream) {
-    return decode_events<true>(desc, row_off, n_events, workspace, workspace_bytes, stream);
+    return decode_events<true>(desc, row_off, nullptr, nullptr, 0, n_events, workspace, workspace_bytes, stream);
+}
+
+extern "C" int b200_decode_events_queue(const b200_decode_desc* desc, const int* row_off, const int* row_end, int* row_last,
+                                        int exit_on_done, int n_events, void* workspace, size_t workspace_bytes,
+                                        cudaStream_t stream) {
+    return decode_events<true, true>(desc, row_off, row_end, row_last, exit_on_done, n_events, workspace, workspace_bytes,
+                                     stream);
 }

@@ -40,6 +40,16 @@ class PagedKV:
     def reset(self):
         self.length = 0
 
+    def row(self, b: int) -> "PagedKV":
+        """Row b alone as a batch-1 cache over the same memory (its slice of every pool, an identity block table), empty:
+        a request's prefill into its slot runs exactly as a batch-1 prefill does.  Never grown."""
+        v = PagedKV.__new__(PagedKV)
+        v.cfg, v.batch, v.page, v.max_pages, v.capacity, v.length = self.cfg, 1, self.page, self.max_pages, self.capacity, 0
+        rows = slice(b * self.max_pages, (b + 1) * self.max_pages)
+        v.k, v.v = [k[rows] for k in self.k], [x[rows] for x in self.v]
+        v.block_table = self.block_table[:1]              # row 0 of the identity table: pages 0 .. max_pages - 1
+        return v
+
     def grow(self, capacity: int) -> None:
         """Re-allocate the pools for at least `capacity` positions, keeping the cached keys / values (row b owns pages
         [b * max_pages, (b+1) * max_pages), so the old pages are copied to the front of each row's new range).  The
@@ -286,8 +296,14 @@ class GraphGenerator:
         self.mask = torch.ones((batch, V), dtype=torch.uint8, device=dev)
         self.row_off = torch.zeros(batch, dtype=torch.int32, device=dev)    # ragged mode: row b at pos + row_off[b]
         self.lengths = None             # ragged mode of the current call: int64 [B] prompt lengths on the device, else None
+        # request-queue mode (run_queue): row b stops at its own EOS or at seq index row_end[b]; row_last[b] is -1 while
+        # the row is live, then the seq index of its last event (-2: empty slot)
+        self.queue = False
+        self.row_end = torch.zeros(batch, dtype=torch.int32, device=dev)
+        self.row_last = torch.full((batch,), -2, dtype=torch.int32, device=dev)
         self.graph = None
         self.graph_ragged = None
+        self.graph_queue = None
         self.stream = torch.cuda.Stream(device=dev)
         self._persist = None            # (descriptor, pointer tables, workspace) of the persistent kernel, built on first use
 
@@ -347,6 +363,14 @@ class GraphGenerator:
         else:
             lib.call("b200_decode_events", ctypes.byref(d), int(n), ws.data_ptr(), ws.numel(), lib.stream())
 
+    def _events_queue(self, n: int, exit_on_done: bool) -> None:
+        """Queue mode: up to `n` events in one launch, which also ends when no row is live or, with `exit_on_done`, after
+        the event in which a row finished."""
+        import ctypes
+        d, ws, _ = self._persistent()
+        lib.call("b200_decode_events_queue", ctypes.byref(d), self.row_off.data_ptr(), self.row_end.data_ptr(),
+                 self.row_last.data_ptr(), int(exit_on_done), int(n), ws.data_ptr(), ws.numel(), lib.stream())
+
     def set_deny(self, ids) -> None:
         """Token ids that may never be sampled (empty = plain grammar)."""
         self.mask.fill_(1)
@@ -357,7 +381,7 @@ class GraphGenerator:
     def _event(self):
         B, T = self.B, self.T
         emb_o, emb_i = self.outer.eng.embed, self.inner.eng.embed
-        ragged = self.lengths is not None
+        ragged = self.lengths is not None or self.queue
         e = ops.embed_sum(self.ev_in, emb_o)
         hidden = self.outer.step(e, self.kv1, 1, pos_dev=self.pos, max_T=self.max_len,
                                  row_off=self.row_off if ragged else None)
@@ -378,7 +402,11 @@ class GraphGenerator:
             lib.call("b200_sample_from_logits", logits.data_ptr(), B, self.V, logits.stride(0), self.temp, self.top_p,
                      self.top_k, i, self.ev_t.data_ptr(), self.g.lut.data_ptr(), self.g.n_event_types, self.g.eos, self.g.pad,
                      self.mask.data_ptr(), self.u.data_ptr(), self.ev_t.data_ptr() + 8 * B * i, 1, lib.stream())
-        if ragged:
+        if self.queue:
+            lib.call("b200_event_commit_queue", self.ev_t.data_ptr(), self.seq.data_ptr(), self.ev_in.data_ptr(),
+                     self.pos.data_ptr(), B, T, self.max_len, self.row_off.data_ptr(), self.row_end.data_ptr(),
+                     self.row_last.data_ptr(), self.g.eos, lib.stream())
+        elif ragged:
             lib.call("b200_event_commit_ragged", self.ev_t.data_ptr(), self.seq.data_ptr(), self.ev_in.data_ptr(),
                      self.pos.data_ptr(), B, T, self.max_len, self.row_off.data_ptr(), lib.stream())
         else:
@@ -418,16 +446,17 @@ class GraphGenerator:
         self.lengths = torch.tensor(list(lengths), dtype=torch.int64).to(self.seq.device)
 
     def _graph(self):
+        if self.queue:
+            return self.graph_queue
         return self.graph_ragged if self.lengths is not None else self.graph
 
-    def _prepare(self, prompt: torch.Tensor, use_graph, lengths=None) -> None:
-        """Load the prompt into the device state; capture the per-event graph of this mode (rectangular or ragged) on first
-        use (current stream = self.stream)."""
-        self._set_lengths(prompt, lengths)
-        self._set_state(prompt)
+    def _capture(self, use_graph, set_state) -> None:
+        """Capture the per-event graph of the current mode on first use (current stream = self.stream); `set_state()`
+        loads the call's state and undoes the warm-up's changes to it."""
+        set_state()
         if self.table_version != self.outer.version:    # RoPE tables were re-created: the captured addresses are stale
             self.graph, self.table_version = None, self.outer.version
-            self.graph_ragged = None
+            self.graph_ragged = self.graph_queue = None
         if use_graph == "persist":
             return
         if use_graph and self._graph() is None:
@@ -436,11 +465,20 @@ class GraphGenerator:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, stream=self.stream):
                 self._event()
-            if self.lengths is not None:
+            if self.queue:
+                self.graph_queue = g
+            elif self.lengths is not None:
                 self.graph_ragged = g
             else:
                 self.graph = g
-            self._set_state(prompt)             # undo the warm-up's state changes
+            set_state()
+
+    def _prepare(self, prompt: torch.Tensor, use_graph, lengths=None) -> None:
+        """Load the prompt into the device state; capture the per-event graph of this mode (rectangular or ragged) on first
+        use (current stream = self.stream)."""
+        self.queue = False
+        self._set_lengths(prompt, lengths)
+        self._capture(use_graph, lambda: self._set_state(prompt))
 
     def _mode(self, use_graph):
         """True / "graph": CUDA-graph replay per event; False: the same launches issued from the host; "persist": the
@@ -528,6 +566,90 @@ class GraphGenerator:
             if self.lengths is not None:
                 # rows end at L_b + n_done: events a row generated past the stop point (same check_every block) become pad
                 pad_past(out, self.lengths + (out.shape[1] - P), self.tok.pad_id)
+        cur.wait_stream(self.stream)
+        return out
+
+    # ------------------------------------------------------------------ request queue (continuous batching)
+    def _set_queue_state(self) -> None:
+        """Every slot empty, the shared counter at 0, the RNG counter at its start."""
+        self.seq.fill_(self.tok.pad_id)
+        self.ev_in.fill_(self.tok.pad_id)
+        self.pos.zero_()
+        self.row_off.zero_()
+        self.row_end.zero_()
+        self.row_last.fill_(-2)
+        self.counter.copy_(torch.tensor([0, self.seed], dtype=torch.int64))
+
+    def _admit(self, b: int, prompt: torch.Tensor) -> None:
+        """Request `prompt` (int64 [L, T] on the device) into slot b: events 0 .. L-2 prefilled at batch 1 into the slot's
+        pages (nothing for a one-event prompt), event L-1 fed to the next event."""
+        L = prompt.shape[0]
+        self.seq[b].fill_(self.tok.pad_id)
+        self.seq[b, :L] = prompt
+        if L > 1:
+            self.outer.step(ops.embed_sum(prompt[:L - 1].contiguous(), self.outer.eng.embed), self.kv1.row(b), L - 1)
+        self.ev_in[b] = prompt[L - 1]
+
+    def run_queue(self, prompts, budgets, use_graph=True) -> list:
+        """Continuous batching: requests i = 0 .. N-1 (prompts[i]: int64 [L_i, T] on the device, L_i >= 1; budgets[i] >= 1
+        new events) through this loop's B slots.  Request i ends after its first new event whose event type is EOS (that
+        event is kept) or after budgets[i] new events, and its slot is refilled with the next waiting request.  Returns
+        request i's prompt and new events, int64 [L_i + n_i, T] on the device, in input order.
+
+        Row b sits at pos + row_off[b], as in ragged mode.  Between launches a finished slot takes the next request (its
+        batch-1 prefill) or becomes empty, and the rows are rebased: pos = the largest live position, row_off[b] = r_b - pos
+        <= 0, an empty slot at position 0.  So the kernel's `pos + 1 >= max_len` exit never comes before a budget, and an
+        empty slot's position stays below a live row's.  The persistent kernel runs until a row finishes while requests
+        wait (exit_on_done), else until no row is live; the graph and host-issued loops check after every event."""
+        use_graph = self._mode(use_graph)
+        N, B = len(prompts), self.B
+        ends = [p.shape[0] - 1 + int(n) for p, n in zip(prompts, budgets)]     # seq index of each request's last event
+        if max(ends) >= self.max_len:
+            raise lib.B200Error(f"a request ends at event {max(ends)}, past this loop's max_len {self.max_len}")
+        out = [None] * N
+        slot = [None] * B                  # request held by slot b (None: empty)
+        posn = [0] * B                     # position of slot b's row: the seq index of the event it feeds next
+        nxt = 0
+        cur = torch.cuda.current_stream()
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            self.queue, self.lengths = True, None
+            self._capture(use_graph, self._set_queue_state)
+            graph = self._graph()
+            free = list(range(B))
+            while True:
+                if free:
+                    for b in free:
+                        slot[b] = None
+                        if nxt < N:
+                            self._admit(b, prompts[nxt])
+                            slot[b], posn[b] = nxt, prompts[nxt].shape[0] - 1
+                            nxt += 1
+                    live = [b for b in range(B) if slot[b] is not None]
+                    if not live:
+                        break
+                    pos = max(posn[b] for b in live)
+                    offs = [posn[b] - pos if slot[b] is not None else -pos for b in range(B)]
+                    self.pos.fill_(pos)
+                    self.row_off.copy_(torch.tensor(offs, dtype=torch.int32))
+                    self.row_end.copy_(torch.tensor([ends[s] if s is not None else 0 for s in slot], dtype=torch.int32))
+                    self.row_last.copy_(torch.tensor([-1 if s is not None else -2 for s in slot], dtype=torch.int32))
+                if use_graph == "persist":
+                    self._events_queue(max(ends[slot[b]] - posn[b] for b in live), exit_on_done=nxt < N)
+                elif use_graph:
+                    graph.replay()
+                else:
+                    self._event()
+                state = torch.cat([self.pos, self.row_last]).cpu()          # one small device->host copy per launch
+                p_now, last = int(state[0]), state[1:].tolist()
+                free = []
+                for b in live:
+                    if last[b] >= 0:
+                        out[slot[b]] = self.seq[b, :last[b] + 1].clone()
+                        free.append(b)
+                    else:
+                        posn[b] = p_now + offs[b]
+                live = [b for b in live if b not in free]
         cur.wait_stream(self.stream)
         return out
 

@@ -82,10 +82,12 @@ SIGNATURES = {
     "b200_attn_decode_fused_ragged": (i32, [vp, vp, vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp, i32, i32, i32, f32, i32,
                                             vp, sz, vp, vp]),
     "b200_event_commit_ragged": (i32, [vp, vp, vp, vp, i32, i32, i32, vp, vp]),
+    "b200_event_commit_queue": (i32, [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, i32, vp]),
     "b200_decode_desc_bytes": (sz, []),
     "b200_decode_events_workspace_bytes": (sz, [vp]),
     "b200_decode_events": (i32, [vp, i32, vp, sz, vp]),
     "b200_decode_events_ragged": (i32, [vp, vp, i32, vp, sz, vp]),
+    "b200_decode_events_queue": (i32, [vp, vp, vp, vp, i32, i32, vp, sz, vp]),
 }
 
 

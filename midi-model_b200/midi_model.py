@@ -1001,6 +1001,64 @@ class MIDIModel(PreTrainedModel):
             self._return_generator(key, gg)
         return out.cpu().numpy()
 
+    def _queue_requests(self, prompts, max_new, dev):
+        """(prompts as int64 [L_i, T] device tensors, budgets) of a `generate_many` call, checked."""
+        what = "generate_many"
+        if os.environ.get("B200_GENERATE", "persist") == "eager":
+            raise _lib.B200Error(f"{what}: the request queue needs the device-resident loop (B200_GENERATE=eager)")
+        if not isinstance(prompts, collections.abc.Sequence) or isinstance(prompts, (str, bytes)) or len(prompts) == 0:
+            raise _lib.B200Error(f"{what}: prompts must be a non-empty list of [events, tokens] arrays")
+        reqs = []
+        for i, p in enumerate(prompts):
+            if isinstance(p, torch.Tensor):
+                if p.device.type != "cpu":
+                    raise _lib.B200Error(f"{what}: prompt {i} must be a numpy array or a CPU tensor, got {p.device}")
+                p = p.numpy()
+            if not isinstance(p, np.ndarray) or p.dtype.kind not in "iu" or p.ndim != 2 or p.shape[0] < 1:
+                raise _lib.B200Error(f"{what}: prompt {i} must be a 2-D integer array with at least one event, got "
+                                     f"{getattr(p, 'dtype', type(p).__name__)} {tuple(getattr(p, 'shape', ()))}")
+            reqs.append(self._prompt_tensor(p, 1, dev)[0])
+        if isinstance(max_new, numbers.Integral) and not isinstance(max_new, bool):
+            budgets = [int(max_new)] * len(reqs)
+        else:
+            budgets = _host_ints(max_new, f"{what}: max_new")
+            if len(budgets) != len(reqs):
+                raise _lib.B200Error(f"{what}: max_new has {len(budgets)} entries for {len(reqs)} prompts")
+        if min(budgets) < 1:
+            raise _lib.B200Error(f"{what}: max_new must be >= 1, got {min(budgets)}")
+        return reqs, budgets
+
+    def generate_many(self, prompts, max_new, batch_size=8, temp=1.0, top_p=0.98, top_k=20, generator=None):
+        """Continue every prompt of a request queue, each to its own end, through `batch_size` slots (continuous batching).
+
+        `prompts`: a non-empty list of 2-D integer arrays [L_i, <= T] (numpy or CPU tensors, L_i >= 1; tokens padded to T as
+        generate pads them).  `max_new`: one int or one per request, each >= 1.  Request i ends after its first new event
+        whose event type is EOS (kept) or after max_new_i new events; its slot then takes the next waiting request, so no
+        slot idles while requests wait.  Returns request i's prompt and its new events, int64 [L_i + n_i, T], in input
+        order and without pad events: the shape of generate(prompt_i, batch_size=1, max_len=L_i + max_new_i).
+
+        The call uses min(batch_size, N) slots and shares its sampling settings across requests.  A greedy request
+        (top_k=1) equals generating its prompt alone.  A sampled request draws from its slot's counter-based stream, so it
+        is reproducible for the same seed, prompts, budgets and batch_size, but it is not in general what sampling its
+        prompt alone would give.  Runs on the device-resident loop (B200_GENERATE persist, graph or nograph);
+        B200_GENERATE=eager raises B200Error."""
+        rt = self._rt()
+        dev = rt.store.device
+        reqs, budgets = self._queue_requests(prompts, max_new, dev)
+        if isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral) or batch_size < 1:
+            raise _lib.B200Error(f"generate_many: batch_size must be an int >= 1, got {batch_size!r}")
+        if rt.grammar is None:
+            rt.grammar = _dec.GrammarLUT(self.tokenizer, dev)
+        mode = os.environ.get("B200_GENERATE", "persist")
+        max_len = max(r.shape[0] + n for r, n in zip(reqs, budgets))
+        key, gg = self._checkout_generator(min(int(batch_size), len(reqs)), max_len, temp, top_p, top_k, generator)
+        try:
+            gg.set_deny(())
+            out = gg.run_queue(reqs, budgets, use_graph=_loop_mode(mode))
+        finally:
+            self._return_generator(key, gg)
+        return [o.cpu().numpy() for o in out]
+
     # ------------------------------------------------------------------ fused training path (non-reference API)
     def training_loss(self, batch: torch.Tensor, backward: bool = True, accumulate: bool = False, grad_ready=None,
                       sample_idx=None, lengths=None):
