@@ -269,6 +269,20 @@ int b200_event_commit_ragged(const long long* ev_t, long long* seq, long long* e
  *      A row that is not live writes nothing.  *pos still advances by one. */
 int b200_event_commit_queue(const long long* ev_t, long long* seq, long long* ev_next, int* pos_dev, int B, int T,
                             int max_len, const int* row_off, const int* row_end, int* row_last, int eos_id, cudaStream_t s);
+/*      per-request queue (generate_many with per-request settings or seeds):
+ *        sample_from_logits_rows: b200_sample_from_logits with row r's settings from row_temp, row_top_p, row_top_k (device
+ *          float / float / int32 [rows]).  Preconditions (the caller's: checking device values would need a sync): row_temp[r]
+ *          > 0 and row_top_k[r] >= 1.  top_k > 64 takes the general path, as in b200_sample_from_logits.
+ *        uniform_fill_rows: u[b] = hash(row_seed[b], 8 j + step, 0) with j = *pos_dev + row_off[b] - row_first[b] (row_first:
+ *          device int32 [B], seq index of the request's last prompt event; row_seed: device uint64 [B]), i.e. the draw that
+ *          b200_uniform_fill makes for a batch-1 loop seeded row_seed[b] at its new event j, token step `step`.  The position
+ *          is read on the device, so the call can be captured in a graph.  No counter is advanced. */
+int b200_sample_from_logits_rows(const void* logits, int rows, int V, int ld, const float* row_temp, const float* row_top_p,
+                                 const int* row_top_k, int step, const long long* event_tok, const int* lut, int n_event_types,
+                                 int eos_id, int pad_id, const unsigned char* dense_mask /*may be NULL*/,
+                                 const float* uniforms, long long* out, int out_stride, cudaStream_t s);
+int b200_uniform_fill_rows(float* u, int B, const int* pos_dev, const int* row_off, const int* row_first,
+                           const unsigned long long* row_seed, int step, cudaStream_t s);
 
 
 /* ---- persistent generate kernel (midi_model.py:192-248: one generated event = event-level decode step + up to 8
@@ -323,6 +337,17 @@ int b200_decode_events_ragged(const b200_decode_desc* d, const int* row_off, int
  *      the finish flags from the same values, so that exit needs no extra grid barrier. */
 int b200_decode_events_queue(const b200_decode_desc* d, const int* row_off, const int* row_end, int* row_last,
                              int exit_on_done, int n_events, void* workspace, size_t workspace_bytes, cudaStream_t s);
+/*      per-request queue: b200_decode_events_queue where row b samples with its own settings (row_temp, row_top_p,
+ *      row_top_k: device float / float / int32 [batch]) and draws hash(row_seed[b], 8 j + t, 0) at its new event
+ *      j = *pos + row_off[b] - row_first[b], token step t (b200_uniform_fill_rows); the descriptor's temp / top_p / top_k
+ *      and rng_state seed are not used for draws.  Row b's event-level attention is cut into chunks exactly as the batch-1
+ *      kernel cuts it at row b's own length, so with the same pages, position, settings, seed and mask row, row b commits
+ *      bit for bit what b200_decode_events at batch 1 commits.  Preconditions (the caller's): every live row has
+ *      row_temp > 0, 0 < row_top_p <= 1 and 1 <= row_top_k <= 64. */
+int b200_decode_events_queue_rows(const b200_decode_desc* d, const int* row_off, const int* row_end, int* row_last,
+                                  int exit_on_done, int n_events, void* workspace, size_t workspace_bytes,
+                                  const float* row_temp, const float* row_top_p, const int* row_top_k,
+                                  const unsigned long long* row_seed, const int* row_first, cudaStream_t s);
 
 #ifdef __cplusplus
 }

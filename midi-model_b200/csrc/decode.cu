@@ -532,16 +532,24 @@ sample_probs_kernel(const T* __restrict__ probs, int V, int ld, float top_p, int
 //   step 0            : [eos_id, eos_id + n_event_types]  (eos + the event-type ids, contiguous)
 //   step i > 0        : lut[(ev - first_event) * 8 + (i-1)] = (lo, hi) of that parameter; pad only if exhausted / ended
 // `event_tok` [rows] holds the step-0 token of the current event; `dense_mask` (optional, [rows, V] uint8) is ANDed.
+// ROWS: row r samples with row_temp[r], row_top_p[r], row_top_k[r] instead of the scalar settings.
+template <bool ROWS>
 __global__ void __launch_bounds__(SMP_THREADS)
 sample_logits_kernel(const bf16* __restrict__ logits, int V, int ld, float temp, float top_p, int top_k, int step,
                      const long long* __restrict__ event_tok, const int* __restrict__ lut, int n_event_types, int eos_id,
                      int pad_id, const unsigned char* __restrict__ dense_mask, const float* __restrict__ uniforms,
-                     long long* __restrict__ out, int out_stride) {
+                     long long* __restrict__ out, int out_stride, const float* __restrict__ row_temp,
+                     const float* __restrict__ row_top_p, const int* __restrict__ row_top_k) {
     __shared__ float s_p[SMP_MAXV];
     __shared__ int s_i[SMP_MAXV];
     __shared__ int s_cnt[SMP_THREADS + 8];
     __shared__ float s_red[64];
     const int r = blockIdx.x;
+    if constexpr (ROWS) {
+        temp = row_temp[r];
+        top_p = row_top_p[r];
+        top_k = row_top_k[r];
+    }
     int lo, hi;
     if (step == 0) {
         lo = eos_id; hi = eos_id + 1 + n_event_types;
@@ -568,15 +576,22 @@ __global__ void philox_uniform_kernel(float* __restrict__ u, int n, unsigned lon
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long c = counter[0];
     seed ^= counter[1];
-    if (i < n) {
-        unsigned long long z = seed + 0x9E3779B97F4A7C15ULL * (c * 4096ULL + (unsigned long long)i + 1ULL);
-        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-        z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-        z = z ^ (z >> 31);
-        u[i] = (float)(z >> 40) * (1.0f / 16777216.0f);
-    }
+    if (i < n) u[i] = smp::counter_uniform(seed, c, (unsigned long long)i);
     __syncthreads();
     if (i == 0) *counter = c + 1;
+}
+
+// Keyed uniforms of the per-request queue: row b's draw at token step `step` of its new event j = *pos + row_off[b] -
+// row_first[b] is the draw of generating the request alone (batch 1, row 0, seed row_seed[b]): hash(row_seed[b], 8 j + step,
+// 0).  The position is read on the device, so a captured graph replays it.
+__global__ void uniform_rows_kernel(float* __restrict__ u, int B, const int* __restrict__ pos, const int* __restrict__ row_off,
+                                    const int* __restrict__ row_first, const unsigned long long* __restrict__ row_seed,
+                                    int step) {
+    const int b = threadIdx.x;
+    if (b < B) {
+        const int j = *pos + row_off[b] - row_first[b];
+        u[b] = smp::counter_uniform(row_seed[b], (unsigned long long)j * 8ULL + (unsigned long long)step, 0ULL);
+    }
 }
 
 // End of one generated event (graph-captured loop): ev_t [T][B] (token-major scratch written by the sampler)
@@ -881,10 +896,26 @@ extern "C" int b200_sample_from_logits(const void* logits, int rows, int V, int 
     B200_CHECK_ARG(temp > 0.f, "sample_from_logits: temperature must be positive");
     if (rows == 0) return B200_OK;
     if (top_k < 1) top_k = 1;
-    sample_logits_kernel<<<rows, SMP_THREADS, 0, stream>>>((const bf16*)logits, V, ld, temp, top_p, top_k, step,
-                                                          event_tok, lut, n_event_types, eos_id, pad_id, dense_mask,
-                                                          uniforms, out, out_stride);
+    sample_logits_kernel<false><<<rows, SMP_THREADS, 0, stream>>>((const bf16*)logits, V, ld, temp, top_p, top_k, step,
+                                                                 event_tok, lut, n_event_types, eos_id, pad_id, dense_mask,
+                                                                 uniforms, out, out_stride, nullptr, nullptr, nullptr);
     B200_CHECK_LAUNCH("sample_from_logits");
+    return B200_OK;
+}
+
+extern "C" int b200_sample_from_logits_rows(const void* logits, int rows, int V, int ld, const float* row_temp,
+                                            const float* row_top_p, const int* row_top_k, int step, const long long* event_tok,
+                                            const int* lut, int n_event_types, int eos_id, int pad_id,
+                                            const unsigned char* dense_mask, const float* uniforms, long long* out,
+                                            int out_stride, cudaStream_t stream) {
+    B200_CHECK_ARG(V <= SMP_MAXV, "sample_from_logits_rows: vocabulary %d exceeds %d", V, SMP_MAXV);
+    B200_CHECK_ARG(row_temp != nullptr && row_top_p != nullptr && row_top_k != nullptr,
+                   "sample_from_logits_rows: row_temp, row_top_p and row_top_k required");
+    if (rows == 0) return B200_OK;
+    sample_logits_kernel<true><<<rows, SMP_THREADS, 0, stream>>>((const bf16*)logits, V, ld, 1.f, 1.f, 1, step, event_tok,
+                                                                lut, n_event_types, eos_id, pad_id, dense_mask, uniforms,
+                                                                out, out_stride, row_temp, row_top_p, row_top_k);
+    B200_CHECK_LAUNCH("sample_from_logits_rows");
     return B200_OK;
 }
 
@@ -893,6 +924,16 @@ extern "C" int b200_uniform_fill(float* u, int n, unsigned long long seed, unsig
     B200_CHECK_ARG(n >= 1 && n <= 1024, "uniform_fill: n outside 1..1024");
     philox_uniform_kernel<<<1, 1024, 0, stream>>>(u, n, seed, counter_dev);
     B200_CHECK_LAUNCH("uniform_fill");
+    return B200_OK;
+}
+
+extern "C" int b200_uniform_fill_rows(float* u, int B, const int* pos_dev, const int* row_off, const int* row_first,
+                                      const unsigned long long* row_seed, int step, cudaStream_t stream) {
+    B200_CHECK_ARG(B >= 1 && B <= 1024, "uniform_fill_rows: B outside 1..1024");
+    B200_CHECK_ARG(pos_dev != nullptr && row_off != nullptr && row_first != nullptr && row_seed != nullptr,
+                   "uniform_fill_rows: pos, row_off, row_first and row_seed required");
+    uniform_rows_kernel<<<1, (B + 31) / 32 * 32, 0, stream>>>(u, B, pos_dev, row_off, row_first, row_seed, step);
+    B200_CHECK_LAUNCH("uniform_fill_rows");
     return B200_OK;
 }
 

@@ -74,8 +74,16 @@ struct PDQueue : PDRagged {
     int* row_last;                       // [B]: -1 while row b is live, else the seq index of its last event (-2: empty)
     int exit_on_done;                    // leave after the event in which a row finished
 };
-template <bool RAGGED, bool QUEUE = false>
-using PDArg = std::conditional_t<QUEUE, PDQueue, std::conditional_t<RAGGED, PDRagged, PD>>;
+// parameters of the per-request queue kernel (b200_decode_events_queue_rows): the queue ones plus each row's sampling
+// settings and RNG key; row b's new event j = pos + row_off[b] - row_first[b] draws hash(row_seed[b], 8 j + t, 0)
+struct PDRows : PDQueue {
+    const float *row_temp, *row_top_p;   // [B]
+    const int* row_top_k;                // [B], 1..64
+    const unsigned long long* row_seed;  // [B]
+    const int* row_first;                // [B]: seq index of the request's last prompt event
+};
+template <bool RAGGED, bool QUEUE = false, bool ROWS = false>
+using PDArg = std::conditional_t<ROWS, PDRows, std::conditional_t<QUEUE, PDQueue, std::conditional_t<RAGGED, PDRagged, PD>>>;
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
     unsigned v;
@@ -332,14 +340,26 @@ __device__ __forceinline__ size_t kv_base(const int* bt, int max_pages, int page
     return (((size_t)pg * nh + h) * page + (t % page)) * D;
 }
 
+// The chunk grid of the batch-1 kernel over a context of T positions (outer_attention with B = 1): returns the chunk length
+// and sets n_chunks.  The ROWS kernel cuts each row this way, so that the row's sums do not depend on the batch.
+__device__ __forceinline__ int rows_grid(int T, int nh, int ngw, int& n_chunks) {
+    const int target = min(PD_MAXC, max(1, ngw / nh));
+    const int chunk = ((T + target - 1) / target + 31) / 32 * 32;
+    n_chunks = (T + chunk - 1) / chunk;
+    return chunk;
+}
+
 // RAGGED: row b's new position is pos + row_off[b] <= pos.  The chunk grid stays on the shared length pos + 1 (uniform
 // across the grid), so the trailing chunks of a shorter row can be empty: their key loop does not run and they write the
 // neutral partial (m = -inf, l = 0, o = 0), which the combine pass weights by exp(-inf - mx) = 0.  Chunk 0 is never empty.
 // QUEUE: a row that is not live (row_last[b] != -1, written by CTA 0 at the last commit and read after a grid barrier)
 // skips its items: it appends nothing and reads none of its pages.
-template <bool RAGGED, bool QUEUE = false>
-__device__ __noinline__ void outer_attention(const PDArg<RAGGED, QUEUE>& p, int layer, int pos_shared, int B, int gw, int ngw,
-                                                int lane, float* q_s, bf16* kn_s, bf16* vn_s, int& n_chunks_out) {
+// ROWS (implies QUEUE): each live row's context is cut as the batch-1 kernel cuts it at the row's own length (rows_grid),
+// so its attention sums in the order of generating it alone; the items run over (b, h, c < n_chunks_b) of the live rows.
+// A row with one chunk writes its output directly; n_chunks_out is the largest count of a live row, the same in every CTA.
+template <bool RAGGED, bool QUEUE = false, bool ROWS = false>
+__device__ __noinline__ void outer_attention(const PDArg<RAGGED, QUEUE, ROWS>& p, int layer, int pos_shared, int B, int gw,
+                                                int ngw, int lane, float* q_s, bf16* kn_s, bf16* vn_s, int& n_chunks_out) {
     const DD& d = p.d;
     constexpr int D = 64;
     const int nh = d.nh_outer, H = d.H;
@@ -352,18 +372,41 @@ __device__ __noinline__ void outer_attention(const PDArg<RAGGED, QUEUE>& p, int 
     chunk = (chunk + 31) / 32 * 32;
     const int n_chunks = (T + chunk - 1) / chunk;
     n_chunks_out = n_chunks;
+    int n_items = 0;                                     // ROWS: items of the live rows
+    if constexpr (ROWS) {
+        n_chunks_out = 1;
+        for (int b = 0; b < B; b++) {
+            if (__ldcg(p.row_last + b) != -1) continue;
+            int nc;
+            rows_grid(pos_shared + p.row_off[b] + 1, nh, ngw, nc);
+            n_items += nh * nc;
+            n_chunks_out = max(n_chunks_out, nc);
+        }
+    }
     bf16* kpool = reinterpret_cast<bf16*>(d.kv_outer[layer * 2 + 0]);
     bf16* vpool = reinterpret_cast<bf16*>(d.kv_outer[layer * 2 + 1]);
     const float scale = 0.125f;
-    for (int it = gw; it < items * n_chunks; it += ngw) {
-        const int bh = it / n_chunks, c = it % n_chunks;
-        const int b = bh / nh, h = bh % nh;
-        if constexpr (QUEUE) {
+    for (int it = gw; it < (ROWS ? n_items : items * n_chunks); it += ngw) {
+        int bh = it / n_chunks, c = it % n_chunks;
+        int b = bh / nh, h = bh % nh;
+        int chunk_b = chunk, n_chunks_b = n_chunks;      // ROWS: the grid of row b
+        if constexpr (ROWS) {
+            int r = it;                                  // item r of the live rows' items, in row order
+            for (b = 0;; b++) {
+                if (__ldcg(p.row_last + b) != -1) continue;
+                chunk_b = rows_grid(pos_shared + p.row_off[b] + 1, nh, ngw, n_chunks_b);
+                if (r < nh * n_chunks_b) break;
+                r -= nh * n_chunks_b;
+            }
+            h = r / n_chunks_b;
+            c = r % n_chunks_b;
+            bh = b * nh + h;
+        } else if constexpr (QUEUE) {
             if (__ldcg(p.row_last + b) != -1) continue;
         }
         int pos = pos_shared;
         if constexpr (RAGGED) pos += p.row_off[b];
-        const int t0 = c * chunk, t1 = min(pos + 1, t0 + chunk);
+        const int t0 = c * chunk_b, t1 = min(pos + 1, t0 + chunk_b);
         const bf16* row = p.qkv + (size_t)b * 3 * H;
         const float cs = __bfloat162float(d.cos_outer[(size_t)pos * 32 + lane]), sn = __bfloat162float(d.sin_outer[(size_t)pos * 32 + lane]);
         {
@@ -451,7 +494,7 @@ __device__ __noinline__ void outer_attention(const PDArg<RAGGED, QUEUE>& p, int 
             av[j] += __shfl_xor_sync(0xffffffffu, av[j], 8);
             av[j] += __shfl_xor_sync(0xffffffffu, av[j], 16);
         }
-        if (n_chunks == 1) {
+        if (n_chunks_b == 1) {
             if (kg == 0) {
                 const float inv = 1.f / l_run;
 #pragma unroll
@@ -489,6 +532,37 @@ __device__ __noinline__ void outer_attention_combine(const PD& p, int B, int n_c
             a1 = fmaf(o.y, w, a1);
         }
         const int b = bh / nh, h = bh % nh;
+        const float inv = 1.f / l;
+        *reinterpret_cast<bf162*>(p.attn + (size_t)b * H + h * D + 2 * lane) = __floats2bfloat162_rn(a0 * inv, a1 * inv);
+    }
+}
+// ROWS: each live row with more than one chunk combines exactly its own n_chunks_b partials (outer_attention)
+__device__ __noinline__ void outer_attention_combine_rows(const PDRows& p, int pos_shared, int B, int gw, int ngw, int lane) {
+    constexpr int D = 64;
+    const int nh = p.d.nh_outer, H = p.d.H;
+    for (int bh = gw; bh < B * nh; bh += ngw) {
+        const int b = bh / nh;
+        if (__ldcg(p.row_last + b) != -1) continue;
+        int n_chunks;
+        rows_grid(pos_shared + p.row_off[b] + 1, nh, ngw, n_chunks);
+        if (n_chunks == 1) continue;
+        // the arithmetic of outer_attention_combine for this (row, head), written out here so that the instructions of
+        // that function (and of the kernels that call it) stay as they are
+        const float* pp = p.partial + (size_t)bh * PD_MAXC * (D + 2);
+        float mx = -INFINITY;
+        for (int c = lane; c < n_chunks; c += 32) mx = fmaxf(mx, __ldcg(pp + c * (D + 2)));
+        mx = warp_max(mx);
+        float l = 0.f;
+        for (int c = lane; c < n_chunks; c += 32) l += __ldcg(pp + c * (D + 2) + 1) * __expf(__ldcg(pp + c * (D + 2)) - mx);
+        l = warp_sum(l);
+        float a0 = 0.f, a1 = 0.f;
+        for (int c = 0; c < n_chunks; c++) {
+            const float w = __expf(__ldcg(pp + c * (D + 2)) - mx);
+            const float2 o = __ldcg(reinterpret_cast<const float2*>(pp + c * (D + 2) + 2 + 2 * lane));
+            a0 = fmaf(o.x, w, a0);
+            a1 = fmaf(o.y, w, a1);
+        }
+        const int h = bh % nh;
         const float inv = 1.f / l;
         *reinterpret_cast<bf162*>(p.attn + (size_t)b * H + h * D + 2 * lane) = __floats2bfloat162_rn(a0 * inv, a1 * inv);
     }
@@ -571,6 +645,8 @@ __device__ __noinline__ void inner_attention(const PD& p, int layer, int step, i
 }
 
 // ---- sampling of one row by one CTA (sample_logits_kernel of decode.cu, for PD_THREADS threads) -------------------
+// ROWS: row b's own temp / top_p / top_k instead of the descriptor's
+template <bool ROWS = false>
 __device__ __noinline__ int sample_row(const PD& p, int b, int step, long long ev0, float u, float* s_p, int* s_i, int* s_cnt, float* s_red) {
     const DD& d = p.d;
     const int V = d.V;
@@ -586,25 +662,30 @@ __device__ __noinline__ int sample_row(const PD& p, int b, int step, long long e
             if (hi <= lo) { lo = d.pad_id; hi = d.pad_id + 1; }
         }
     }
+    if constexpr (ROWS) {
+        const PDRows& r = static_cast<const PDRows&>(p);
+        return smp::sample_logits_row<PD_THREADS, true>(p.logits + (size_t)b * d.pitch, V, r.row_temp[b], r.row_top_p[b],
+                                                        r.row_top_k[b], lo, hi, d.dense_mask ? d.dense_mask + (size_t)b * V : nullptr,
+                                                        u, s_p, s_i, s_cnt, s_red, true);
+    }
     return smp::sample_logits_row<PD_THREADS, true>(p.logits + (size_t)b * d.pitch, V, d.temp, d.top_p, d.top_k, lo, hi,
                                               d.dense_mask ? d.dense_mask + (size_t)b * V : nullptr, u, s_p, s_i, s_cnt, s_red,
                                               true);
 }
 
 __device__ __forceinline__ float rng_uniform(unsigned long long seed, unsigned long long c, int i) {
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ULL * (c * 4096ULL + (unsigned long long)i + 1ULL);
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z = z ^ (z >> 31);
-    return (float)(z >> 40) * (1.0f / 16777216.0f);
+    return smp::counter_uniform(seed, c, (unsigned long long)i);
 }
 
 // =================================================================================================================
 // QUEUE (implies RAGGED): each row stops on its own.  A live row finishes at the commit of an event that is EOS or lands on
 // row_end[b]; a row that is not live commits nothing, takes no part in the token-step count and skips its attention items.
-template <int BM, bool RAGGED, bool QUEUE = false>
-__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED, QUEUE> p) {
+// ROWS (implies QUEUE): per-request rows.  Row b samples with its own settings and draws from its own key (PDRows), and its
+// event-level attention is cut on its own length (outer_attention), so a row's events do not depend on the other rows.
+template <int BM, bool RAGGED, bool QUEUE = false, bool ROWS = false>
+__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED, QUEUE, ROWS> p) {
     static_assert(!QUEUE || RAGGED, "the queue kernel positions its rows through row_off");
+    static_assert(!ROWS || QUEUE, "per-request rows are queue rows");
     extern __shared__ __align__(16) uint8_t pd_smem[];
     const DD& d = p.d;
     const int B = d.batch, H = d.H;
@@ -688,12 +769,13 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
             grid_sync(gb);
             prof.mark(PH_QKV_O);
             int n_chunks;
-            outer_attention<RAGGED, QUEUE>(p, l, pos, B, gw, ngw, lane, q_s, kn_s, vn_s, n_chunks);
+            outer_attention<RAGGED, QUEUE, ROWS>(p, l, pos, B, gw, ngw, lane, q_s, kn_s, vn_s, n_chunks);
             prof.sub(PH_ATT_O, 1);
             if (n_chunks > 1) {
                 grid_sync(gb);
                 prof.mark(PH_ATT_O);
-                outer_attention_combine(p, B, n_chunks, gw, ngw, lane);
+                if constexpr (ROWS) outer_attention_combine_rows(p, pos, B, gw, ngw, lane);
+                else outer_attention_combine(p, B, n_chunks, gw, ngw, lane);
                 prefetch_rows<false>(pre, w.o, H, H, gwv, lane, pol_stream);
                 grid_sync(gb);
                 prof.mark(PH_CMB_O);
@@ -838,8 +920,14 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
                 if constexpr (QUEUE) sample = (live >> b) & 1u;
                 if (sample) {
                     const long long ev0 = (i == 0) ? 0 : __ldcg(p.ev_t + b);
-                    const float u = rng_uniform(rng_seed, rng_c0 + (unsigned long long)(events_done * PD_T + i), b);
-                    const int id = sample_row(p, b, i, ev0, u, s_p, s_i, s_cnt, s_red);
+                    float u;
+                    if constexpr (ROWS) {       // the draw of generating the request alone: batch 1, row 0, its own seed
+                        const int j = pos + p.row_off[b] - p.row_first[b];
+                        u = rng_uniform(p.row_seed[b], (unsigned long long)(j * PD_T + i), 0);
+                    } else {
+                        u = rng_uniform(rng_seed, rng_c0 + (unsigned long long)(events_done * PD_T + i), b);
+                    }
+                    const int id = sample_row<ROWS>(p, b, i, ev0, u, s_p, s_i, s_cnt, s_red);
                     if (threadIdx.x == 0) p.ev_t[(size_t)i * B + b] = id;
                 } else if (threadIdx.x == 0) {
                     p.ev_t[(size_t)i * B + b] = d.pad_id;     // a row that is not live draws nothing
@@ -922,12 +1010,23 @@ extern "C" size_t b200_decode_desc_bytes(void) { return sizeof(b200_decode_desc)
 
 namespace {
 
-template <bool RAGGED, bool QUEUE = false>
+// per-request settings of the ROWS kernel (b200_decode_events_queue_rows)
+struct RowArgs {
+    const float *temp, *top_p;
+    const int* top_k;
+    const unsigned long long* seed;
+    const int* first;
+};
+
+template <bool RAGGED, bool QUEUE = false, bool ROWS = false>
 int decode_events(const b200_decode_desc* desc, const int* row_off, const int* row_end, int* row_last, int exit_on_done,
-                  int n_events, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+                  int n_events, void* workspace, size_t workspace_bytes, cudaStream_t stream, const RowArgs* rows = nullptr) {
     const b200_decode_desc& d = *desc;
     B200_CHECK_ARG(!RAGGED || row_off != nullptr, "decode_events_ragged: row_off required");
     B200_CHECK_ARG(!QUEUE || (row_end != nullptr && row_last != nullptr), "decode_events_queue: row_end and row_last required");
+    B200_CHECK_ARG(!ROWS || (rows != nullptr && rows->temp != nullptr && rows->top_p != nullptr && rows->top_k != nullptr &&
+                             rows->seed != nullptr && rows->first != nullptr),
+                   "decode_events_queue_rows: row_temp, row_top_p, row_top_k, row_seed and row_first required");
     B200_CHECK_ARG(d.batch >= 1 && d.batch <= 16, "decode_events: batch %d outside 1..16", d.batch);
     B200_CHECK_ARG(d.H == 1024 && d.nh_outer * 64 == d.H && d.nh_inner * 256 == d.H,
                    "decode_events: built for hidden 1024 (16 x 64 event-level heads, 4 x 256 token-level heads)");
@@ -965,7 +1064,7 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, const int* r
     p.k_max = d.I_outer > d.I_inner ? d.I_outer : d.I_inner;
     if (p.k_max < d.H) p.k_max = d.H;
     B200_CUDA(cudaMemsetAsync(p.bar, 0, 256, stream), "decode_events: barrier reset");
-    PDArg<RAGGED, QUEUE> pk;
+    PDArg<RAGGED, QUEUE, ROWS> pk;
     static_cast<PD&>(pk) = p;
     if constexpr (RAGGED) pk.row_off = row_off;
     if constexpr (QUEUE) {
@@ -973,17 +1072,24 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, const int* r
         pk.row_last = row_last;
         pk.exit_on_done = exit_on_done;
     }
+    if constexpr (ROWS) {
+        pk.row_temp = rows->temp;
+        pk.row_top_p = rows->top_p;
+        pk.row_top_k = rows->top_k;
+        pk.row_seed = rows->seed;
+        pk.row_first = rows->first;
+    }
     const int bm = d.batch <= 1 ? 1 : d.batch <= 2 ? 2 : d.batch <= 4 ? 4 : d.batch <= 8 ? 8 : 16;
     const size_t smem = (size_t)bm * p.k_max * 2 + (size_t)smp::SMP_MAXV * 8 + (PD_THREADS + 8) * 4 + 64 * 4 +
                         PD_WARPS * 64 * (4 + 2 + 2) + (size_t)bm * PD_T * 4 + 64;
     void* args[] = {(void*)&pk};
     const void* fn = nullptr;
     switch (bm) {
-        case 1: fn = (const void*)decode_events_kernel<1, RAGGED, QUEUE>; break;
-        case 2: fn = (const void*)decode_events_kernel<2, RAGGED, QUEUE>; break;
-        case 4: fn = (const void*)decode_events_kernel<4, RAGGED, QUEUE>; break;
-        case 8: fn = (const void*)decode_events_kernel<8, RAGGED, QUEUE>; break;
-        default: fn = (const void*)decode_events_kernel<16, RAGGED, QUEUE>; break;
+        case 1: fn = (const void*)decode_events_kernel<1, RAGGED, QUEUE, ROWS>; break;
+        case 2: fn = (const void*)decode_events_kernel<2, RAGGED, QUEUE, ROWS>; break;
+        case 4: fn = (const void*)decode_events_kernel<4, RAGGED, QUEUE, ROWS>; break;
+        case 8: fn = (const void*)decode_events_kernel<8, RAGGED, QUEUE, ROWS>; break;
+        default: fn = (const void*)decode_events_kernel<16, RAGGED, QUEUE, ROWS>; break;
     }
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "decode_events smem attr");
     int per_sm = 0;
@@ -1012,4 +1118,14 @@ extern "C" int b200_decode_events_queue(const b200_decode_desc* desc, const int*
                                         cudaStream_t stream) {
     return decode_events<true, true>(desc, row_off, row_end, row_last, exit_on_done, n_events, workspace, workspace_bytes,
                                      stream);
+}
+
+extern "C" int b200_decode_events_queue_rows(const b200_decode_desc* desc, const int* row_off, const int* row_end,
+                                             int* row_last, int exit_on_done, int n_events, void* workspace,
+                                             size_t workspace_bytes, const float* row_temp, const float* row_top_p,
+                                             const int* row_top_k, const unsigned long long* row_seed, const int* row_first,
+                                             cudaStream_t stream) {
+    const RowArgs rows{row_temp, row_top_p, row_top_k, row_seed, row_first};
+    return decode_events<true, true, true>(desc, row_off, row_end, row_last, exit_on_done, n_events, workspace,
+                                           workspace_bytes, stream, &rows);
 }

@@ -12,6 +12,15 @@ constexpr int SMP_MAXV = 4096;
 // sampler
 // ---------------------------------------------------------------------------------------------
 
+// The generate loops' counter-based uniform in [0, 1): draw i of counter value c under `seed` (a splitmix64 finaliser).
+__device__ __forceinline__ float counter_uniform(unsigned long long seed, unsigned long long c, unsigned long long i) {
+    unsigned long long z = seed + 0x9E3779B97F4A7C15ULL * (c * 4096ULL + i + 1ULL);
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+    z = z ^ (z >> 31);
+    return (float)(z >> 40) * (1.0f / 16777216.0f);
+}
+
 __device__ __forceinline__ bool key_before(float pa, int ia, float pb, int ib) {   // sort order: prob desc, id asc
     return (pa > pb) || (pa == pb && ia < ib);
 }

@@ -301,16 +301,35 @@ class GraphGenerator:
         self.queue = False
         self.row_end = torch.zeros(batch, dtype=torch.int32, device=dev)
         self.row_last = torch.full((batch,), -2, dtype=torch.int32, device=dev)
+        # per-request queue (run_queue with `settings`): slot b's request samples with its own temp / top_p / top_k and
+        # draws hash(row_seed[b], 8 j + t, 0) at its new event j = pos + row_off[b] - row_first[b] (the `_rows` entries);
+        # the arrays are allocated by the first per-request call (alloc_rows)
+        self.rows = False
+        self.req_top_k = []             # top_k of every request of the current per-request call (persistent_ok)
+        self.row_temp = self.row_top_p = self.row_top_k = self.row_seed = self.row_first = None
         self.graph = None
         self.graph_ragged = None
         self.graph_queue = None
+        self.graph_queue_rows = None
         self.stream = torch.cuda.Stream(device=dev)
         self._persist = None            # (descriptor, pointer tables, workspace) of the persistent kernel, built on first use
+
+    def alloc_rows(self) -> None:
+        """The per-request arrays, allocated by the first per-request call: a loop that only runs scalar settings does
+        not carry them."""
+        if self.row_temp is None:
+            dev, B = self.pos.device, self.B
+            self.row_temp = torch.ones(B, dtype=torch.float32, device=dev)
+            self.row_top_p = torch.ones(B, dtype=torch.float32, device=dev)
+            self.row_top_k = torch.ones(B, dtype=torch.int32, device=dev)
+            self.row_seed = torch.zeros(B, dtype=torch.int64, device=dev)
+            self.row_first = torch.zeros(B, dtype=torch.int32, device=dev)
 
     # ------------------------------------------------------------------ persistent kernel (csrc/decode_persist.cu)
     def persistent_ok(self) -> bool:
         c1, c2 = self.outer.eng.cfg, self.inner.eng.cfg
-        return (self.B <= 16 and 1 <= self.top_k <= 64 and c1.hidden == 1024 and c2.hidden == 1024 and c1.head_dim == 64 and c2.head_dim == 256
+        top_ks = self.req_top_k if self.rows else [self.top_k]
+        return (self.B <= 16 and all(1 <= k <= 64 for k in top_ks) and c1.hidden == 1024 and c2.hidden == 1024 and c1.head_dim == 64 and c2.head_dim == 256
                 and c1.inner % 256 == 0 and c2.inner % 256 == 0 and self.T == 8 and self.kv1.page % 32 == 0)
 
     def _persistent(self):
@@ -368,8 +387,14 @@ class GraphGenerator:
         the event in which a row finished."""
         import ctypes
         d, ws, _ = self._persistent()
-        lib.call("b200_decode_events_queue", ctypes.byref(d), self.row_off.data_ptr(), self.row_end.data_ptr(),
-                 self.row_last.data_ptr(), int(exit_on_done), int(n), ws.data_ptr(), ws.numel(), lib.stream())
+        if self.rows:
+            lib.call("b200_decode_events_queue_rows", ctypes.byref(d), self.row_off.data_ptr(), self.row_end.data_ptr(),
+                     self.row_last.data_ptr(), int(exit_on_done), int(n), ws.data_ptr(), ws.numel(),
+                     self.row_temp.data_ptr(), self.row_top_p.data_ptr(), self.row_top_k.data_ptr(),
+                     self.row_seed.data_ptr(), self.row_first.data_ptr(), lib.stream())
+        else:
+            lib.call("b200_decode_events_queue", ctypes.byref(d), self.row_off.data_ptr(), self.row_end.data_ptr(),
+                     self.row_last.data_ptr(), int(exit_on_done), int(n), ws.data_ptr(), ws.numel(), lib.stream())
 
     def set_deny(self, ids) -> None:
         """Token ids that may never be sampled (empty = plain grammar)."""
@@ -398,6 +423,14 @@ class GraphGenerator:
             else:
                 hs = self.inner.step(xin, self.kv2, 1)
                 logits = _linear(hs, self.lm_head, pitch=self.pitch)
+            if self.rows:
+                lib.call("b200_uniform_fill_rows", self.u.data_ptr(), B, self.pos.data_ptr(), self.row_off.data_ptr(),
+                         self.row_first.data_ptr(), self.row_seed.data_ptr(), i, lib.stream())
+                lib.call("b200_sample_from_logits_rows", logits.data_ptr(), B, self.V, logits.stride(0),
+                         self.row_temp.data_ptr(), self.row_top_p.data_ptr(), self.row_top_k.data_ptr(), i,
+                         self.ev_t.data_ptr(), self.g.lut.data_ptr(), self.g.n_event_types, self.g.eos, self.g.pad,
+                         self.mask.data_ptr(), self.u.data_ptr(), self.ev_t.data_ptr() + 8 * B * i, 1, lib.stream())
+                continue
             lib.call("b200_uniform_fill", self.u.data_ptr(), B, 0, self.counter.data_ptr(), lib.stream())
             lib.call("b200_sample_from_logits", logits.data_ptr(), B, self.V, logits.stride(0), self.temp, self.top_p,
                      self.top_k, i, self.ev_t.data_ptr(), self.g.lut.data_ptr(), self.g.n_event_types, self.g.eos, self.g.pad,
@@ -447,7 +480,7 @@ class GraphGenerator:
 
     def _graph(self):
         if self.queue:
-            return self.graph_queue
+            return self.graph_queue_rows if self.rows else self.graph_queue
         return self.graph_ragged if self.lengths is not None else self.graph
 
     def _capture(self, use_graph, set_state) -> None:
@@ -456,7 +489,7 @@ class GraphGenerator:
         set_state()
         if self.table_version != self.outer.version:    # RoPE tables were re-created: the captured addresses are stale
             self.graph, self.table_version = None, self.outer.version
-            self.graph_ragged = self.graph_queue = None
+            self.graph_ragged = self.graph_queue = self.graph_queue_rows = None
         if use_graph == "persist":
             return
         if use_graph and self._graph() is None:
@@ -465,7 +498,9 @@ class GraphGenerator:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, stream=self.stream):
                 self._event()
-            if self.queue:
+            if self.queue and self.rows:
+                self.graph_queue_rows = g
+            elif self.queue:
                 self.graph_queue = g
             elif self.lengths is not None:
                 self.graph_ragged = g
@@ -476,7 +511,7 @@ class GraphGenerator:
     def _prepare(self, prompt: torch.Tensor, use_graph, lengths=None) -> None:
         """Load the prompt into the device state; capture the per-event graph of this mode (rectangular or ragged) on first
         use (current stream = self.stream)."""
-        self.queue = False
+        self.queue = self.rows = False
         self._set_lengths(prompt, lengths)
         self._capture(use_graph, lambda: self._set_state(prompt))
 
@@ -580,17 +615,26 @@ class GraphGenerator:
         self.row_last.fill_(-2)
         self.counter.copy_(torch.tensor([0, self.seed], dtype=torch.int64))
 
-    def _admit(self, b: int, prompt: torch.Tensor) -> None:
+    def _admit(self, b: int, prompt: torch.Tensor, setting=None) -> None:
         """Request `prompt` (int64 [L, T] on the device) into slot b: events 0 .. L-2 prefilled at batch 1 into the slot's
-        pages (nothing for a one-event prompt), event L-1 fed to the next event."""
+        pages (nothing for a one-event prompt), event L-1 fed to the next event.  Per-request mode: `setting` = (temp, top_p,
+        top_k, seed, denied token ids) becomes slot b's settings, RNG key (row_first = L-1: its new event j is at seq index
+        L + j) and mask row."""
         L = prompt.shape[0]
+        if setting is not None:
+            temp, top_p, top_k, seed, deny = setting
+            self.row_temp[b], self.row_top_p[b], self.row_top_k[b] = temp, top_p, top_k
+            self.row_seed[b], self.row_first[b] = seed, L - 1
+            self.mask[b].fill_(1)
+            if deny:
+                self.mask[b, torch.tensor(sorted(deny), dtype=torch.long, device=self.mask.device)] = 0
         self.seq[b].fill_(self.tok.pad_id)
         self.seq[b, :L] = prompt
         if L > 1:
             self.outer.step(ops.embed_sum(prompt[:L - 1].contiguous(), self.outer.eng.embed), self.kv1.row(b), L - 1)
         self.ev_in[b] = prompt[L - 1]
 
-    def run_queue(self, prompts, budgets, use_graph=True) -> list:
+    def run_queue(self, prompts, budgets, use_graph=True, settings=None) -> list:
         """Continuous batching: requests i = 0 .. N-1 (prompts[i]: int64 [L_i, T] on the device, L_i >= 1; budgets[i] >= 1
         new events) through this loop's B slots.  Request i ends after its first new event whose event type is EOS (that
         event is kept) or after budgets[i] new events, and its slot is refilled with the next waiting request.  Returns
@@ -600,7 +644,16 @@ class GraphGenerator:
         batch-1 prefill) or becomes empty, and the rows are rebased: pos = the largest live position, row_off[b] = r_b - pos
         <= 0, an empty slot at position 0.  So the kernel's `pos + 1 >= max_len` exit never comes before a budget, and an
         empty slot's position stays below a live row's.  The persistent kernel runs until a row finishes while requests
-        wait (exit_on_done), else until no row is live; the graph and host-issued loops check after every event."""
+        wait (exit_on_done), else until no row is live; the graph and host-issued loops check after every event.
+
+        `settings` (per-request mode): one (temp, top_p, top_k, seed, denied token ids) per request, with temp > 0,
+        0 < top_p <= 1, top_k >= 1 (checked by the caller).  Request i then samples with its own settings and mask row and
+        draws what a batch-1 loop seeded `seed` draws, through the `_rows` entries; the persistent kernel needs every top_k
+        <= 64.  Without it, every slot shares this loop's settings, seed stream and mask."""
+        self.rows = settings is not None
+        self.req_top_k = [s[2] for s in settings] if self.rows else []
+        if self.rows:
+            self.alloc_rows()
         use_graph = self._mode(use_graph)
         N, B = len(prompts), self.B
         ends = [p.shape[0] - 1 + int(n) for p, n in zip(prompts, budgets)]     # seq index of each request's last event
@@ -622,7 +675,7 @@ class GraphGenerator:
                     for b in free:
                         slot[b] = None
                         if nxt < N:
-                            self._admit(b, prompts[nxt])
+                            self._admit(b, prompts[nxt], settings[nxt] if self.rows else None)
                             slot[b], posn[b] = nxt, prompts[nxt].shape[0] - 1
                             nxt += 1
                     live = [b for b in range(B) if slot[b] is not None]

@@ -83,11 +83,14 @@ SIGNATURES = {
                                             vp, sz, vp, vp]),
     "b200_event_commit_ragged": (i32, [vp, vp, vp, vp, i32, i32, i32, vp, vp]),
     "b200_event_commit_queue": (i32, [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, i32, vp]),
+    "b200_sample_from_logits_rows": (i32, [vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, i32, i32, i32, vp, vp, vp, i32, vp]),
+    "b200_uniform_fill_rows": (i32, [vp, i32, vp, vp, vp, vp, i32, vp]),
     "b200_decode_desc_bytes": (sz, []),
     "b200_decode_events_workspace_bytes": (sz, [vp]),
     "b200_decode_events": (i32, [vp, i32, vp, sz, vp]),
     "b200_decode_events_ragged": (i32, [vp, vp, i32, vp, sz, vp]),
     "b200_decode_events_queue": (i32, [vp, vp, vp, vp, i32, i32, vp, sz, vp]),
+    "b200_decode_events_queue_rows": (i32, [vp, vp, vp, vp, i32, i32, vp, sz, vp, vp, vp, vp, vp, vp]),
 }
 
 

@@ -787,13 +787,20 @@ class MIDIModel(PreTrainedModel):
                             constant_values=tok.pad_id)
         return torch.from_numpy(np.ascontiguousarray(prompt)).to(dtype=torch.long, device=dev)
 
-    def _checkout_generator(self, batch_size, max_len, temp, top_p, top_k, generator):
+    def _checkout_generator(self, batch_size, max_len, temp, top_p, top_k, generator, per_row=False):
         """Exclusive use of a device-resident generate loop for these settings, reseeded from `generator`; hand it back
-        with _return_generator.  Idle generators are reused (graph capture and KV pools are the expensive part)."""
+        with _return_generator.  Idle generators are reused (graph capture and KV pools are the expensive part).
+        `per_row`: a loop for per-request settings and seeds (generate_many), which are set per slot, so neither they nor a
+        loop seed are part of the loop: `temp`, `top_p`, `top_k` and `generator` are not used."""
         rt = self._rt()
-        gen_dev = generator.device if generator is not None else torch.device("cpu")
-        seed = int(torch.randint(0, 2 ** 62, (1,), generator=generator, device=gen_dev).item())
-        key = (batch_size, max_len, float(temp), float(top_p), int(top_k))
+        if per_row:
+            seed = 0
+            key = (batch_size, max_len, "per_row")
+            temp, top_p, top_k = 1.0, 1.0, 1
+        else:
+            gen_dev = generator.device if generator is not None else torch.device("cpu")
+            seed = int(torch.randint(0, 2 ** 62, (1,), generator=generator, device=gen_dev).item())
+            key = (batch_size, max_len, float(temp), float(top_p), int(top_k))
         self._refresh_merged(rt)
         with rt.pool_lock:
             idle = rt.gen_pool.get(key)
@@ -1028,6 +1035,78 @@ class MIDIModel(PreTrainedModel):
             raise _lib.B200Error(f"{what}: max_new must be >= 1, got {min(budgets)}")
         return reqs, budgets
 
+    def _request_settings(self, n, temp, top_p, top_k, disable_patch_change, disable_control_change, disable_channels,
+                          seeds, generator):
+        """Per-request mode of `generate_many`: one (temp, top_p, top_k, seed, denied token ids) per request, checked, or
+        None when every setting is a single value and no seeds are given (the scalar queue)."""
+        what = "generate_many"
+
+        def seq(v):
+            if isinstance(v, torch.Tensor):
+                return v.dim() == 1
+            if isinstance(v, np.ndarray):
+                return v.ndim == 1
+            return isinstance(v, collections.abc.Sequence) and not isinstance(v, (str, bytes))
+
+        def listed(v):
+            return v.tolist() if isinstance(v, (torch.Tensor, np.ndarray)) else list(v)
+
+        def channels(v, name):
+            if not seq(v):
+                raise _lib.B200Error(f"{what}: {name} must be a list of channel numbers, got {v!r}")
+            v = listed(v)
+            bad = [c for c in v if isinstance(c, bool) or not isinstance(c, numbers.Integral) or not 0 <= c <= 15]
+            if bad:
+                raise _lib.B200Error(f"{what}: {name} holds {bad[0]!r}, not a channel number in 0..15")
+            return [int(c) for c in v]
+
+        # disable_channels: None, one list of channels for every request, or one entry (None or a list) per request
+        chans_per_req = (disable_channels is not None and seq(disable_channels) and len(disable_channels) > 0
+                         and all(c is None or seq(c) for c in listed(disable_channels)))
+        if disable_channels is not None and not chans_per_req:
+            chans = channels(disable_channels, "disable_channels")
+        per_req = seeds is not None or chans_per_req or any(
+            seq(v) for v in (temp, top_p, top_k, disable_patch_change, disable_control_change))
+        if not per_req:
+            return None
+
+        def each(v, name):
+            v = listed(v) if seq(v) else [v] * n
+            if len(v) != n:
+                raise _lib.B200Error(f"{what}: {name} has {len(v)} entries for {n} prompts")
+            return v
+
+        temps, top_ps, top_ks = each(temp, "temp"), each(top_p, "top_p"), each(top_k, "top_k")
+        patch, control = each(disable_patch_change, "disable_patch_change"), each(disable_control_change,
+                                                                                   "disable_control_change")
+        if chans_per_req:
+            chans = [None if c is None else channels(c, f"disable_channels[{i}]")
+                     for i, c in enumerate(each(disable_channels, "disable_channels"))]
+        else:
+            chans = [chans if disable_channels is not None else None] * n
+        for i in range(n):
+            t, p, k = temps[i], top_ps[i], top_ks[i]
+            if isinstance(t, bool) or not isinstance(t, numbers.Real) or not math.isfinite(t) or t <= 0:
+                raise _lib.B200Error(f"{what}: temp of request {i} must be a finite number > 0, got {t!r}")
+            if isinstance(p, bool) or not isinstance(p, numbers.Real) or not 0 < p <= 1:
+                raise _lib.B200Error(f"{what}: top_p of request {i} must be in (0, 1], got {p!r}")
+            if isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1:
+                raise _lib.B200Error(f"{what}: top_k of request {i} must be an int >= 1, got {k!r}")
+        if seeds is None:
+            gen_dev = generator.device if generator is not None else torch.device("cpu")
+            seeds = [int(torch.randint(0, 2 ** 62, (1,), generator=generator, device=gen_dev).item()) for _ in range(n)]
+        else:
+            if isinstance(seeds, torch.Tensor) and seeds.device.type != "cpu":
+                raise _lib.B200Error(f"{what}: seeds must be a CPU tensor or a Python sequence")
+            if not seq(seeds) or len(seeds) != n:
+                raise _lib.B200Error(f"{what}: seeds must hold one int per prompt ({n}), got {seeds!r}")
+            seeds = listed(seeds)
+            bad = [v for v in seeds if isinstance(v, bool) or not isinstance(v, numbers.Integral) or not 0 <= v < 2 ** 62]
+            if bad:
+                raise _lib.B200Error(f"{what}: seeds must be ints in [0, 2**62), got {bad[0]!r}")
+        return [(float(temps[i]), float(top_ps[i]), int(top_ks[i]), int(seeds[i]),
+                 self._deny_ids(bool(patch[i]), bool(control[i]), chans[i])) for i in range(n)]
+
     def generate_many(self, prompts, max_new, batch_size=8, temp=1.0, top_p=0.98, top_k=20, generator=None):
         """Continue every prompt of a request queue, each to its own end, through `batch_size` slots (continuous batching).
 
@@ -1037,25 +1116,61 @@ class MIDIModel(PreTrainedModel):
         slot idles while requests wait.  Returns request i's prompt and its new events, int64 [L_i + n_i, T], in input
         order and without pad events: the shape of generate(prompt_i, batch_size=1, max_len=L_i + max_new_i).
 
-        The call uses min(batch_size, N) slots and shares its sampling settings across requests.  A greedy request
-        (top_k=1) equals generating its prompt alone.  A sampled request draws from its slot's counter-based stream, so it
-        is reproducible for the same seed, prompts, budgets and batch_size, but it is not in general what sampling its
-        prompt alone would give.  Runs on the device-resident loop (B200_GENERATE persist, graph or nograph);
-        B200_GENERATE=eager raises B200Error."""
+        `temp`, `top_p` and `top_k` take one value or one per request (per-request mode, see generate_many_requests, which
+        also takes the app's grammar options and per-request seeds).  This is generate_many_requests without those
+        keyword options."""
+        return self.generate_many_requests(prompts, max_new, batch_size, temp, top_p, top_k, generator)
+
+    def generate_many_requests(self, prompts, max_new, batch_size=8, temp=1.0, top_p=0.98, top_k=20, generator=None, *,
+                               disable_patch_change=False, disable_control_change=False, disable_channels=None,
+                               seeds=None):
+        """generate_many with each request's own sampling settings, grammar options and seed (app.py serves each user with
+        their own): `prompts`, `max_new`, the result and the request queue are those of generate_many.
+
+        The call uses min(batch_size, N) slots.  The grammar options are those of generate_stream (`disable_patch_change`,
+        `disable_control_change`, `disable_channels` = channel numbers 0..15).  A greedy request (top_k=1) equals
+        generating its prompt alone.
+
+        Scalar settings and no `seeds`: every request shares the settings and the grammar options, and a sampled request
+        draws from its slot's counter-based stream, so it is reproducible for the same seed, prompts, budgets and
+        batch_size, but it is not in general what sampling its prompt alone would give.
+
+        Per-request mode, when `seeds` (N ints in [0, 2**62)) is given or any of `temp`, `top_p`, `top_k`,
+        `disable_patch_change`, `disable_control_change` is a sequence of one value per request, or `disable_channels` is a
+        list of one entry (None or a list of channels) per request: request i samples with its own settings and grammar
+        options and draws, at its new event j and token step t, hash(seeds[i], 8 j + t, 0) -- the draw of generate's loop
+        at batch 1 seeded seeds[i].  Without `seeds`, seed i is torch.randint(0, 2**62, (1,), generator=generator), drawn
+        once per request in input order.  On the persistent kernel (B200_GENERATE=persist, batch_size <= 16, every top_k
+        <= 64) request i's attention is also summed as at batch 1, so its result is bit for bit
+        generate(prompt_i, batch_size=1, max_len=L_i + max_new_i, temp_i, top_p_i, top_k_i, generator=g_i), g_i being a
+        generator whose first draw is seeds[i] (with grammar options: the events generate_stream yields at batch 1, for
+        prompts of at most 4096 events), whatever batch_size, slot, order and other requests.  On the graph and
+        host-issued loops the settings and draws are per request too, and a sampled request is reproducible for the same
+        inputs and batch_size, but its attention's split count follows the loop's max_len, so that guarantee is not made
+        there.
+
+        Runs on the device-resident loop (B200_GENERATE persist, graph or nograph); B200_GENERATE=eager raises
+        B200Error, as do malformed prompts, budgets, per-request sequences of the wrong length, temp <= 0, top_p outside
+        (0, 1], top_k < 1, seeds out of range or of the wrong count, and channels outside 0..15."""
         rt = self._rt()
         dev = rt.store.device
         reqs, budgets = self._queue_requests(prompts, max_new, dev)
         if isinstance(batch_size, bool) or not isinstance(batch_size, numbers.Integral) or batch_size < 1:
             raise _lib.B200Error(f"generate_many: batch_size must be an int >= 1, got {batch_size!r}")
+        settings = self._request_settings(len(reqs), temp, top_p, top_k, disable_patch_change, disable_control_change,
+                                          disable_channels, seeds, generator)
         if rt.grammar is None:
             rt.grammar = _dec.GrammarLUT(self.tokenizer, dev)
         mode = os.environ.get("B200_GENERATE", "persist")
         max_len = max(r.shape[0] + n for r, n in zip(reqs, budgets))
-        key, gg = self._checkout_generator(min(int(batch_size), len(reqs)), max_len, temp, top_p, top_k, generator)
+        key, gg = self._checkout_generator(min(int(batch_size), len(reqs)), max_len, temp, top_p, top_k, generator,
+                                           per_row=settings is not None)
         try:
-            gg.set_deny(())
-            out = gg.run_queue(reqs, budgets, use_graph=_loop_mode(mode))
+            gg.set_deny(() if settings is not None else
+                        self._deny_ids(disable_patch_change, disable_control_change, disable_channels))
+            out = gg.run_queue(reqs, budgets, use_graph=_loop_mode(mode), settings=settings)
         finally:
+            gg.set_deny(())
             self._return_generator(key, gg)
         return [o.cpu().numpy() for o in out]
 
