@@ -75,14 +75,17 @@ int b200_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd /*may be
 int b200_add_rmsnorm_fwd(const void* x, const void* res, const void* w, void* h_out, void* y, float* rstd /*may be NULL*/,
                          int M, int H, float eps, cudaStream_t s);
 int b200_rmsnorm_bwd_parts(void);
-/* dx = dres + d(norm)/dx ; dw (+)= column sums.  workspace: float[b200_rmsnorm_bwd_parts() * H]; its first H + 1 words
- * (fp32 accumulator row + arrival ticket of the fused column sum) must be ZERO when first handed in -- the kernel hands
- * them back zeroed, so one cudaMemset at allocation is enough */
+/* dx = dres + d(norm)/dx ; dw (+)= column sums (M = 0: dw = 0, or unchanged when accumulating).  workspace:
+ * float[b200_rmsnorm_bwd_parts() * H]; its first H + 1 words (fp32 accumulator row + arrival ticket of the fused column
+ * sum at H = 256 / 512 / 1024) must be ZERO when first handed in.  Every call hands back zeroed all it used (the other
+ * sizes write per-CTA partials over parts * H words and clear them), so one cudaMemset at allocation is enough, whatever
+ * sequence of H the workspace then serves */
 int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, const void* dres /*may be NULL*/,
                      void* dx, void* dw /*may be NULL*/, int M, int H, int accumulate_dw, void* workspace,
                      size_t workspace_bytes, cudaStream_t s);
 
 /* ---- RoPE (hf modeling_llama.py:124-168), applied in place to the q,k thirds of packed qkv -------- */
+/* cos_t / sin_t [n_pos][half] for positions base .. base + n_pos - 1, base = *pos0_dev when given (it replaces pos0) */
 int b200_rope_table(const float* inv_freq, int half, int n_pos, int pos0, const int* pos0_dev /*may be NULL*/,
                     void* cos_t, void* sin_t, cudaStream_t s);
 /* row r sits at absolute position pos0 (+ *pos0_dev) + r % S; tables are indexed by absolute position */

@@ -808,7 +808,10 @@ extern "C" int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, co
     B200_CHECK_ARG(H % 8 == 0 && H <= ROW_THREADS * 8 * MAXV, "rmsnorm_bwd: unsupported hidden size %d", H);
     const int parts = b200_rmsnorm_bwd_parts();
     B200_CHECK_ARG(workspace_bytes >= (size_t)parts * H * sizeof(float), "rmsnorm_bwd: workspace too small");
-    if (M == 0) return B200_OK;
+    if (M == 0) {   // no rows: the column sum is zero
+        if (dw && !accumulate_dw) B200_CUDA(cudaMemsetAsync(dw, 0, (size_t)H * sizeof(bf16), stream), "rmsnorm_bwd dw");
+        return B200_OK;
+    }
     if (H == 256 || H == 512 || H == 1024) {
         int g = (M + WRB_WARPS - 1) / WRB_WARPS;
         if (g > parts) g = parts;
@@ -841,6 +844,8 @@ extern "C" int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, co
                                                                         accumulate_dw);
         B200_CHECK_LAUNCH("rmsnorm_bwd_dw");
     }
+    // the partials overwrote the warp kernels' accumulator row and ticket: hand the workspace back zeroed, as they do
+    B200_CUDA(cudaMemsetAsync(workspace, 0, (size_t)parts * H * sizeof(float), stream), "rmsnorm_bwd workspace");
     return B200_OK;
 }
 

@@ -2381,6 +2381,671 @@ def check_persist_vs_phase():
     return out
 
 
+# ------------------------------------------------------------------------------------------ train-step conformance groups
+# The rest of the train step -- embeddings, RMSNorm, RoPE, SwiGLU, token-level attention, cross-entropy, grad clip and
+# AdamW (elementwise.cu, attn_tiny.cu, train_misc.cu) -- through the C ABI, as the groups above treat the GEMM, attention
+# and decode kernels: every dispatch variant, operands in NaN-poisoned buffers, outputs in NaN buffers, scored per
+# element (or per attention row) against the fp64 restatements of tests/parity_metrics.py rounded at the kernels' own
+# rounding points (DESIGN.md 3.3).
+def _gen(seed):
+    return torch.Generator(device=DEV).manual_seed(seed)
+
+
+def _ne(a, b):
+    """Number of elements that differ (a NaN differs from everything)."""
+    return float((a != b).sum())
+
+
+# all copies and the fp32 gather-sum in the kernel's order are exact claims.  Against fp64, H100 80GB HBM3 at 700 W: the
+# gather-sum and the backward (fp32 segment sums in an order the atomics choose, one rounding; accumulate one more)
+# were correctly rounded in every element (frac 0, err_over_tol <= 0.50); the bounds allow a rare fp32 rounding to
+# reach the bf16 result (frac 1e-3 / 2e-3, one ulp, two with accumulate's second rounding)
+@bounded([
+    ("em_sentinels_changed", 0.0), ("em_nan_in_range", 0.0), ("em_sum_vs_seq32_mismatch", 0.0),
+    ("em_inner_mismatch", 0.0), ("em_rows_mismatch", 0.0), ("em_rows_ysel_mismatch", 0.0),
+    ("em_rows_bwd_mismatch", 0.0), ("em_bwd_padrow_changed", 0.0), ("em_bwd_empty_mismatch", 0.0),
+    ("min:em_bwd_cases", 16.0), ("min:em_bwd_capped_ids", 4.0), ("min:em_bwd_multislice_ids", 8.0),
+    ("em_sum_frac", 1e-3), ("em_sum_maxulp", 1.0), ("em_bwd_frac", 2e-3), ("em_bwd_maxulp", 1.0),
+    ("em_bwdacc_frac", 2e-3), ("em_bwdacc_maxulp", 2.0),
+    *[(f"em_{f}_err_over_tol", 1.0) for f in ("sum", "bwd", "bwdacc")],
+])
+def check_embed_conformance():
+    """b200_embed_sum_fwd (T = 1 / 8, ids -1 / V / 1e12 skipped, NaN table rows past V), b200_inner_input_fwd with and
+    without hidden (out-of-range ids read row 0), b200_inner_input_rows_fwd / _rows_bwd_hidden (rows outside [0, n_rows)
+    and inv = -1 give zero rows), and b200_embed_bwd in the model's two layouts (outer: 8 ids per gradient row; inner: 7
+    ids per event at rows e*8 + 1 + j, the never-read rows e*8 NaN) with one id in one slice (40 occurrences), one in
+    many (500: red.add) and one past the 32-slice cap (5000), V = 3406 / 5000 (4 / 5 scan items per thread), pad_id 0 /
+    17, accumulate 0 / 1, skipped ids -1 / V and n_ids = 0."""
+    W = _Worst("em_")
+    H = 1032                    # 129 vectors of 8: the 128-thread CTAs take a second vector
+    V = 3406
+    table = P.nan_buffer((V + 2, H), device=DEV)     # rows V, V + 1 NaN: an unclamped id reads them
+    table[:V] = randn(V, H, scale=0.02, seed=6000)
+    bad = torch.tensor([-1, V, 10 ** 12, V + 1], device=DEV)
+    # ---- gather-sum: one fp32 sum in t order, one rounding
+    for T in (1, 8):
+        M = 301
+        ids = torch.randint(0, V, (M, T), generator=_gen(6001 + T), device=DEV)
+        flat = ids.view(-1)
+        flat[::7] = bad[torch.arange(flat[::7].numel(), device=DEV) % 4]
+        out = P.nan_buffer((M + 2, H), device=DEV)
+        lib.call("b200_embed_sum_fwd", ids.data_ptr(), table.data_ptr(), out.data_ptr(), M, T, H, V, lib.stream())
+        ok = ((ids >= 0) & (ids < V))[..., None]
+        rows = table[ids.clamp(0, V - 1)]
+        seq = torch.zeros(M, H, device=DEV)
+        for t in range(T):
+            seq = seq + torch.where(ok[:, t], rows[:, t].float(), torch.zeros_like(seq))
+        case = f"sum T{T}"
+        W.add("sum", case, P.exact_metrics(out[:M], torch.where(ok, rows.double(), 0.0).sum(1)))
+        W.add("", case, {"sum_vs_seq32_mismatch": _ne(out[:M], seq.to(BF))})
+        W.add("", case, P.sentinel_report(out, (slice(0, M),)))
+    # ---- inner input builder: copies, out-of-range ids read row 0
+    E, n_ids = 57, 7
+    ids = torch.randint(0, V, (E, n_ids), generator=_gen(6010), device=DEV)
+    ids[::5, 2] = bad[torch.arange(ids[::5].shape[0], device=DEV) % 4]
+    hid = randn(E, H, seed=6011)
+    emb = table[torch.where((ids >= 0) & (ids < V), ids, 0)]
+    for has_hidden in (0, 1):
+        Tin = n_ids + has_hidden
+        out = P.nan_buffer((E * Tin + 2, H), device=DEV)
+        lib.call("b200_inner_input_fwd", hid.data_ptr() if has_hidden else None, ids.data_ptr(), table.data_ptr(),
+                 out.data_ptr(), E, n_ids, H, V, lib.stream())
+        ref = (torch.cat([hid[:, None], emb], 1) if has_hidden else emb).reshape(-1, H)
+        case = f"inner hidden{has_hidden}"
+        W.add("", case, {"inner_mismatch": _ne(out[:E * Tin], ref)})
+        W.add("", case, P.sentinel_report(out, (slice(0, E * Tin),)))
+    # ---- --sample-seq rows: unique selected rows, rows -1 / n_rows read nothing
+    n_rows, T = 90, 8
+    hid = randn(n_rows, H, seed=6020)
+    y = torch.randint(0, V, (n_rows, T), generator=_gen(6021), device=DEV)
+    y[::4, 3] = bad[torch.arange(y[::4].shape[0], device=DEV) % 4]
+    sel = torch.randperm(n_rows, generator=_gen(6022), device=DEV)[:40].int()
+    sel[5], sel[17] = -1, n_rows
+    n = sel.numel()
+    out = P.nan_buffer((n * T + 2, H), device=DEV)
+    y_sel = torch.full((n * T + 5,), -777, dtype=torch.long, device=DEV)
+    lib.call("b200_inner_input_rows_fwd", hid.data_ptr(), y.data_ptr(), sel.data_ptr(), table.data_ptr(), out.data_ptr(),
+             y_sel.data_ptr(), n, n_rows, T, H, V, lib.stream())
+    live = (sel >= 0) & (sel < n_rows)
+    r = sel.long().clamp(0, n_rows - 1)
+    yr = y[r]
+    ref = torch.cat([hid[r][:, None], table[torch.where((yr[:, :-1] >= 0) & (yr[:, :-1] < V), yr[:, :-1], 0)]], 1)
+    ref = torch.where(live[:, None, None], ref, torch.zeros_like(ref)).reshape(n * T, H)
+    ysel_ref = torch.where(live[:, None], yr, torch.full_like(yr, -1)).reshape(-1)
+    W.add("", "rows fwd", {"rows_mismatch": _ne(out[:n * T], ref),
+                           "rows_ysel_mismatch": _ne(y_sel[:n * T], ysel_ref) + _ne(y_sel[n * T:], -777)})
+    W.add("", "rows fwd", P.sentinel_report(out, (slice(0, n * T),)))
+    # backward for hidden: only rows e * Tin of dx are read (the rest NaN)
+    Tin = T
+    dx = P.nan_buffer((n * Tin + 3, H), device=DEV)
+    dx[0:n * Tin:Tin] = randn(n, H, seed=6023)
+    inv = torch.full((n_rows,), -1, dtype=torch.int32, device=DEV)
+    inv[sel[live].long()] = torch.arange(n, device=DEV, dtype=torch.int32)[live]
+    dh = P.nan_buffer((n_rows + 2, H), device=DEV)
+    lib.call("b200_inner_input_rows_bwd_hidden", dx.data_ptr(), inv.data_ptr(), dh.data_ptr(), n_rows, n, Tin, H,
+             lib.stream())
+    ref = torch.where((inv >= 0)[:, None], dx[inv.long().clamp(0) * Tin], torch.zeros(n_rows, H, dtype=BF, device=DEV))
+    W.add("", "rows bwd", {"rows_bwd_mismatch": _ne(dh[:n_rows], ref)})
+    W.add("", "rows bwd", P.sentinel_report(dh, (slice(0, n_rows),)))
+    # ---- embedding backward
+    n_cases = capped = multi = 0
+    hot = {40: 123, 500: 2001, 5000: 3}             # occurrences -> id
+    for V in (3406, 5000):
+        for layout in ("outer", "inner"):
+            per_row, row_stride, row_inner, row_off = (8, 1, 0, 0) if layout == "outer" else (7, 8, 1, 1)
+            n_ev = 1000 if layout == "outer" else 1100
+            n = n_ev * per_row
+            g = _gen(6100 + V + per_row)
+            ids = torch.randint(0, V, (n,), generator=g, device=DEV)
+            pos = torch.randperm(n, generator=g, device=DEV)
+            k = 0
+            for occ, vid in hot.items():
+                ids[pos[k:k + occ]] = vid
+                k += occ
+            ids[pos[k:k + 30]] = torch.tensor([-1, V], device=DEV).repeat(15)
+            n_dout = n_ev * row_stride if layout == "inner" else n_ev
+            dvals = randn(n_dout, H, seed=6200 + V + per_row)
+            if layout == "outer":                        # gradient rows whose ids are all skipped are never read
+                for rr in (4, n_ev - 1):
+                    ids[rr * 8:rr * 8 + 8] = torch.tensor([-1, V] * 4, device=DEV)
+                    dvals[rr] = float("nan")
+            else:                                        # rows e*8 (the hidden position) are never read
+                dvals[0::8] = float("nan")
+            dout = P.poisoned(dvals, n_dout + 3, H)
+            for pad_id in (0, 17):
+                ids_p = ids.clone()
+                ids_p[pos[k + 30:k + 60]] = pad_id
+                ref = P.embed_bwd64(ids_p, dout, V, per_row, row_stride, row_inner, row_off, pad_id)
+                nbytes = int(lib.query("b200_embed_bwd_workspace_bytes", n, V, H))
+                for acc in (0, 1):
+                    ws = torch.full((nbytes,), 255, dtype=torch.uint8, device=DEV)     # NaN floats, -1 ints
+                    dt = P.nan_buffer((V + 2, H), device=DEV)
+                    old = randn(V, H, seed=6300 + V + pad_id) if acc else None
+                    if acc:
+                        dt[:V] = old
+                    lib.call("b200_embed_bwd", ids_p.data_ptr(), n, dout.data_ptr(), dt.data_ptr(), V, H, per_row,
+                             row_stride, row_inner, row_off, pad_id, acc, ws.data_ptr(), nbytes, lib.stream())
+                    case = f"V{V} {layout} pad{pad_id} acc{acc}"
+                    if acc:
+                        base = P.round_bf16(ref)
+                        W.add("bwdacc", case, P.exact_metrics(dt[:V], base + old.double(),
+                                                              (base + old.double()).to(torch.float32).to(BF), inter=ref))
+                        W.add("", case, {"bwd_padrow_changed": _ne(dt[pad_id], old[pad_id])})
+                    else:
+                        W.add("bwd", case, P.exact_metrics(dt[:V], ref))
+                        W.add("", case, {"bwd_padrow_changed": float((dt[pad_id] != 0).sum())})
+                    W.add("", case, P.sentinel_report(dt, (slice(0, V),)))
+                    n_cases += 1
+            cnt = torch.bincount(ids[(ids >= 0) & (ids < V)], minlength=V)
+            capped += int((cnt > 32 * 48).sum())
+            multi += int((cnt > 48).sum())
+    # n_ids = 0: zeros, or the old table when accumulating
+    V = 3406
+    nbytes = int(lib.query("b200_embed_bwd_workspace_bytes", 0, V, H))
+    for acc in (0, 1):
+        ws = torch.full((nbytes,), 255, dtype=torch.uint8, device=DEV)
+        dt = P.nan_buffer((V + 2, H), device=DEV)
+        old = randn(V, H, seed=6400)
+        if acc:
+            dt[:V] = old
+        lib.call("b200_embed_bwd", None, 0, None, dt.data_ptr(), V, H, 8, 1, 0, 0, 0, acc, ws.data_ptr(), nbytes,
+                 lib.stream())
+        W.add("", f"empty acc{acc}", {"bwd_empty_mismatch": _ne(dt[:V], old if acc else torch.zeros_like(old))})
+        W.add("", f"empty acc{acc}", P.sentinel_report(dt, (slice(0, V),)))
+    out = W.report()
+    out["em_bwd_cases"], out["em_bwd_capped_ids"], out["em_bwd_multislice_ids"] = float(n_cases), float(capped), float(multi)
+    return out
+
+
+RN_WARP_HS = (256, 512, 1024, 2048)     # forward warp kernels (add_rmsnorm's sizes); the backward's are 256 / 512 / 1024
+RN_BLOCK_HS = (200, 768, 1032, 4096)
+
+
+# forward: one fp32 rstd, two roundings (bf16(x rstd), then w * that); add_rmsnorm's h_out = bf16(x + res) is exact.
+# backward: dx one rounding, dw an fp32 column sum in an order the atomics choose, one rounding (two when accumulating).
+# The workspace is shared by every call, as ops.rmsnorm_bwd shares it, and must be all zero after each.  H100 80GB HBM3
+# at 700 W: rstd 1.6e-7 relative; y not correctly rounded 8.6e-6 (warp) / 6.3e-6 (block) / 7.1e-6 (add), <= 2 ulp, and
+# err_over_tol 1.30: a flipped inner rounding (<= 2^-7 relative) plus the final half ulp can reach 1.5, the bound.  dx
+# 1.6e-4, 1 ulp, 0.48; dw one element of 512 (2.0e-3), 1 ulp, 0.47.  Bounds about 5x.  Before the block path cleared its
+# partials, the alternating sequence left dw unwritten (wsseq_dw_frac 1, nan_in_range 1024) and M = 0 left dw unwritten
+@bounded([
+    ("rn_sentinels_changed", 0.0), ("rn_nan_in_range", 0.0), ("rn_add_h_mismatch", 0.0), ("rn_ws_nonzero_after", 0.0),
+    ("rn_m0_dw_mismatch", 0.0),
+    ("min:rn_fwd_cases", 36.0), ("min:rn_bwd_cases", 150.0), ("min:rn_bwd_block_cases", 92.0),
+    ("rn_rstd_rel", 8e-7),
+    *[(f"rn_{f}_frac", 5e-5) for f in ("fwd_warp", "fwd_block", "add")],
+    ("rn_dx_frac", 8e-4), *[(f"rn_{f}_frac", 1e-2) for f in ("dw", "dwacc", "wsseq_dw")],
+    *[(f"rn_{f}_maxulp", 1.0) for f in ("dx", "dw", "wsseq_dw")],
+    *[(f"rn_{f}_maxulp", 2.0) for f in ("fwd_warp", "fwd_block", "add", "dwacc")],
+    *[(f"rn_{f}_err_over_tol", 1.5) for f in ("fwd_warp", "fwd_block", "add")],
+    *[(f"rn_{f}_err_over_tol", 1.0) for f in ("dx", "dw", "dwacc", "wsseq_dw")],
+])
+def check_rmsnorm_conformance():
+    """b200_rmsnorm_fwd at H in {256, 512, 1024, 2048} (warp kernels) and {200, 768, 1032, 4096} (block kernel),
+    M in {1, 3, 5000} (5000 rows is past the grid cap: rows loop), b200_add_rmsnorm_fwd at its four sizes, and
+    b200_rmsnorm_bwd at every H with dres null / set, dw null / set, accumulate_dw 0 / 1 and M = 0, all on ONE
+    workspace; plus an H order that alternates the block and warp backward paths (1024, 768, 1024, 2048, 256, 1024)
+    with dw in a NaN buffer, so a warp call that starts from a dirty accumulator or ticket leaves dw unwritten."""
+    W = _Worst("rn_")
+    eps = 1e-6
+    parts = int(lib.query("b200_rmsnorm_bwd_parts"))
+    ws = torch.zeros(parts * max(RN_BLOCK_HS) + 64, dtype=torch.float32, device=DEV)
+    n_fwd = n_bwd = n_block = 0
+
+    def weight(H, seed):
+        w = P.nan_buffer((H + 8,), device=DEV)
+        w[:H] = (1 + 0.1 * randn(H, seed=seed).float()).to(BF)
+        return w
+
+    def fwd(x, w, M, H, res=None):
+        X = P.poisoned(x, M + 2, H)
+        y = P.nan_buffer((M + 2, H), device=DEV)
+        rstd = torch.full((M + 4,), float("nan"), device=DEV)
+        if res is None:
+            lib.call("b200_rmsnorm_fwd", X.data_ptr(), w.data_ptr(), y.data_ptr(), rstd.data_ptr(), M, H, eps, lib.stream())
+            return y, rstd, None
+        R = P.poisoned(res, M + 2, H)
+        h = P.nan_buffer((M + 2, H), device=DEV)
+        lib.call("b200_add_rmsnorm_fwd", X.data_ptr(), R.data_ptr(), w.data_ptr(), h.data_ptr(), y.data_ptr(),
+                 rstd.data_ptr(), M, H, eps, lib.stream())
+        return y, rstd, h
+
+    def score_fwd(fam, case, y, rstd, x, w, M, H):
+        x64 = x.double()
+        r64 = 1.0 / torch.sqrt(x64.pow(2).mean(-1) + eps)
+        W.add(fam, case, P.exact_metrics(y[:M], w[:H].double() * P.round_bf16(x64 * r64[:, None])))
+        W.add("", case, {"rstd_rel": float(((rstd[:M].double() - r64) / r64).abs().max())})
+        W.add("", case, P.sentinel_report(y, (slice(0, M),)))
+        W.add("", case, P.sentinel_report(rstd, (slice(0, M),)))
+
+    def bwd(case, dy, x, w, rstd, dres, dw, M, H, acc, fam_dw="dw"):
+        nonlocal n_bwd, n_block
+        DY, X = P.poisoned(dy, M + 2, H), P.poisoned(x, M + 2, H)
+        DR = P.poisoned(dres, M + 2, H) if dres is not None else None
+        dx = P.nan_buffer((M + 2, H), device=DEV)
+        old = dw[:H].clone() if dw is not None else None
+        lib.call("b200_rmsnorm_bwd", DY.data_ptr(), X.data_ptr(), w.data_ptr(), rstd.data_ptr(), lib.ptr(DR), dx.data_ptr(),
+                 lib.ptr(dw), M, H, acc, ws.data_ptr(), ws.numel() * 4, lib.stream())
+        dx64, dw64 = P.rmsnorm_bwd64(dy, x, w[:H], rstd[:M], dres)
+        W.add("dx", case, P.exact_metrics(dx[:M], dx64))
+        W.add("", case, P.sentinel_report(dx, (slice(0, M),)))
+        if dw is not None:
+            if acc:
+                base = P.round_bf16(dw64)
+                W.add(fam_dw + "acc", case, P.exact_metrics(dw[:H], base + old.double(),
+                                                            (base + old.double()).to(torch.float32).to(BF), inter=dw64))
+            else:
+                W.add(fam_dw, case, P.exact_metrics(dw[:H], dw64))
+            W.add("", case, P.sentinel_report(dw, (slice(0, H),)))
+        W.add("", case, {"ws_nonzero_after": float((ws.view(torch.int32) != 0).sum())})
+        n_bwd += 1
+        n_block += H not in (256, 512, 1024)
+
+    for hi, H in enumerate(RN_WARP_HS + RN_BLOCK_HS):
+        w = weight(H, 7000 + H)
+        fam = "fwd_warp" if H in RN_WARP_HS else "fwd_block"
+        for M in (1, 3, 5000):
+            x = randn(M, H, scale=3.0 if M == 3 else 1.0, seed=7100 + H + M)
+            y, rstd, _ = fwd(x, w, M, H)
+            score_fwd(fam, f"fwd H{H} M{M}", y, rstd, x, w, M, H)
+            n_fwd += 1
+            if H in RN_WARP_HS:
+                res = randn(M, H, seed=7200 + H + M)
+                ya, rstda, h = fwd(x, w, M, H, res)
+                href = (x.float() + res.float()).to(BF)
+                case = f"add H{H} M{M}"
+                W.add("", case, {"add_h_mismatch": _ne(h[:M], href)})
+                W.add("", case, P.sentinel_report(h, (slice(0, M),)))
+                score_fwd("add", case, ya, rstda, href, w, M, H)
+                n_fwd += 1
+            # backward from the forward kernel's rstd: every dres / dw / accumulate combination
+            dy = randn(M, H, seed=7300 + H + M)
+            dres = randn(M, H, seed=7400 + H + M)
+            for use_res in (0, 1):
+                for mode in ("none", "acc0", "acc1"):
+                    dw = None
+                    if mode != "none":
+                        dw = P.nan_buffer((H + 8,), device=DEV)
+                        if mode == "acc1":
+                            dw[:H] = randn(H, seed=7500 + H)
+                    bwd(f"bwd H{H} M{M} dres{use_res} dw_{mode}", dy, x, w, rstd, dres if use_res else None, dw, M, H,
+                        int(mode == "acc1"))
+    # M = 0: dw = 0 (accumulate 0) or unchanged (accumulate 1); nothing else written
+    for H in (1024, 768):
+        w = weight(H, 7600 + H)
+        for acc in (0, 1):
+            old = randn(H, seed=7700 + H)
+            dw = P.nan_buffer((H + 8,), device=DEV)
+            dw[:H] = old
+            e = torch.empty(0, dtype=BF, device=DEV)
+            lib.call("b200_rmsnorm_bwd", e.data_ptr(), e.data_ptr(), w.data_ptr(), None, None, e.data_ptr(), dw.data_ptr(),
+                     0, H, acc, ws.data_ptr(), ws.numel() * 4, lib.stream())
+            case = f"M0 H{H} acc{acc}"
+            W.add("", case, {"m0_dw_mismatch": _ne(dw[:H], old if acc else torch.zeros_like(old))})
+            W.add("", case, P.sentinel_report(dw, (slice(0, H),)))
+    # block and warp paths alternating on the one workspace
+    for i, H in enumerate((1024, 768, 1024, 2048, 256, 1024)):
+        M = 300
+        w = weight(H, 7800 + i)
+        x = randn(M, H, seed=7900 + i)
+        _, rstd, _ = fwd(x, w, M, H)
+        dw = P.nan_buffer((H + 8,), device=DEV)
+        bwd(f"ws-seq #{i} H{H}", randn(M, H, seed=8000 + i), x, w, rstd, None, dw, M, H, 0, fam_dw="wsseq_dw")
+    out = W.report()
+    out["rn_fwd_cases"], out["rn_bwd_cases"], out["rn_bwd_block_cases"] = float(n_fwd), float(n_bwd), float(n_block)
+    return out
+
+
+RO_NPOS = 4096 + 64
+
+
+# forward and backward are exact claims: bf16 x bf16 products are exact in fp32, so each sum rounds once to fp32 and
+# then to bf16, as P.round_bf16 rounds the fp64 value (the forward at each of its three rounding points).  H100 80GB HBM3
+# at 700 W: 0 mismatches both ways.  Tables (cosf / sinf of the kernel's fp32 argument, one rounding): 7.5e-6 not
+# correctly rounded, 1 ulp, err_over_tol 0.42; bound about 5x
+@bounded([
+    ("ro_sentinels_changed", 0.0), ("ro_nan_in_range", 0.0), ("ro_fwd_mismatch", 0.0), ("ro_ragged_mismatch", 0.0),
+    ("ro_v_changed", 0.0), ("min:ro_cases", 20.0),
+    ("ro_table_frac", 4e-5), ("ro_table_maxulp", 1.0), ("ro_bwd_frac", 0.0), ("ro_bwd_maxulp", 0.0),
+    ("ro_table_err_over_tol", 1.0), ("ro_bwd_err_over_tol", 1.0),
+])
+def check_rope_conformance():
+    """b200_rope_table (4096 + 64 positions from pos0 = 0, pos0 > 0 and pos0_dev) against cos / sin in fp64 of the kernel's fp32
+    argument; b200_rope_qk forward (0 mismatches against the three-rounding fp64 chain) and backward (the fp64 transpose
+    rounded once: also exact) at head_dim 64 / 256 on rows of ld > 3H with NaN pad columns, with pos0 and pos0_dev; and
+    b200_rope_qk_ragged with mixed row_off.  The v third and the pad columns are never written."""
+    W = _Worst("ro_")
+    n_cases = 0
+    for D in (64, 256):
+        half, nh = D // 2, 1024 // D
+        H = nh * D
+        inv = O.default_inv_freq(D).to(BF).to(DEV).float()
+        for pos0, dev in ((0, None), (1000, None), (7, 4000)):
+            n_pos = RO_NPOS
+            c = P.nan_buffer((n_pos + 2, half), device=DEV)
+            s = P.nan_buffer((n_pos + 2, half), device=DEV)
+            pd = torch.tensor([dev], dtype=torch.int32, device=DEV) if dev is not None else None
+            lib.call("b200_rope_table", inv.data_ptr(), half, n_pos, pos0, lib.ptr(pd), c.data_ptr(), s.data_ptr(),
+                     lib.stream())
+            base = pos0 if dev is None else dev                          # *pos0_dev replaces pos0
+            arg = (torch.arange(n_pos, device=DEV) + base).float()[:, None] * inv[None]   # the kernel's fp32 argument
+            case = f"table D{D} pos0 {pos0} dev {dev}"
+            W.add("table", case, P.exact_metrics(c[:n_pos], torch.cos(arg.double())))
+            W.add("table", case, P.exact_metrics(s[:n_pos], torch.sin(arg.double())))
+            W.add("", case, P.sentinel_report(c, (slice(0, n_pos),)))
+            W.add("", case, P.sentinel_report(s, (slice(0, n_pos),)))
+            n_cases += 1
+        cos, sin = ops.rope_table(O.default_inv_freq(D).to(BF).to(DEV), RO_NPOS)
+        S, ld = 37, 3 * H + 24
+        rows = 3 * S
+
+        def run(vals, pos, call):
+            buf = P.poisoned(vals, vals.shape[0] + 2, ld)
+            call(buf)
+            R = vals.shape[0]
+            qk = buf[:R, :2 * H].view(R, 2, nh, D)
+            W.add("", case, {"v_changed": _ne(buf[:R, 2 * H:3 * H], vals[:, 2 * H:])})
+            W.add("", case, P.sentinel_report(buf, (slice(0, R), slice(0, 3 * H))))
+            return qk, vals[:, :2 * H].view(R, 2, nh, D), pos.view(R, 1, 1)
+
+        for pos0, dev in ((0, None), (RO_NPOS - S, None), (17, RO_NPOS - S - 40)):
+            pd = torch.tensor([dev], dtype=torch.int32, device=DEV) if dev is not None else None
+            pos = pos0 + (dev or 0) + torch.arange(rows, device=DEV) % S
+            case = f"qk D{D} pos0 {pos0} dev {dev}"
+            for bwd in (0, 1):
+                vals = randn(rows, 3 * H, seed=8100 + D + pos0 + bwd)
+                qk, x, p = run(vals, pos, lambda b: lib.call(
+                    "b200_rope_qk", b.data_ptr(), cos.data_ptr(), sin.data_ptr(), rows, S, H, D, ld, bwd, pos0,
+                    lib.ptr(pd), lib.stream()))
+                if bwd:
+                    W.add("bwd", case, P.exact_metrics(qk, P.rope_bwd64(x, cos, sin, p)))
+                else:
+                    W.add("", case, {"fwd_mismatch": _ne(qk, _rope_chain64(x, cos, sin, p)[0].to(torch.float32).to(BF))})
+                n_cases += 1
+        # ragged: sequence b at pos0 + *pos0_dev + row_off[b]
+        Sg, row_off = 5, torch.tensor([0, -3, -100, 0, -4000, -1, -4090], dtype=torch.int32, device=DEV)
+        R = Sg * row_off.numel()
+        pos0, dev = 4000, 90
+        pd = torch.tensor([dev], dtype=torch.int32, device=DEV)
+        pos = pos0 + dev + row_off.long().repeat_interleave(Sg) + torch.arange(R, device=DEV) % Sg
+        case = f"ragged D{D}"
+        vals = randn(R, 3 * H, seed=8200 + D)
+        qk, x, p = run(vals, pos, lambda b: lib.call(
+            "b200_rope_qk_ragged", b.data_ptr(), cos.data_ptr(), sin.data_ptr(), R, Sg, H, D, ld, pos0, pd.data_ptr(),
+            row_off.data_ptr(), lib.stream()))
+        W.add("", case, {"ragged_mismatch": _ne(qk, _rope_chain64(x, cos, sin, p)[0].to(torch.float32).to(BF))})
+        n_cases += 1
+    out = W.report()
+    out["ro_cases"] = float(n_cases)
+    return out
+
+
+# forward: bf16(bf16(silu(g)) u) with the SFU sigmoid (relative error ~2^-22): two roundings; backward one.  scale_bf16
+# is one fp32 product and one rounding, restated exactly.  H100 80GB HBM3 at 700 W: forward correctly rounded in every
+# element of 9.1M (the bound leaves room for a flipped inner rounding: 1e-4, 2 ulp); backward 3.2e-5 not correctly
+# rounded, 1 ulp (bound about 5x); err_over_tol <= 0.49
+@bounded([
+    ("sw_sentinels_changed", 0.0), ("sw_nan_in_range", 0.0), ("sw_scale_mismatch", 0.0),
+    ("min:sw_grid_sweeps", 2.0), ("min:sw_scale_tails", 7.0),
+    ("sw_fwd_frac", 1e-4), ("sw_fwd_maxulp", 2.0), ("sw_bwd_frac", 2e-4), ("sw_bwd_maxulp", 1.0),
+    ("sw_fwd_err_over_tol", 1.0), ("sw_bwd_err_over_tol", 1.0),
+])
+def check_swiglu_conformance():
+    """b200_swiglu_fwd / _bwd at I in {8, 1024, 4096}, row counts that are not a multiple of the grid (and exceed one
+    grid-stride sweep), gates out to +-20 where the sigmoid saturates; b200_scale_bf16 with every n % 8 (the scalar
+    tail) and n past one grid-stride sweep."""
+    W = _Worst("sw_")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    sweep = sms * 16 * 256                         # 16-byte vectors per grid-stride sweep (grid_for's cap)
+    sweeps = 0
+    for I, rows in ((8, sweep + 4099), (1024, 777), (4096, 1501)):
+        g = randn(rows, I, scale=6.0, seed=8300 + I).float().clamp(-20, 20)
+        g[0, :4] = torch.tensor([20.0, -20.0, 19.5, -19.5])
+        g = g.to(BF)
+        u = randn(rows, I, seed=8301 + I)
+        gu = torch.cat([g, u], 1)
+        GU = P.poisoned(gu, rows + 3, 2 * I)
+        act = P.nan_buffer((rows + 2, I), device=DEV)
+        lib.call("b200_swiglu_fwd", GU.data_ptr(), act.data_ptr(), rows, I, lib.stream())
+        g64, u64 = g.double(), u.double()
+        case = f"I{I} rows{rows}"
+        W.add("fwd", case, P.exact_metrics(act[:rows], P.round_bf16(g64 * torch.sigmoid(g64)) * u64))
+        W.add("", case, P.sentinel_report(act, (slice(0, rows),)))
+        dact = randn(rows, I, seed=8302 + I)
+        DA = P.poisoned(dact, rows + 3, I)
+        dgu = P.nan_buffer((rows + 2, 2 * I), device=DEV)
+        lib.call("b200_swiglu_bwd", GU.data_ptr(), DA.data_ptr(), dgu.data_ptr(), rows, I, lib.stream())
+        W.add("bwd", case, P.exact_metrics(dgu[:rows], P.swiglu_bwd64(gu, dact)))
+        W.add("", case, P.sentinel_report(dgu, (slice(0, rows),)))
+        sweeps = max(sweeps, math.ceil(rows * I // 8 / sweep))
+    tails = set()
+    for n in (*range(1, 9), 8 * 1000 + 3, 8 * sweep + 8 * 1000 + 5):
+        x = P.nan_buffer((n + 16,), device=DEV)
+        x[:n] = randn(n, seed=8400 + n)
+        y = P.nan_buffer((n + 16,), device=DEV)
+        lib.call("b200_scale_bf16", x.data_ptr(), y.data_ptr(), n, 0.37, lib.stream())
+        case = f"scale n{n}"
+        W.add("", case, {"scale_mismatch": _ne(y[:n], (x[:n].float() * 0.37).to(BF))})
+        W.add("", case, P.sentinel_report(y, (slice(0, n),)))
+        tails.add(n % 8)
+    out = W.report()
+    out["sw_grid_sweeps"], out["sw_scale_tails"] = float(sweeps), float(len(tails - {0}))
+    return out
+
+
+# H100 80GB HBM3 at 700 W: worst row 4.1e-3 (o), 4.2e-3 / 4.4e-3 / 4.5e-3 (dq / dk / dv), 4.1e-3 / 4.3e-3 with the RoPE
+# backward fused: the bf16 rounding of P dominates, as in attn_edges, whose row bound this shares.  The fused RoPE
+# forward writes the rotated q / k exactly (the stand-alone chain)
+AT_ROW = 1e-2
+
+
+@bounded([
+    ("at_sentinels_changed", 0.0), ("at_nan_in_range", 0.0), ("at_rope_qk_mismatch", 0.0), ("at_qkv_changed", 0.0),
+    ("min:at_lengths", 8.0), ("min:at_cases", 48.0),
+    *[(f"at_{n}_row", AT_ROW) for n in ("o", "dq", "dk", "dv", "rope_dq", "rope_dk")],
+])
+def check_attn_tiny_conformance():
+    """b200_attn_tiny_fwd / _bwd at every L = 1..8 (a template instantiation each), n_heads 1 / 4 / 5 (partial CTAs of
+    the warp grid), ld_qkv > 3H and ld_out > H with NaN padding, with and without the fused RoPE (forward rotates q and
+    k in place: checked exactly; backward returns the gradient of the pre-RoPE projections), scored per (event, head,
+    row) against fp64 attention with scale 1/16.  The backward recomputes P in fp32 and forms delta = sum_j P dP from
+    it, i.e. from the exact o, so the reference's delta uses the exact o too."""
+    W = _Worst("at_")
+    D, scale = 256, 1.0 / 16
+    cos, sin = ops.rope_table(O.default_inv_freq(D).to(BF).to(DEV), 8)
+    lengths, n_cases = set(), 0
+    for L in range(1, 9):
+        for nh, N in ((1, 13), (4, 9), (5, 7)):
+            for rope in (False, True):
+                H = nh * D
+                ldq, ldo = 3 * H + 40, H + 24
+                R = N * L
+                case = f"L{L} h{nh} N{N}" + (" rope" if rope else "")
+                seed = 8500 + 10 * L + nh + 100 * rope
+                vals = randn(R, 3 * H, seed=seed)
+                QKV = P.poisoned(vals, R + 2, ldq)
+                dov = randn(R, H, seed=seed + 1)
+                DO = P.poisoned(dov, R + 2, ldo)
+                ob = P.nan_buffer((R + 2, ldo), device=DEV)
+                rc, rs = (cos.data_ptr(), sin.data_ptr()) if rope else (None, None)
+                lib.call("b200_attn_tiny_fwd", QKV.data_ptr(), ob.data_ptr(), N, L, nh, D, ldq, ldo, scale, rc, rs,
+                         lib.stream())
+                post = QKV[:R, :3 * H]
+                if rope:
+                    x = vals[:, :2 * H].view(N, L, 2, nh, D)
+                    chain = _rope_chain64(x, cos, sin, torch.arange(L, device=DEV).view(1, L, 1, 1))[0]
+                    W.add("", case, {"rope_qk_mismatch": _ne(post[:, :2 * H].view(N, L, 2, nh, D),
+                                                             chain.to(torch.float32).to(BF)),
+                                     "qkv_changed": _ne(post[:, 2 * H:], vals[:, 2 * H:])})
+                else:
+                    W.add("", case, {"qkv_changed": _ne(post, vals)})
+                W.add("", case, P.sentinel_report(QKV, (slice(0, R), slice(0, 3 * H))))
+                q, k, v = post.reshape(N, L, 3, nh, D).permute(2, 0, 3, 1, 4)
+                do = dov.view(N, L, nh, D).transpose(1, 2)
+                o64, _, dq64, dk64, dv64 = P.attn_ref64(q, k, v, do, 0, scale)
+                atol = 1e-3 * float(do.double().norm(dim=-1).median())
+                o = ob[:R, :H].view(N, L, nh, D).transpose(1, 2)
+                W.add("", case, {"o_row": P.row_worst(o, o64, atol=atol)})
+                W.add("", case, P.sentinel_report(ob, (slice(0, R), slice(0, H))))
+                dq = P.nan_buffer((R + 2, ldq), device=DEV)
+                lib.call("b200_attn_tiny_bwd", QKV.data_ptr(), DO.data_ptr(), dq.data_ptr(), N, L, nh, D, ldq, ldo, scale,
+                         rc, rs, lib.stream())
+                g = dq[:R, :3 * H].reshape(N, L, 3, nh, D).permute(2, 0, 3, 1, 4)
+                pos = torch.arange(L, device=DEV)
+                if rope:
+                    dq64, dk64 = P.rope_bwd64(dq64, cos, sin, pos), P.rope_bwd64(dk64, cos, sin, pos)
+                pre = "rope_" if rope else ""
+                W.add("", case, {f"{pre}dq_row": P.row_worst(g[0], dq64, atol=atol),
+                                 f"{pre}dk_row": P.row_worst(g[1], dk64, atol=atol),
+                                 "dv_row": P.row_worst(g[2], dv64, atol=atol)})
+                W.add("", case, P.sentinel_report(dq, (slice(0, R), slice(0, 3 * H))))
+                lengths.add(L)
+                n_cases += 1
+    out = W.report()
+    out["at_lengths"], out["at_cases"] = float(len(lengths)), float(n_cases)
+    return out
+
+
+LO_VOCABS = (1001, 2041, 3406, 4090, 5003)    # ce_fwd: warp kernels of 4 / 8 / 14 / 16 vectors per lane, CTA kernel
+LO_TV2O_MEDIUM_PARAMS = 233842688
+
+
+# lse / row loss: fp32 with __expf; the mean an fp32 sum; the count exact.  dlogits: one rounding.  Clip: fp32 sums of
+# squares.  AdamW: p one rounding of the fp32 update, m / v fp32.  H100 80GB HBM3 at 700 W: lse and row loss 4.0e-6
+# absolute, mean 1.2e-7 relative; dlogits 6.6e-5 not correctly rounded, 1 ulp, err_over_tol 0.49; norm 5.9e-7 and
+# coefficient 5.4e-7 relative (at 234M elements); p 1.6e-4, 1 ulp, 0.47; m / v 1.2e-7 / 1.9e-7 relative to the terms
+# they add.  Bounds about 5x
+@bounded([
+    ("lo_sentinels_changed", 0.0), ("lo_nan_in_range", 0.0), ("lo_padcols_nonzero", 0.0), ("lo_ce_count_abs", 0.0),
+    ("lo_ce_all_ignored_", 0.0), ("min:lo_ce_variants", 5.0), ("min:lo_adamw_steps", 4.0), ("min:lo_clip_cases", 12.0),
+    ("lo_ce_lse_abs", 2e-5), ("lo_ce_rowloss_abs", 2e-5), ("lo_ce_mean_rel", 6e-7),
+    ("lo_ce_bwd_frac", 3e-4), ("lo_ce_bwd_maxulp", 1.0), ("lo_ce_bwd_err_over_tol", 1.0),
+    ("lo_clip_norm_rel", 3e-6), ("lo_clip_coef_rel", 3e-6),
+    ("lo_adamw_p_frac", 8e-4), ("lo_adamw_p_maxulp", 1.0), ("lo_adamw_p_err_over_tol", 1.0),
+    ("lo_adamw_m_rel", 1e-6), ("lo_adamw_v_rel", 1e-6),
+])
+def check_loss_optim_conformance():
+    """b200_ce_fwd / _bwd at every row kernel (V in LO_VOCABS, none a multiple of 8) with NaN pad columns, targets that
+    are ignore_index / -1 / V, an all-ignored batch, logits out to +-60 and grad_scale_dev in fp32 and bf16;
+    b200_grad_clip_coef at n = 0, 5, 8k + 3 and the tv2o-medium parameter count, norm below and above max_norm and
+    max_norm = 0; b200_adamw_step element by element at steps 1, 2, 3 and 1000, with and without an active clip, with
+    lr wd large enough that decay moves p by several bf16 ulps and zero-gradient blocks on both sides of no-decay
+    boundaries."""
+    W = _Worst("lo_")
+    variants = set()
+    # ---- cross-entropy
+    for vi, V in enumerate(LO_VOCABS):
+        V8 = _rup8(V)
+        ld, R = V8 + 16, 9001 if V == 2041 else 1000
+        ign = 0 if vi % 2 else 17
+        z = randn(R, V, scale=3.0, seed=8700 + V).float()
+        z[1] = -60.0
+        z[1, 7] = 60.0                               # saturated row
+        z[2] = (z[2] * 20).clamp(-60, 60)
+        z = z.to(BF)
+        t = torch.randint(0, V, (R,), generator=_gen(8701 + V), device=DEV)
+        t[1], t[4], t[R - 1] = 7, V - 1, V - 2       # targets in the masked last vector
+        t[::7], t[3::11], t[5::13] = ign, -1, V
+        buf = P.poisoned(z, R + 2, ld)
+        lse = torch.full((R + 4,), float("nan"), device=DEV)
+        rl = torch.full((R + 4,), float("nan"), device=DEV)
+        lac = torch.full((4,), float("nan"), device=DEV)
+        lib.call("b200_ce_fwd", buf.data_ptr(), t.data_ptr(), lse.data_ptr(), rl.data_ptr(), lac.data_ptr(), R, V, ld, ign,
+                 lib.stream())
+        lse64, rl64, mean64, cnt64, d64 = P.ce64(z, t, V, ign)
+        case = f"V{V} R{R}"
+        W.add("ce", case, {"lse_abs": float((lse[:R].double() - lse64).abs().max()),
+                           "rowloss_abs": float((rl[:R].double() - rl64).abs().max()),
+                           "mean_rel": abs(float(lac[0]) - mean64) / abs(mean64), "count_abs": abs(float(lac[1]) - cnt64)})
+        for b_ in (lse, rl, lac):
+            W.add("", case, P.sentinel_report(b_, (slice(0, b_.numel() - (2 if b_ is lac else 4)),)))
+        vpl = (V8 // 8 + 31) // 32
+        variants.add(next((b for b in (4, 8, 14, 16) if vpl <= b), "cta"))
+        for gs, dev in ((1.0, None), (0.5, torch.tensor(3.0, device=DEV)), (2.0, torch.tensor(0.75, dtype=BF, device=DEV))):
+            b = buf.clone()
+            lib.call("b200_ce_bwd", b.data_ptr(), t.data_ptr(), lse.data_ptr(), lac.data_ptr(), R, V, ld, ign, gs,
+                     lib.ptr(dev), int(dev is not None and dev.dtype == BF), lib.stream())
+            scale = gs * (float(dev) if dev is not None else 1.0)
+            c = case + f" gscale {gs} x {None if dev is None else dev.dtype}"
+            W.add("ce_bwd", c, P.exact_metrics(b[:R, :V], d64 * scale))
+            W.add("", c, P.sentinel_report(b, (slice(0, R), slice(0, V)), (slice(0, R), slice(V, V8))))
+    # every target ignored: loss 0, count 0, zero gradient
+    V, R = 3406, 64
+    buf = P.poisoned(randn(R, V, scale=3.0, seed=8800), R, _rup8(V) + 16)
+    t = torch.full((R,), 0, dtype=torch.long, device=DEV)
+    t[::3] = -1
+    lse = torch.empty(R, device=DEV)
+    rl = torch.empty(R, device=DEV)
+    lac = torch.full((2,), float("nan"), device=DEV)
+    lib.call("b200_ce_fwd", buf.data_ptr(), t.data_ptr(), lse.data_ptr(), rl.data_ptr(), lac.data_ptr(), R, V,
+             buf.stride(0), 0, lib.stream())
+    lib.call("b200_ce_bwd", buf.data_ptr(), t.data_ptr(), lse.data_ptr(), lac.data_ptr(), R, V, buf.stride(0), 0, 1.0, None,
+             0, lib.stream())
+    W.add("", "all ignored", {"ce_all_ignored_loss": abs(float(lac[0])), "ce_all_ignored_count": abs(float(lac[1])),
+                              "ce_all_ignored_grad_nonzero": float((buf[:, :_rup8(V)] != 0).sum())})
+    # ---- grad-norm clip
+    parts = int(lib.query("b200_gradnorm_parts"))
+    ws = torch.full((parts + 8,), float("nan"), device=DEV)
+    n_clip = 0
+    for n in (0, 5, 8 * 1234 + 3, LO_TV2O_MEDIUM_PARAMS):
+        g = P.nan_buffer((n + 16,), device=DEV)
+        if n:
+            g[:n] = randn(n, scale=1e-3, seed=8900 + n % 1000)
+        norm64 = float(torch.linalg.vector_norm(g[:n], dtype=torch.float64)) if n else 0.0
+        for max_norm in (0.0, norm64 / 3, norm64 * 3 + 1.0):
+            nc = torch.full((4,), float("nan"), device=DEV)
+            lib.call("b200_grad_clip_coef", g.data_ptr(), n, max_norm, nc.data_ptr(), ws.data_ptr(), ws.numel() * 4,
+                     lib.stream())
+            coef64 = min(1.0, max_norm / (norm64 + 1e-6)) if max_norm > 0 else 1.0
+            case = f"clip n{n} max_norm {max_norm:.3g}"
+            W.add("clip", case, {"norm_rel": abs(float(nc[0]) - norm64) / max(norm64, 1e-30),
+                                 "coef_rel": abs(float(nc[1]) - coef64) / coef64})
+            W.add("", case, P.sentinel_report(nc, (slice(0, 2),)))
+            n_clip += 1
+        del g
+    # ---- AdamW
+    n = 256 * 9000                                 # past one grid-stride sweep of 8 x SMs CTAs x 256 threads x 8
+    blocks = torch.arange(n // 256, device=DEV)
+    nodecay = ((blocks // 3) % 2).to(torch.uint8)  # no-decay runs of 3 blocks
+    gz = (blocks % 5 == 1).repeat_interleave(256)   # zero-gradient blocks on both sides of the boundaries
+    g = torch.where(gz, 0.0, randn(n, scale=0.5, seed=9000).float()).to(BF)
+    nc = torch.zeros(2, device=DEV)
+    cws = torch.empty(parts, device=DEV)
+    lib.call("b200_grad_clip_coef", g.data_ptr(), n, 1.0, nc.data_ptr(), cws.data_ptr(), cws.numel() * 4, lib.stream())
+    steps_run = set()
+    b1, b2, eps = 0.9, 0.99, 1e-8
+
+    def f32(*a):                                   # the kernel's fp32 hyperparameters (1 - b2 is 1.2e-6 off 0.01)
+        return [float(np.float32(x)) for x in a]
+    for lr, wd, clip in ((1e-3, 0.01, False), (1e-2, 5.0, True)):
+        p = P.nan_buffer((n + 8,), device=DEV)
+        p[:n] = randn(n, scale=0.05, seed=9001)
+        m = torch.zeros(n, device=DEV)
+        v = torch.zeros(n, device=DEV)
+        coef = float(nc[1]) if clip else 1.0
+        for step in (1, 2, 3, 1000):
+            if step == 1000:                       # a late step from a moment state of that age
+                m = randn(n, scale=0.05, seed=9002).float()
+                v = randn(n, scale=0.05, seed=9003).float().pow(2)
+            p0, m0, v0 = p[:n].clone(), m.clone(), v.clone()
+            lib.call("b200_adamw_step", p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), nodecay.data_ptr(), n, lr,
+                     b1, b2, eps, wd, step, nc.data_ptr() if clip else None, lib.stream())
+            p64, m64, v64 = P.adamw64(p0, g, m0, v0, nodecay, *f32(lr, b1, b2, eps, wd), step, coef)
+            case = f"adamw lr {lr} wd {wd} clip {coef:.3g} step {step}"
+            W.add("adamw_p", case, P.exact_metrics(p[:n], p64))
+            # relative to the terms the fp32 update adds (the moments cancel where the gradient turns)
+            gc = g.double() * coef
+            m_scale = b1 * m0.double().abs() + (1 - b1) * gc.abs() + 1e-30
+            v_scale = b2 * v0.double() + (1 - b2) * gc * gc + 1e-30
+            W.add("adamw", case, {"m_rel": float(((m.double() - m64).abs() / m_scale).max()),
+                                  "v_rel": float(((v.double() - v64).abs() / v_scale).max())})
+            W.add("", case, P.sentinel_report(p, (slice(0, n),)))
+            steps_run.add(step)
+    out = W.report()
+    out["lo_ce_variants"], out["lo_adamw_steps"], out["lo_clip_cases"] = float(len(variants)), float(len(steps_run)), float(n_clip)
+    return out
+
+
 # in the order tests/test_gpu_parity.py runs them
 GROUPS = {
     "gemm_fwd": check_gemm_fwd, "gemm_swiglu": check_gemm_swiglu, "gemm_dgrad": check_gemm_dgrad, "gemm_wgrad": check_gemm_wgrad,
@@ -2393,4 +3058,7 @@ GROUPS = {
     "gemm_matrix": check_gemm_matrix, "gemm_epilogues": check_gemm_epilogues, "attn_edges": check_attn_edges,
     "gemv_matrix": check_gemv_conformance, "decode_attn_edges": check_decode_attn_conformance,
     "sampler_exact": check_sampler_conformance, "persist_vs_phase": check_persist_vs_phase,
+    "embed_exact": check_embed_conformance, "rmsnorm_exact": check_rmsnorm_conformance, "rope_exact": check_rope_conformance,
+    "swiglu_exact": check_swiglu_conformance, "attn_tiny_exact": check_attn_tiny_conformance,
+    "loss_optim_exact": check_loss_optim_conformance,
 }

@@ -167,7 +167,72 @@ def attn_ref64(q, k, v, do, off, scale=0.125, o_in=None):
 
 
 def rope_bwd64(g, cos, sin, pos):
-    """gradient w.r.t. the pre-rotation projection: the transpose of x' = x c + rotate_half(x) s, in fp64 at `pos`."""
+    """gradient w.r.t. the pre-rotation projection: the transpose of x' = x c + rotate_half(x) s, in fp64 at `pos`
+    (g (..., D), tables [positions, D/2])."""
+    half = g.shape[-1] // 2
     c, s = cos.double()[pos], sin.double()[pos]
-    g1, g2 = g[..., :32], g[..., 32:]
+    g1, g2 = g[..., :half].double(), g[..., half:].double()
     return torch.cat([g1 * c + g2 * s, g2 * c - g1 * s], -1)
+
+
+def rmsnorm_bwd64(dy, x, w, rstd=None, dres=None, eps=1e-6):
+    """RMSNorm y = w * x * rstd backward in fp64 over rows of (M, H): (dx, dw) with dx = [dres +] rstd (dn - n mean(dn n)),
+    dn = dy w, n = x rstd, and dw = sum over rows of dy n.  rstd: the per-row value the backward is handed (the forward
+    kernel's fp32 rstd); None = exact 1 / sqrt(mean(x^2) + eps), which makes this fp64 autograd."""
+    dy, x, w = dy.double(), x.double(), w.double()
+    r = 1.0 / torch.sqrt(x.pow(2).mean(-1, keepdim=True) + eps) if rstd is None else rstd.double().view(-1, 1)
+    n, dn = x * r, dy * w
+    dx = r * (dn - n * (dn * n).mean(-1, keepdim=True))
+    if dres is not None:
+        dx = dx + dres.double()
+    return dx, (dy * n).sum(0)
+
+
+def ce64(logits, targets, V, ignore_index, grad_scale=1.0):
+    """Mean cross-entropy over rows of logits[:, :V] in fp64, rows whose target is ignore_index or outside [0, V)
+    ignored: (lse [R], row_loss [R] (0 on ignored rows), mean loss, count, dlogits [R, V] = (softmax - onehot) *
+    grad_scale / max(count, 1) on live rows, 0 on ignored ones)."""
+    z = logits[:, :V].double()
+    t = targets.long()
+    live = (t != ignore_index) & (t >= 0) & (t < V)
+    lse = torch.logsumexp(z, -1)
+    tc = torch.where(live, t, torch.zeros_like(t))
+    row_loss = torch.where(live, lse - z.gather(1, tc[:, None])[:, 0], torch.zeros_like(lse))
+    count = int(live.sum())
+    mean = float(row_loss.sum()) / count if count else 0.0
+    d = torch.exp(z - lse[:, None])
+    d[torch.arange(len(t), device=z.device)[live], t[live]] -= 1.0
+    d = torch.where(live[:, None], d * (grad_scale / max(count, 1)), torch.zeros_like(d))
+    return lse, row_loss, mean, count, d
+
+
+def adamw64(p, g, m, v, nodecay, lr, b1, b2, eps, wd, step, coef=1.0):
+    """One torch.optim.AdamW step (decoupled decay, bias correction) in fp64 over a flat buffer, with the gradient
+    multiplied by the clip coefficient first and the decay skipped on the 256-element blocks nodecay marks: (p, m, v)
+    unrounded.  The kernel stores p in bf16 (one rounding) and m, v in fp32."""
+    p, g, m, v = p.double(), g.double() * float(coef), m.double(), v.double()
+    decay = torch.where(nodecay.bool().repeat_interleave(256), torch.ones_like(p), torch.full_like(p, 1.0 - lr * wd))
+    m = b1 * m + (1 - b1) * g
+    v = b2 * v + (1 - b2) * g * g
+    denom = v.sqrt() / math.sqrt(1 - b2 ** step) + eps
+    return p * decay - lr / (1 - b1 ** step) * (m / denom), m, v
+
+
+def embed_bwd64(ids, dout, V, per_row, row_stride, row_inner, row_off, pad_id):
+    """Embedding backward in fp64: row v of the [V, H] result sums the gradient rows of every id i == v, where id i (flat
+    index) reads row (i // per_row) * row_stride + (i % per_row) * row_inner + row_off of dout; ids outside [0, V) and
+    pad_id contribute nothing (the pad row is 0).  Rows no valid id reads are never touched, so they may hold NaN."""
+    ids = ids.reshape(-1).long()
+    i = torch.arange(ids.numel(), device=ids.device)
+    keep = (ids >= 0) & (ids < V) & (ids != pad_id)
+    rows = (i // per_row) * row_stride + (i % per_row) * row_inner + row_off
+    out = torch.zeros(V, dout.shape[1], dtype=torch.float64, device=dout.device)
+    return out.index_add_(0, ids[keep], dout[rows[keep]].double())
+
+
+def swiglu_bwd64(gu, dact):
+    """act = silu(g) u on packed [rows, 2I] = [g | u]: (dg | du) in fp64 = (dact u silu'(g) | dact silu(g))."""
+    I = gu.shape[1] // 2
+    g, u, d = gu[:, :I].double(), gu[:, I:].double(), dact.double()
+    sg = torch.sigmoid(g)
+    return torch.cat([d * u * sg * (1 + g * (1 - sg)), d * g * sg], 1)

@@ -211,3 +211,169 @@ def test_poisoned_operand_keeps_values_and_pads_with_nan():
     t = P.poisoned(v, 4, 8)
     assert torch.equal(t[:3, :5], v)
     assert bool(torch.isnan(t[:3, 5:].float()).all()) and bool(torch.isnan(t[3].float()).all())
+
+
+# ------------------------------------------------------------------------------------------ train-step references
+def _ex(prefix, family, y, ref, **kw):
+    return {f"{prefix}_{family}_{k}": v for k, v in P.exact_metrics(y, ref, **kw).items()}
+
+
+def test_rmsnorm_bwd64_is_fp64_autograd():
+    x, dy, dres = _randn(7, 40, seed=20), _randn(7, 40, seed=21), _randn(7, 40, seed=22)
+    w = 1 + 0.1 * _randn(40, seed=23)
+    xa, wa = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
+    (wa * xa * torch.rsqrt(xa.pow(2).mean(-1, keepdim=True) + 1e-6)).backward(dy)
+    dx, dw = P.rmsnorm_bwd64(dy, x, w, dres=dres)
+    assert torch.allclose(dx, xa.grad + dres, rtol=1e-12, atol=1e-12)
+    assert torch.allclose(dw, wa.grad, rtol=1e-12, atol=1e-12)
+    # the rstd the backward is handed replaces the exact one
+    r = torch.rsqrt(x.pow(2).mean(-1) + 1e-6)
+    assert torch.allclose(P.rmsnorm_bwd64(dy, x, w, r, dres)[0], dx, rtol=1e-12, atol=1e-12)
+
+
+def test_rmsnorm_dw_from_one_cta_partial_fails():
+    """dw is the column sum over every row; one CTA's partial (the rows of a grid-stride loop over 528 CTAs) fails."""
+    M, H = 5000, 768
+    dy, x = _randn(M, H, seed=24).to(BF), _randn(M, H, seed=25).to(BF)
+    w = (1 + 0.1 * _randn(H, seed=26)).to(BF)
+    dx64, dw64 = P.rmsnorm_bwd64(dy, x, w)
+    r = torch.rsqrt(x.float().pow(2).mean(-1, keepdim=True) + 1e-6)
+    contrib = dy.float() * (x.float() * r)
+    full = contrib.flip(0).sum(0).to(BF)                 # fp32 in another order, one rounding
+    assert not _fails("rmsnorm_exact", _ex("rn", "dw", full, dw64))
+    part = contrib[0::528].sum(0).to(BF)
+    assert _fails("rmsnorm_exact", _ex("rn", "dw", part, dw64))
+    assert not _fails("rmsnorm_exact", _ex("rn", "dx", dx64.float().to(BF), dx64))
+
+
+def test_ce64_is_fp64_cross_entropy():
+    V, ign = 37, 5
+    z = _randn(11, V, seed=30) * 3
+    t = torch.randint(0, V, (11,), generator=torch.Generator().manual_seed(31))
+    t[::4] = ign
+    za = z.clone().requires_grad_(True)
+    loss = torch.nn.functional.cross_entropy(za, t, ignore_index=ign)
+    (loss * 0.5).backward()
+    lse, row_loss, mean, count, d = P.ce64(z, t, V, ign, grad_scale=0.5)
+    assert count == int((t != ign).sum()) and abs(mean - float(loss.detach())) < 1e-12
+    assert torch.allclose(lse, torch.logsumexp(z, -1), rtol=1e-13)
+    assert torch.allclose(d, za.grad, rtol=1e-12, atol=1e-14)
+    # targets -1 and V count as ignored: zero loss and gradient on their rows
+    t2 = t.clone()
+    t2[1], t2[2] = -1, V
+    _, rl2, _, c2, d2 = P.ce64(z, t2, V, ign)
+    assert c2 == count - 2 + int(t[1] == ign) + int(t[2] == ign)
+    assert float(rl2[1:3].abs().max()) == 0 and float(d2[1:3].abs().max()) == 0
+
+
+def test_ce_zeroed_last_vector_fails():
+    V, R = 3406, 200
+    z = (_randn(R, V, seed=32) * 3).to(BF)
+    t = torch.randint(0, V, (R,), generator=torch.Generator().manual_seed(33))
+    d64 = P.ce64(z, t, V, 0)[4]
+    y = ((torch.exp(z.float() - torch.logsumexp(z.float(), -1, keepdim=True))
+          - torch.nn.functional.one_hot(t, V).float()) / R).to(BF)         # fp32, another evaluation order
+    assert not _fails("loss_optim_exact", _ex("lo", "ce_bwd", y, d64))
+    y[:, 3400:] = 0                                                          # the masked last vector, 3400..3405
+    assert _fails("loss_optim_exact", _ex("lo", "ce_bwd", y, d64))
+
+
+def test_adamw64_is_torch_adamw_in_fp64():
+    n = 4 * 256
+    p0, g = _randn(n, seed=40) * 0.05, _randn(n, seed=41) * 0.5
+    nodecay = torch.tensor([0, 0, 1, 1], dtype=torch.uint8)
+    pa, pb = torch.nn.Parameter(p0[:512].clone()), torch.nn.Parameter(p0[512:].clone())
+    opt = torch.optim.AdamW([dict(params=[pa], weight_decay=5.0), dict(params=[pb], weight_decay=0.0)], lr=1e-2,
+                            betas=(0.9, 0.99), eps=1e-8)
+    p, m, v = p0, torch.zeros(n, dtype=torch.float64), torch.zeros(n, dtype=torch.float64)
+    for step in (1, 2, 3):
+        pa.grad, pb.grad = g[:512] * 0.3, g[512:] * 0.3
+        opt.step()
+        p, m, v = P.adamw64(p, g, m, v, nodecay, 1e-2, 0.9, 0.99, 1e-8, 5.0, step, coef=0.3)
+        assert torch.allclose(p, torch.cat([pa, pb]).detach(), rtol=1e-12, atol=1e-15)
+        assert torch.allclose(m, torch.cat([opt.state[pa]["exp_avg"], opt.state[pb]["exp_avg"]]), rtol=1e-12)
+
+
+def test_adamw_decay_on_a_nodecay_block_fails():
+    n = 64 * 256
+    p0 = (_randn(n, seed=42) * 0.05).to(BF)
+    g = (_randn(n, seed=43) * 0.5).to(BF)
+    g[256:512] = 0                                        # decay alone moves this block
+    nodecay = torch.zeros(n // 256, dtype=torch.uint8)
+    nodecay[1::2] = 1
+    m, v = torch.zeros(n), torch.zeros(n)
+    args = (0.9, 0.99, 1e-8, 5.0, 1)
+    p64 = P.adamw64(p0, g, m, v, nodecay, 1e-2, *args)[0]
+    assert not _fails("loss_optim_exact", _ex("lo", "adamw_p", p64.float().to(BF), p64))
+    wrong = P.adamw64(p0, g, m, v, torch.zeros_like(nodecay), 1e-2, *args)[0]
+    assert _fails("loss_optim_exact", _ex("lo", "adamw_p", wrong.float().to(BF), p64))
+    inverted = P.adamw64(p0, g, m, v, 1 - nodecay, 1e-2, *args)[0]
+    assert _fails("loss_optim_exact", _ex("lo", "adamw_p", inverted.float().to(BF), p64))
+
+
+@pytest.mark.parametrize("layout", ["outer", "inner"])
+def test_embed_bwd64_is_fp64_embedding_backward(layout):
+    V, H, pad = 50, 16, 17
+    g = torch.Generator().manual_seed(50)
+    per_row = 8 if layout == "outer" else 7
+    ids = torch.randint(0, V, (30, per_row), generator=g)
+    ids[3, 2] = pad
+    table = _randn(V, H, seed=51).requires_grad_(True)
+    if layout == "outer":
+        dout = _randn(30, H, seed=52)
+        torch.nn.functional.embedding(ids, table, padding_idx=pad).sum(-2).backward(dout)
+        ref = P.embed_bwd64(ids, dout, V, 8, 1, 0, 0, pad)
+    else:
+        dout = _randn(30 * 8, H, seed=52)
+        torch.nn.functional.embedding(ids, table, padding_idx=pad).backward(dout.view(30, 8, H)[:, 1:])
+        dout[0::8] = float("nan")                           # rows e*8 are never read
+        ref = P.embed_bwd64(ids, dout, V, 7, 8, 1, 1, pad)
+    assert torch.allclose(ref, table.grad, rtol=1e-12, atol=1e-12)
+    # ids outside [0, V) contribute nothing
+    ids2 = ids.clone()
+    ids2[0, 0], ids2[1, 1] = -1, V
+    assert bool(torch.isfinite(P.embed_bwd64(ids2, dout, V, per_row, *((1, 0, 0) if layout == "outer" else (8, 1, 1)),
+                                             pad)).all())
+
+
+def test_swiglu_bwd64_is_fp64_autograd():
+    gu, d = _randn(9, 48, seed=60) * 6, _randn(9, 24, seed=61)
+    a = gu.clone().requires_grad_(True)
+    (torch.nn.functional.silu(a[:, :24]) * a[:, 24:]).backward(d)
+    assert torch.allclose(P.swiglu_bwd64(gu, d), a.grad, rtol=1e-12, atol=1e-14)
+
+
+def _rope_tables(D, S):
+    half = D // 2
+    ang = torch.arange(S, dtype=torch.float64)[:, None] * (10000.0 ** (-torch.arange(half, dtype=torch.float64) / half))
+    return ang.cos(), ang.sin()
+
+
+@pytest.mark.parametrize("D", [64, 256])
+def test_rope_bwd64_is_the_transpose_of_the_rotation(D):
+    S, half = 9, D // 2
+    cos, sin = _rope_tables(D, S)
+    x = _randn(2, 3, S, D, seed=70).requires_grad_(True)
+    gy = _randn(2, 3, S, D, seed=71)
+    c, s = torch.cat([cos, cos], -1), torch.cat([sin, sin], -1)
+    (x * c + torch.cat([-x[..., half:], x[..., :half]], -1) * s).backward(gy)
+    assert torch.allclose(P.rope_bwd64(gy, cos, sin, torch.arange(S)), x.grad, rtol=1e-12, atol=1e-12)
+
+
+def test_rope_swapped_pair_fails():
+    """The forward is an exact claim against the three-rounding chain; one rotated pair stored swapped fails, as it
+    does in the backward's per-element score."""
+    D, S, nh = 64, 37, 4
+    cos, sin = (t.to(BF) for t in _rope_tables(D, S))
+    x = _randn(S, nh, D, seed=72).to(BF)
+    pos = torch.arange(S).view(S, 1)
+    want = G._rope_chain64(x, cos, sin, pos)[0].float().to(BF)
+    bad = want.clone()
+    bad[5, 2, 3], bad[5, 2, 3 + D // 2] = want[5, 2, 3 + D // 2], want[5, 2, 3]
+    assert not _fails("rope_exact", {"ro_fwd_mismatch": G._ne(want, want)})
+    assert _fails("rope_exact", {"ro_fwd_mismatch": G._ne(bad, want)})
+    g64 = P.rope_bwd64(x, cos, sin, pos)
+    y = g64.float().to(BF)
+    assert not _fails("rope_exact", _ex("ro", "bwd", y, g64))
+    y[5, 2, 3], y[5, 2, 3 + D // 2] = g64[5, 2, 3 + D // 2].float().to(BF), g64[5, 2, 3].float().to(BF)
+    assert _fails("rope_exact", _ex("ro", "bwd", y, g64))
