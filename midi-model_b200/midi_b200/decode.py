@@ -50,6 +50,21 @@ class PagedKV:
         v.block_table = self.block_table[:1]              # row 0 of the identity table: pages 0 .. max_pages - 1
         return v
 
+    def table_row(self, b: int) -> "PagedKV":
+        """Row b of the block table as a batch-1 cache over the whole pools, empty: a prefill through it writes the pages
+        that row b's entries name, which need not be the row's own range (shared prompts, GraphGenerator.run_queue).
+        Never grown."""
+        v = PagedKV.__new__(PagedKV)
+        v.cfg, v.batch, v.page, v.max_pages, v.capacity, v.length = self.cfg, 1, self.page, self.max_pages, self.capacity, 0
+        v.k, v.v = list(self.k), list(self.v)
+        v.block_table = self.block_table[b:b + 1]
+        return v
+
+    def identity_table(self) -> None:
+        """Row b owns pages [b * max_pages, (b+1) * max_pages) again."""
+        n = self.batch * self.max_pages
+        self.block_table.copy_(torch.arange(n, dtype=torch.int32).view(self.batch, self.max_pages))
+
     def grow(self, capacity: int) -> None:
         """Re-allocate the pools for at least `capacity` positions, keeping the cached keys / values (row b owns pages
         [b * max_pages, (b+1) * max_pages), so the old pages are copied to the front of each row's new range).  The
@@ -70,6 +85,120 @@ class PagedKV:
                 pools[li] = new
         self.block_table = torch.arange(self.batch * self.max_pages, dtype=torch.int32, device=dev).view(
             self.batch, self.max_pages).contiguous()
+
+
+def _share_keys(prompts, page: int) -> list:
+    """Share key of each request of a queue call (prompts: int64 [L, T] tensors): the index of the first request with an
+    equal prompt, or None.  Only prompts of at least page + 1 events share, so that at least one whole page is prefilled;
+    a prompt that no other request repeats gets None.  A hash of the bytes only picks the candidates: equality is exact."""
+    keys = [None] * len(prompts)
+    by_shape = {}
+    for i, p in enumerate(prompts):
+        if p.shape[0] - 1 >= page:
+            by_shape.setdefault(tuple(p.shape), []).append(i)
+    for idx in by_shape.values():
+        if len(idx) < 2:
+            continue
+        host = {i: prompts[i].cpu().numpy() for i in idx}
+        firsts = {}                                  # hash of the bytes -> first requests with those bytes
+        for i in idx:
+            cands = firsts.setdefault(hash(host[i].tobytes()), [])
+            keys[i] = next((j for j in cands if np.array_equal(host[i], host[j])), None)
+            if keys[i] is None:
+                cands.append(i)
+                keys[i] = i
+    count = {}
+    for k in keys:
+        count[k] = count.get(k, 0) + 1
+    return [k if k is not None and count[k] > 1 else None for k in keys]
+
+
+class SharedPages:
+    """Page assignment of a queue call in which requests share prompts.  The outer cache keeps its batch * max_pages pages;
+    they are handed out from a host free list and each slot's block-table row is written when the slot takes a request.
+
+    A request of L prompt events with share key k reads positions below S = ((L - 1) // page) * page from k's shared
+    pages, which the first request of k prefills and the last live one of k gives back.  Every other entry of its row is a
+    private page; the one at S, the prompt's tail page, also holds prompt positions S .. L - 2 and is copied for each
+    later sharer.  A request has max_pages distinct pages at most and sharing only lowers the total, so the pool suffices.
+
+    An empty slot still appends on the graph and host-issued loops (at positions 0, 1, 2, ... of its row), so every entry
+    of its row names one private page of the last request it held; it keeps that page until the call ends.  A slot is
+    only left empty when no request waits, so no later admission can be handed that page."""
+
+    def __init__(self, kv: PagedKV):
+        self.kv = kv
+        self.n_pages = kv.batch * kv.max_pages
+        self.free = list(range(self.n_pages - 1, -1, -1))
+        self.groups = {}                          # share key -> (shared page ids, live slots)
+        self.rows = [None] * kv.batch             # page ids of slot b's block-table row, as written
+        self.held = [[] for _ in range(kv.batch)]  # private pages of slot b
+        self.key = [None] * kv.batch              # share key of slot b's live request
+        self.shared = [0] * kv.batch              # S of slot b's live request (0: nothing shared)
+
+    def _take(self, n: int) -> list:
+        if n > len(self.free):
+            raise lib.B200Error(f"KV page pool exhausted: {n} pages wanted, {len(self.free)} free")
+        return [self.free.pop() for _ in range(n)]
+
+    def _write(self, b: int, row: list) -> None:
+        self.rows[b] = row
+        self.kv.block_table[b].copy_(torch.tensor(row, dtype=torch.int32))
+
+    def release(self, b: int) -> None:
+        """Slot b's request finished: its share of the prompt's pages goes back (with the last live sharer)."""
+        k = self.key[b]
+        if k is not None:
+            pages, live = self.groups[k]
+            live.remove(b)
+            if not live:
+                self.free.extend(reversed(pages))
+                del self.groups[k]
+        self.key[b], self.shared[b] = None, 0
+
+    def admit(self, b: int, L: int, key) -> Optional[int]:
+        """Row b for a request of L prompt events and share key `key` (None: shares nothing).  Returns a live sharer's slot
+        whose tail page holds the prompt, or None when the request must be prefilled."""
+        self.free.extend(reversed(self.held[b]))
+        page, mp = self.kv.page, self.kv.max_pages
+        S = (L - 1) // page * page if key is not None else 0
+        group = self.groups.get(key) if key is not None else None
+        src = group[1][0] if group is not None else None
+        if key is not None and group is None:
+            group = self.groups[key] = (self._take(S // page), [])
+        self.held[b] = self._take(mp - S // page)
+        if group is not None:
+            group[1].append(b)
+        self.key[b], self.shared[b] = key, S
+        self._write(b, (group[0] if group is not None else []) + self.held[b])
+        return src
+
+    def copy_tail(self, src: int, b: int, L: int) -> None:
+        """Prompt positions S .. L - 2 of sharer `src`'s tail page into b's (nothing when L - 1 == S)."""
+        if L - 1 == self.shared[b]:
+            return
+        t = self.shared[b] // self.kv.page
+        s, d = self.rows[src][t], self.rows[b][t]
+        for pools in (self.kv.k, self.kv.v):
+            for pool in pools:
+                pool[d].copy_(pool[s])
+
+    def park(self, b: int) -> None:
+        """Slot b stays empty: every entry of its row names one private page of its last request (a free one if it never
+        held a request)."""
+        if not self.held[b]:
+            self.held[b] = self._take(1)
+        self.free.extend(reversed(self.held[b][1:]))
+        self.held[b] = self.held[b][:1]
+        self._write(b, self.held[b] * self.kv.max_pages)
+
+    def close(self) -> None:
+        """End of the call: every page back on the free list, and the identity table restored."""
+        for b in range(self.kv.batch):
+            self.release(b)
+            self.free.extend(reversed(self.held[b]))
+            self.held[b] = []
+        self.kv.identity_table()
 
 
 def _linear(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None,
@@ -615,11 +744,13 @@ class GraphGenerator:
         self.row_last.fill_(-2)
         self.counter.copy_(torch.tensor([0, self.seed], dtype=torch.int64))
 
-    def _admit(self, b: int, prompt: torch.Tensor, setting=None) -> None:
+    def _admit(self, b: int, prompt: torch.Tensor, setting=None, pages: Optional[SharedPages] = None, key=None) -> None:
         """Request `prompt` (int64 [L, T] on the device) into slot b: events 0 .. L-2 prefilled at batch 1 into the slot's
         pages (nothing for a one-event prompt), event L-1 fed to the next event.  Per-request mode: `setting` = (temp, top_p,
         top_k, seed, denied token ids) becomes slot b's settings, RNG key (row_first = L-1: its new event j is at seq index
-        L + j) and mask row."""
+        L + j) and mask row.  With `pages` (a call that shares prompts) slot b's row is written first and the prefill goes
+        through it; a request whose prompt a live request of the same share `key` already holds is not prefilled, it only
+        gets its own copy of the prompt's tail page."""
         L = prompt.shape[0]
         if setting is not None:
             temp, top_p, top_k, seed, deny = setting
@@ -630,8 +761,12 @@ class GraphGenerator:
                 self.mask[b, torch.tensor(sorted(deny), dtype=torch.long, device=self.mask.device)] = 0
         self.seq[b].fill_(self.tok.pad_id)
         self.seq[b, :L] = prompt
-        if L > 1:
-            self.outer.step(ops.embed_sum(prompt[:L - 1].contiguous(), self.outer.eng.embed), self.kv1.row(b), L - 1)
+        src = pages.admit(b, L, key) if pages is not None else None
+        if src is not None:
+            pages.copy_tail(src, b, L)
+        elif L > 1:
+            kv = self.kv1.row(b) if pages is None else self.kv1.table_row(b)
+            self.outer.step(ops.embed_sum(prompt[:L - 1].contiguous(), self.outer.eng.embed), kv, L - 1)
         self.ev_in[b] = prompt[L - 1]
 
     def run_queue(self, prompts, budgets, use_graph=True, settings=None) -> list:
@@ -649,7 +784,12 @@ class GraphGenerator:
         `settings` (per-request mode): one (temp, top_p, top_k, seed, denied token ids) per request, with temp > 0,
         0 < top_p <= 1, top_k >= 1 (checked by the caller).  Request i then samples with its own settings and mask row and
         draws what a batch-1 loop seeded `seed` draws, through the `_rows` entries; the persistent kernel needs every top_k
-        <= 64.  Without it, every slot shares this loop's settings, seed stream and mask."""
+        <= 64.  Without it, every slot shares this loop's settings, seed stream and mask.
+
+        Requests with equal prompts of at least 65 events (`_share_keys`) share the KV pages of the prompt's whole pages
+        (SharedPages): the first one resident is prefilled, a later one only copies the prompt's tail page from a live
+        sharer.  Every kernel addresses the cache through the block table, so no request's result changes by a bit.  A call
+        without such a pair keeps the identity block table and prefills every request into its slot's own pages."""
         self.rows = settings is not None
         self.req_top_k = [s[2] for s in settings] if self.rows else []
         if self.rows:
@@ -663,6 +803,9 @@ class GraphGenerator:
         slot = [None] * B                  # request held by slot b (None: empty)
         posn = [0] * B                     # position of slot b's row: the seq index of the event it feeds next
         nxt = 0
+        keys = _share_keys(prompts, self.kv1.page)
+        # a call without a shared prompt keeps the identity block table and each slot's own pages
+        pages = SharedPages(self.kv1) if any(k is not None for k in keys) else None
         cur = torch.cuda.current_stream()
         self.stream.wait_stream(cur)
         with torch.cuda.stream(self.stream):
@@ -670,39 +813,48 @@ class GraphGenerator:
             self._capture(use_graph, self._set_queue_state)
             graph = self._graph()
             free = list(range(B))
-            while True:
-                if free:
-                    for b in free:
-                        slot[b] = None
-                        if nxt < N:
-                            self._admit(b, prompts[nxt], settings[nxt] if self.rows else None)
-                            slot[b], posn[b] = nxt, prompts[nxt].shape[0] - 1
-                            nxt += 1
-                    live = [b for b in range(B) if slot[b] is not None]
-                    if not live:
-                        break
-                    pos = max(posn[b] for b in live)
-                    offs = [posn[b] - pos if slot[b] is not None else -pos for b in range(B)]
-                    self.pos.fill_(pos)
-                    self.row_off.copy_(torch.tensor(offs, dtype=torch.int32))
-                    self.row_end.copy_(torch.tensor([ends[s] if s is not None else 0 for s in slot], dtype=torch.int32))
-                    self.row_last.copy_(torch.tensor([-1 if s is not None else -2 for s in slot], dtype=torch.int32))
-                if use_graph == "persist":
-                    self._events_queue(max(ends[slot[b]] - posn[b] for b in live), exit_on_done=nxt < N)
-                elif use_graph:
-                    graph.replay()
-                else:
-                    self._event()
-                state = torch.cat([self.pos, self.row_last]).cpu()          # one small device->host copy per launch
-                p_now, last = int(state[0]), state[1:].tolist()
-                free = []
-                for b in live:
-                    if last[b] >= 0:
-                        out[slot[b]] = self.seq[b, :last[b] + 1].clone()
-                        free.append(b)
+            try:
+                while True:
+                    if free:
+                        if pages is not None:
+                            for b in free:
+                                pages.release(b)       # all before any admission: a finished group's pages may be reused
+                        for b in free:
+                            slot[b] = None
+                            if nxt < N:
+                                self._admit(b, prompts[nxt], settings[nxt] if self.rows else None, pages, keys[nxt])
+                                slot[b], posn[b] = nxt, prompts[nxt].shape[0] - 1
+                                nxt += 1
+                            elif pages is not None:
+                                pages.park(b)
+                        live = [b for b in range(B) if slot[b] is not None]
+                        if not live:
+                            break
+                        pos = max(posn[b] for b in live)
+                        offs = [posn[b] - pos if slot[b] is not None else -pos for b in range(B)]
+                        self.pos.fill_(pos)
+                        self.row_off.copy_(torch.tensor(offs, dtype=torch.int32))
+                        self.row_end.copy_(torch.tensor([ends[s] if s is not None else 0 for s in slot], dtype=torch.int32))
+                        self.row_last.copy_(torch.tensor([-1 if s is not None else -2 for s in slot], dtype=torch.int32))
+                    if use_graph == "persist":
+                        self._events_queue(max(ends[slot[b]] - posn[b] for b in live), exit_on_done=nxt < N)
+                    elif use_graph:
+                        graph.replay()
                     else:
-                        posn[b] = p_now + offs[b]
-                live = [b for b in live if b not in free]
+                        self._event()
+                    state = torch.cat([self.pos, self.row_last]).cpu()          # one small device->host copy per launch
+                    p_now, last = int(state[0]), state[1:].tolist()
+                    free = []
+                    for b in live:
+                        if last[b] >= 0:
+                            out[slot[b]] = self.seq[b, :last[b] + 1].clone()
+                            free.append(b)
+                        else:
+                            posn[b] = p_now + offs[b]
+                    live = [b for b in live if b not in free]
+            finally:
+                if pages is not None:
+                    pages.close()
         cur.wait_stream(self.stream)
         return out
 

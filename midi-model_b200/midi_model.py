@@ -1149,6 +1149,9 @@ class MIDIModel(PreTrainedModel):
         inputs and batch_size, but its attention's split count follows the loop's max_len, so that guarantee is not made
         there.
 
+        Requests with equal prompts of at least 65 events are prefilled once and share the KV pages of the prompt's whole
+        pages; this changes no request's result.
+
         Runs on the device-resident loop (B200_GENERATE persist, graph or nograph); B200_GENERATE=eager raises
         B200Error, as do malformed prompts, budgets, per-request sequences of the wrong length, temp <= 0, top_p outside
         (0, 1], top_k < 1, seeds out of range or of the wrong count, and channels outside 0..15."""
