@@ -351,6 +351,24 @@ int b200_decode_events_queue_rows(const b200_decode_desc* d, const int* row_off,
                                   int exit_on_done, int n_events, void* workspace, size_t workspace_bytes,
                                   const float* row_temp, const float* row_top_p, const int* row_top_k,
                                   const unsigned long long* row_seed, const int* row_first, cudaStream_t s);
+/*      streaming per-request queue: b200_decode_events_queue_rows that the host can watch and end while it runs.
+ *      out_events (int64 [batch][max_len][8]), committed (int32 [batch]) and ctl (one int32) are pinned host memory
+ *      (cudaHostAlloc / cudaHostRegister; the entry maps them with cudaHostGetDevicePointer and fails with B200_ERR_CUDA
+ *      if it cannot).  At every commit of a live row b at seq index q the kernel writes the event to out_events[b][q]
+ *      (as to seq), issues a system-scope fence, then stores committed[b] = q with a system-scope release: a host that
+ *      reads committed[b] and then out_events[b][.. committed[b]] sees complete events.  Nothing else of out_events
+ *      is written.
+ *      ctl asks the launch to end.  Thread 0 of CTA 0 samples it once per event, after the sampling of the event's last
+ *      token step, and every CTA takes the exit decision from that one sample after the commit barrier.  If the sample
+ *      of event e is nonzero, the launch ends after committing event e, leaving the state as any queue launch leaves it
+ *      (so the next launch continues exactly).  Bound: a store to ctl that is visible to the device while event e runs
+ *      ends the launch after event e or event e + 1; one already visible at the launch ends it after its first event.
+ *      The kernel never waits on ctl and never writes it: the host clears it. */
+int b200_decode_events_queue_stream(const b200_decode_desc* d, const int* row_off, const int* row_end, int* row_last,
+                                    int exit_on_done, int n_events, void* workspace, size_t workspace_bytes,
+                                    const float* row_temp, const float* row_top_p, const int* row_top_k,
+                                    const unsigned long long* row_seed, const int* row_first, long long* out_events,
+                                    int* committed, const int* ctl, cudaStream_t s);
 
 #ifdef __cplusplus
 }

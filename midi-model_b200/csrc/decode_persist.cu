@@ -82,13 +82,30 @@ struct PDRows : PDQueue {
     const unsigned long long* row_seed;  // [B]
     const int* row_first;                // [B]: seq index of the request's last prompt event
 };
-template <bool RAGGED, bool QUEUE = false, bool ROWS = false>
-using PDArg = std::conditional_t<ROWS, PDRows, std::conditional_t<QUEUE, PDQueue, std::conditional_t<RAGGED, PDRagged, PD>>>;
+// parameters of the streaming queue kernel (b200_decode_events_queue_stream): the per-request ones plus the host mirror of
+// the committed events and the host's "leave soon" flag (device pointers of pinned host memory)
+struct PDStream : PDRows {
+    long long* out_events;               // [B][max_len][8]: each committed event, at its seq index
+    int* committed;                      // [B]: seq index of row b's last committed event (release after the event)
+    const int* ctl;                      // the host sets it nonzero to end the launch
+    int* ctl_seen;                       // workspace word: ctl as CTA 0 read it in this event
+};
+template <bool RAGGED, bool QUEUE = false, bool ROWS = false, bool STREAM = false>
+using PDArg = std::conditional_t<STREAM, PDStream, std::conditional_t<ROWS, PDRows, std::conditional_t<QUEUE, PDQueue,
+              std::conditional_t<RAGGED, PDRagged, PD>>>>;
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
     unsigned v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
+}
+__device__ __forceinline__ int ld_acquire_sys_s32(const int* p) {
+    int v;
+    asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release_sys_s32(int* p, int v) {
+    asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ uint4 ldcg16(const void* p) { return __ldcg(reinterpret_cast<const uint4*>(p)); }
 // weights: read-only for the whole launch.  Event-level weights (403 MB) are streamed once per event -> evict first, so
@@ -682,10 +699,17 @@ __device__ __forceinline__ float rng_uniform(unsigned long long seed, unsigned l
 // row_end[b]; a row that is not live commits nothing, takes no part in the token-step count and skips its attention items.
 // ROWS (implies QUEUE): per-request rows.  Row b samples with its own settings and draws from its own key (PDRows), and its
 // event-level attention is cut on its own length (outer_attention), so a row's events do not depend on the other rows.
-template <int BM, bool RAGGED, bool QUEUE = false, bool ROWS = false>
-__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED, QUEUE, ROWS> p) {
+// STREAM (implies ROWS): each committed event is also written to the host mirror out_events, followed by a system fence
+// and a release store of committed[b], so the host reads it while the launch runs.  Once per event, after the last token
+// step's sampling, thread 0 of CTA 0 reads the host's ctl with an acquire load and stores it in the workspace; every CTA
+// reads that word after the commit barrier and, when it is nonzero, leaves after this event's commit through the same
+// uniform exit as exit_on_done.  No CTA reads ctl itself: CTAs that saw different values would deadlock at the next
+// grid barrier.  The kernel only samples ctl, it never waits on host memory.
+template <int BM, bool RAGGED, bool QUEUE = false, bool ROWS = false, bool STREAM = false>
+__global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED, QUEUE, ROWS, STREAM> p) {
     static_assert(!QUEUE || RAGGED, "the queue kernel positions its rows through row_off");
     static_assert(!ROWS || QUEUE, "per-request rows are queue rows");
+    static_assert(!STREAM || ROWS, "the streaming kernel is the per-request queue kernel");
     extern __shared__ __align__(16) uint8_t pd_smem[];
     const DD& d = p.d;
     const int B = d.batch, H = d.H;
@@ -936,8 +960,13 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
             prof.sub(PH_SAMPLE, 1);
         }
         // =============================== commit the event ========================================================
+        if constexpr (STREAM) {                          // published to every CTA by the barrier below
+            if (blockIdx.x == 0 && threadIdx.x == 0) *p.ctl_seen = ld_acquire_sys_s32(p.ctl);
+        }
         grid_sync(gb);                                   // every row's tokens are visible
         prof.mark(PH_SAMPLE);
+        int leave = 0;                                   // STREAM: the same value in every thread of the grid
+        if constexpr (STREAM) leave = __ldcg(p.ctl_seen);
         __syncthreads();
         for (int k = threadIdx.x; k < B * PD_T; k += PD_THREADS) {
             const int b = k / PD_T, t = k % PD_T;
@@ -950,9 +979,17 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
                 if constexpr (RAGGED) row_pos += p.row_off[b];
                 d.seq[((size_t)b * d.max_len + row_pos + 1) * PD_T + t] = v;
                 d.ev_in[k] = v;
+                if constexpr (STREAM) {
+                    p.out_events[((size_t)b * d.max_len + row_pos + 1) * PD_T + t] = v;
+                    __threadfence_system();
+                }
             }
         }
         __syncthreads();
+        if constexpr (STREAM) {                           // after every token of the row's event is fenced
+            const int b = threadIdx.x;
+            if (blockIdx.x == 0 && b < B && ((live >> b) & 1u)) st_release_sys_s32(p.committed + b, pos + p.row_off[b] + 1);
+        }
         prof.mark(PH_COMMIT);
         unsigned fin = 0;                                 // QUEUE: rows that finished in this event
         if constexpr (QUEUE) {
@@ -972,6 +1009,9 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
         events_done++;
         if constexpr (QUEUE) {
             if (live == 0 || (fin != 0 && p.exit_on_done)) break;
+        }
+        if constexpr (STREAM) {
+            if (leave) break;
         }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -1017,10 +1057,17 @@ struct RowArgs {
     const unsigned long long* seed;
     const int* first;
 };
+// host mirror and control flag of the STREAM kernel (b200_decode_events_queue_stream), as device pointers
+struct StreamArgs {
+    long long* out_events;
+    int* committed;
+    const int* ctl;
+};
 
-template <bool RAGGED, bool QUEUE = false, bool ROWS = false>
+template <bool RAGGED, bool QUEUE = false, bool ROWS = false, bool STREAM = false>
 int decode_events(const b200_decode_desc* desc, const int* row_off, const int* row_end, int* row_last, int exit_on_done,
-                  int n_events, void* workspace, size_t workspace_bytes, cudaStream_t stream, const RowArgs* rows = nullptr) {
+                  int n_events, void* workspace, size_t workspace_bytes, cudaStream_t stream, const RowArgs* rows = nullptr,
+                  const StreamArgs* st = nullptr) {
     const b200_decode_desc& d = *desc;
     B200_CHECK_ARG(!RAGGED || row_off != nullptr, "decode_events_ragged: row_off required");
     B200_CHECK_ARG(!QUEUE || (row_end != nullptr && row_last != nullptr), "decode_events_queue: row_end and row_last required");
@@ -1064,7 +1111,7 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, const int* r
     p.k_max = d.I_outer > d.I_inner ? d.I_outer : d.I_inner;
     if (p.k_max < d.H) p.k_max = d.H;
     B200_CUDA(cudaMemsetAsync(p.bar, 0, 256, stream), "decode_events: barrier reset");
-    PDArg<RAGGED, QUEUE, ROWS> pk;
+    PDArg<RAGGED, QUEUE, ROWS, STREAM> pk;
     static_cast<PD&>(pk) = p;
     if constexpr (RAGGED) pk.row_off = row_off;
     if constexpr (QUEUE) {
@@ -1079,17 +1126,23 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, const int* r
         pk.row_seed = rows->seed;
         pk.row_first = rows->first;
     }
+    if constexpr (STREAM) {
+        pk.out_events = st->out_events;
+        pk.committed = st->committed;
+        pk.ctl = st->ctl;
+        pk.ctl_seen = (int*)(ws + L.bar + 128);      // in the barrier's 256 bytes, cleared with them before the launch
+    }
     const int bm = d.batch <= 1 ? 1 : d.batch <= 2 ? 2 : d.batch <= 4 ? 4 : d.batch <= 8 ? 8 : 16;
     const size_t smem = (size_t)bm * p.k_max * 2 + (size_t)smp::SMP_MAXV * 8 + (PD_THREADS + 8) * 4 + 64 * 4 +
                         PD_WARPS * 64 * (4 + 2 + 2) + (size_t)bm * PD_T * 4 + 64;
     void* args[] = {(void*)&pk};
     const void* fn = nullptr;
     switch (bm) {
-        case 1: fn = (const void*)decode_events_kernel<1, RAGGED, QUEUE, ROWS>; break;
-        case 2: fn = (const void*)decode_events_kernel<2, RAGGED, QUEUE, ROWS>; break;
-        case 4: fn = (const void*)decode_events_kernel<4, RAGGED, QUEUE, ROWS>; break;
-        case 8: fn = (const void*)decode_events_kernel<8, RAGGED, QUEUE, ROWS>; break;
-        default: fn = (const void*)decode_events_kernel<16, RAGGED, QUEUE, ROWS>; break;
+        case 1: fn = (const void*)decode_events_kernel<1, RAGGED, QUEUE, ROWS, STREAM>; break;
+        case 2: fn = (const void*)decode_events_kernel<2, RAGGED, QUEUE, ROWS, STREAM>; break;
+        case 4: fn = (const void*)decode_events_kernel<4, RAGGED, QUEUE, ROWS, STREAM>; break;
+        case 8: fn = (const void*)decode_events_kernel<8, RAGGED, QUEUE, ROWS, STREAM>; break;
+        default: fn = (const void*)decode_events_kernel<16, RAGGED, QUEUE, ROWS, STREAM>; break;
     }
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "decode_events smem attr");
     int per_sm = 0;
@@ -1128,4 +1181,25 @@ extern "C" int b200_decode_events_queue_rows(const b200_decode_desc* desc, const
     const RowArgs rows{row_temp, row_top_p, row_top_k, row_seed, row_first};
     return decode_events<true, true, true>(desc, row_off, row_end, row_last, exit_on_done, n_events, workspace,
                                            workspace_bytes, stream, &rows);
+}
+
+extern "C" int b200_decode_events_queue_stream(const b200_decode_desc* desc, const int* row_off, const int* row_end,
+                                               int* row_last, int exit_on_done, int n_events, void* workspace,
+                                               size_t workspace_bytes, const float* row_temp, const float* row_top_p,
+                                               const int* row_top_k, const unsigned long long* row_seed,
+                                               const int* row_first, long long* out_events, int* committed,
+                                               const int* ctl, cudaStream_t stream) {
+    B200_CHECK_ARG(out_events != nullptr && committed != nullptr && ctl != nullptr,
+                   "decode_events_queue_stream: out_events, committed and ctl required (pinned host memory)");
+    StreamArgs st{};
+    void* dev = nullptr;
+    B200_CUDA(cudaHostGetDevicePointer(&dev, (void*)out_events, 0), "decode_events_queue_stream: out_events is not pinned");
+    st.out_events = (long long*)dev;
+    B200_CUDA(cudaHostGetDevicePointer(&dev, (void*)committed, 0), "decode_events_queue_stream: committed is not pinned");
+    st.committed = (int*)dev;
+    B200_CUDA(cudaHostGetDevicePointer(&dev, (void*)ctl, 0), "decode_events_queue_stream: ctl is not pinned");
+    st.ctl = (const int*)dev;
+    const RowArgs rows{row_temp, row_top_p, row_top_k, row_seed, row_first};
+    return decode_events<true, true, true, true>(desc, row_off, row_end, row_last, exit_on_done, n_events, workspace,
+                                                 workspace_bytes, stream, &rows, &st);
 }

@@ -91,6 +91,7 @@ SIGNATURES = {
     "b200_decode_events_ragged": (i32, [vp, vp, i32, vp, sz, vp]),
     "b200_decode_events_queue": (i32, [vp, vp, vp, vp, i32, i32, vp, sz, vp]),
     "b200_decode_events_queue_rows": (i32, [vp, vp, vp, vp, i32, i32, vp, sz, vp, vp, vp, vp, vp, vp]),
+    "b200_decode_events_queue_stream": (i32, [vp, vp, vp, vp, i32, i32, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
 }
 
 
