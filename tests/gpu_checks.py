@@ -2252,18 +2252,21 @@ def check_sampler_conformance():
     return out
 
 
-def _event_step64(eng, e, k_pools, v_pools, bt, page, pos, cos, sin):
-    """The event-level stack's step for a new event at position `pos` in fp64 (no rounding), over the cached keys /
-    values 0 .. pos-1 of each layer's pools.  Returns each layer's new (k, v) as [B, n_heads, D]."""
+def _event_step64(eng, e, k_pools, v_pools, bt, page, pos, cos, sin, want_x=False):
+    """The event-level stack's step for a new event at position `pos` (one for every row, or one per row) in fp64 (no
+    rounding), over the cached keys / values 0 .. pos-1 of each layer's pools.  Returns each layer's new (k, v) as
+    [B, n_heads, D]; with `want_x` also the stack's output x [B, H] (before the final norm)."""
     c = eng.cfg
     nh, D, H = c.n_head, c.head_dim, c.hidden
     B = e.shape[0]
+    rows_pos = [int(pos)] * B if np.ndim(pos) == 0 else [int(p) for p in pos]
+    pidx = torch.tensor(rows_pos, device=e.device)
 
     def rms(x, w):
         return w.double() * x / torch.sqrt(x.pow(2).mean(-1, keepdim=True) + c.eps)
 
     def rope(x):
-        cs, sn = cos[pos].double(), sin[pos].double()
+        cs, sn = cos[pidx].double()[:, None], sin[pidx].double()[:, None]
         x1, x2 = x[..., :D // 2], x[..., D // 2:]
         return torch.cat([x1 * cs - x2 * sn, x2 * cs + x1 * sn], -1)
 
@@ -2275,8 +2278,8 @@ def _event_step64(eng, e, k_pools, v_pools, bt, page, pos, cos, sin):
         q, k = rope(q), rope(k)
         kv.append((k, v))
         o = torch.empty(B, nh, D, dtype=torch.float64, device=e.device)
-        t = torch.arange(pos, device=e.device)
         for b in range(B):
+            t = torch.arange(rows_pos[b], device=e.device)
             pg = bt[b].long()[t // page]
             kc = torch.cat([k_pools[li][pg, :, t % page].transpose(0, 1).double(), k[b][:, None]], 1)
             vc = torch.cat([v_pools[li][pg, :, t % page].transpose(0, 1).double(), v[b][:, None]], 1)
@@ -2286,7 +2289,46 @@ def _event_step64(eng, e, k_pools, v_pools, bt, page, pos, cos, sin):
         gu = rms(h, w.ln2) @ w.gu.double().T
         I = gu.shape[1] // 2
         x = h + (F.silu(gu[:, :I]) * gu[:, I:]) @ w.down.double().T
-    return kv
+    return (kv, x) if want_x else kv
+
+
+def _token_steps64(eng, lm_head, outer_norm, x, tokens, n, cos, sin, *, rope_lag=0):
+    """The token-level half of one event in fp64 (no rounding), from the event-level output x [B, H] and the event's
+    tokens [>= n - 1, B] (teacher-forced): hidden = RMSNorm(x) with the event-level stack's final norm, step i's input is
+    hidden (i = 0) or the token-level embedding of tokens[i - 1] (an id outside [0, V) reads row 0, as the kernel does),
+    causal attention over steps 0 .. i with RoPE at position i (cos / sin: [positions, D / 2]), final norm, lm_head.
+    Returns (k, v) [n_layers, B, n, n_heads, D] and logits [B, n, V].  `rope_lag` rotates step i at position i - 1."""
+    c = eng.cfg
+    nh, D, H = c.n_head, c.head_dim, c.hidden
+    B, V = x.shape[0], lm_head.shape[0]
+
+    def rms(z, w):
+        return w.double() * z / torch.sqrt(z.pow(2).mean(-1, keepdim=True) + c.eps)
+
+    ids = tokens[:n - 1].long().clone()
+    ids[(ids < 0) | (ids >= V)] = 0
+    z = torch.cat([rms(x.double(), outer_norm)[:, None], eng.embed.double()[ids.T]], 1)       # [B, n, H]
+    t = (torch.arange(n, device=x.device) - rope_lag).clamp_min(0)
+    cs, sn = cos[t].double(), sin[t].double()
+
+    def rope(q):                                                                            # [B, nh, n, D]
+        q1, q2 = q[..., :D // 2], q[..., D // 2:]
+        return torch.cat([q1 * cs - q2 * sn, q2 * cs + q1 * sn], -1)
+
+    future = torch.triu(torch.ones(n, n, dtype=torch.bool, device=x.device), 1)
+    ks, vs = [], []
+    for w in eng.layers:
+        qkv = rms(z, w.ln1) @ w.qkv.double().T
+        q, k, v = (qkv[..., i * H:(i + 1) * H].view(B, n, nh, D).transpose(1, 2) for i in range(3))
+        q, k = rope(q), rope(k)
+        ks.append(k.transpose(1, 2))
+        vs.append(v.transpose(1, 2))
+        p = torch.softmax((q @ k.transpose(-1, -2) / math.sqrt(D)).masked_fill(future, float("-inf")), -1)
+        h = z + (p @ v).transpose(1, 2).reshape(B, n, H) @ w.o.double().T
+        gu = rms(h, w.ln2) @ w.gu.double().T
+        I = gu.shape[-1] // 2
+        z = h + (F.silu(gu[..., :I]) * gu[..., I:]) @ w.down.double().T
+    return torch.stack(ks), torch.stack(vs), rms(z, eng.norm) @ lm_head.double().T
 
 
 # same card: layer-0 k / v bit-identical and within 1 ulp of the fp64 chain (frac 1.2e-4); worst (row, head) of any
@@ -2378,6 +2420,365 @@ def check_persist_vs_phase():
             model._return_generator(key, gg)
     out = W.report()
     out["pd_one_chunk_batches"], out["pd_multi_chunk_batches"] = float(len(one_chunk)), float(len(multi_chunk))
+    return out
+
+
+# ------------------------------------------------------------------------------------------ persistent kernel, token level
+PT_SIZES = (1, 2, 3, 4, 5, 8, 9, 16)         # every batch tile BM (1, 2, 4, 8, 16), full and partly filled
+PT_POS = (31, 64, 65, 4095)
+PT_MAX_LEN = 4097
+PT_PLAIN = ((1.0, 0.98, 20), (1.7, 1.0, 64), (0.5, 0.5, 2))      # (temp, top_p, top_k) of b200_decode_events
+PT_RAGGED, PT_QUEUE = (1.0, 0.98, 20), (1.7, 0.5, 64)
+PT_ROW_TEMP, PT_ROW_TOP_P, PT_ROW_TOP_K = (0.5, 1.0, 1.7), (1.0, 0.98, 0.5, 0.1), (1, 2, 20, 64)
+
+
+def _pt_models(names=("base", "peaked")):
+    """persist_vs_phase's seeded random model of the real widths with 2 event-level and 2 token-level layers ("base"), and
+    the same model with an 8x lm_head ("peaked": its peaked logits make top-p cut, EOS and short events occur and the
+    temperature matter)."""
+    cfg = GM.config()
+    cfg.net_config.num_hidden_layers = 2
+    cfg.net_token_config.num_hidden_layers = 2
+    out = {}
+    for name in names:
+        m = GM.cpu_model(cfg)
+        if name == "peaked":
+            with torch.no_grad():
+                m.lm_head.weight.mul_(8.0)
+        out[name] = m.to(DEV, dtype=BF).eval()
+    return out
+
+
+def _ragged_offsets(B, pos):
+    """Row offsets of the ragged / queue tests: 0, -1, -31, -32, -33 and the largest spread (a row at position 0),
+    clipped to positions >= 0."""
+    cyc = [0, -1, -31, -32, -33, -pos]
+    return [max(cyc[b % len(cyc)], -pos) for b in range(B)]
+
+
+def _pt_launch(gg, kind, n):
+    """n events of the persistent kernel's entry `kind` (plain / ragged / queue / rows) on gg's state, without an exit on a
+    finished row."""
+    import ctypes
+    d, ws, _ = gg._persistent()
+    dp, w = ctypes.byref(d), (ws.data_ptr(), ws.numel())
+    if kind == "plain":
+        lib.call("b200_decode_events", dp, n, *w, lib.stream())
+    elif kind == "ragged":
+        lib.call("b200_decode_events_ragged", dp, gg.row_off.data_ptr(), n, *w, lib.stream())
+    elif kind == "queue":
+        lib.call("b200_decode_events_queue", dp, gg.row_off.data_ptr(), gg.row_end.data_ptr(), gg.row_last.data_ptr(), 0, n,
+                 *w, lib.stream())
+    else:
+        lib.call("b200_decode_events_queue_rows", dp, gg.row_off.data_ptr(), gg.row_end.data_ptr(), gg.row_last.data_ptr(),
+                 0, n, *w, gg.row_temp.data_ptr(), gg.row_top_p.data_ptr(), gg.row_top_k.data_ptr(), gg.row_seed.data_ptr(),
+                 gg.row_first.data_ptr(), lib.stream())
+
+
+def _pt_masks(gg, kinds, seed):
+    """gg.mask rows by kind: 0 every id allowed; 1 a random 40 % of the parameter ids denied; 2 every event type denied
+    but EOS (an all-pad event); 3 EOS and every event type but the 7-parameter note denied (8 steps)."""
+    g = gg.g
+    ev = torch.arange(g.eos + 1, g.eos + 1 + g.n_event_types, device=DEV)
+    note = next(e for e, n_ in g.n_params.items() if n_ == 7)
+    gen = torch.Generator(device=DEV).manual_seed(seed)
+    gg.mask.fill_(1)
+    for b, k in enumerate(kinds):
+        if k == 1:
+            deny = torch.rand(gg.V, generator=gen, device=DEV) < 0.4
+            deny[:g.eos + 1 + g.n_event_types] = False
+            gg.mask[b, deny] = 0
+        elif k == 2:
+            gg.mask[b, ev] = 0
+        elif k == 3:
+            gg.mask[b, ev[ev != note]] = 0
+            gg.mask[b, g.eos] = 0
+
+
+def _pt_state(gg, pools0, prompt, pos, offs, live, c0):
+    """Device state of one event: the prefilled pools with every slot from row b's new position on (and every slot of a
+    row that is not live) NaN, row b at pos + offs[b] fed its prompt event there, seq all -5.  Returns the pools as set."""
+    kv, B = gg.kv1, gg.B
+    nh, D, page, mp = kv.cfg.n_head, kv.cfg.head_dim, kv.page, kv.max_pages
+    ctx = torch.tensor([pos + o for o in offs], device=DEV)
+    past = (torch.arange(mp * page, device=DEV)[None] >= ctx[:, None]) | ~torch.tensor(live, device=DEV)[:, None]
+    pre = []
+    for pool, s in zip(kv.k + kv.v, pools0):
+        pool.copy_(s)
+        pool.view(B, mp, nh, page, D).masked_fill_(past.view(B, mp, 1, page, 1), float("nan"))
+        pre.append(pool.clone())
+    gg.pos.fill_(pos)
+    gg.ev_in.copy_(prompt[torch.arange(B, device=DEV), ctx])
+    gg.counter.copy_(torch.tensor([c0, gg.seed], dtype=torch.int64))
+    gg.seq.fill_(-5)
+    gg.row_off.copy_(torch.tensor(offs, dtype=torch.int32))
+    return pre
+
+
+def _pt_loop(gg, x, ev_t, n):
+    """The launch-per-phase loop's token-level half (GraphGenerator._event) from the event-level output x, teacher-forced
+    with the tokens ev_t [8, B] (ids outside [0, V) read row 0, as the persistent kernel does): returns the token-level
+    cache (a fresh PagedKV of page 8) and each step's logits [n, B, V]."""
+    from midi_b200 import decode as dec
+    eng, B, V = gg.inner.eng, gg.B, gg.V
+    hidden = ops.rmsnorm(x, gg.outer.eng.norm, gg.outer.eng.cfg.eps)
+    kv2 = dec.PagedKV(eng.cfg, B, 8, 8, DEV)
+    logits = []
+    for i in range(n):
+        if i == 0:
+            xin = ops.inner_input(hidden, None, eng.embed)
+        else:
+            ids = ev_t[i - 1].clone()
+            ids[(ids < 0) | (ids >= V)] = 0
+            xin = ops.inner_input(None, ids.view(B, 1), eng.embed)
+        hs = gg.inner.step(xin, kv2, 1, final_norm=False)
+        logits.append(dec._gemv_fused(hs, gg.lm_head, V, norm_w=eng.norm, eps=eng.cfg.eps, ldy=gg.pitch)[:, :V])
+    return kv2, torch.stack(logits)
+
+
+def _pt_ws(ws, L, name, dtype, shape):
+    n = math.prod(shape) * torch.empty((), dtype=dtype).element_size()
+    return ws[L[name]:L[name] + n].clone().view(dtype).view(shape)
+
+
+# H100 80GB HBM3, 700 W: the token-level half was bit-identical to the launch-per-phase kernels (k / v of every step and
+# layer, last logits) and all 15912 unambiguous draws were the restated ones; 3.1 % of the draws were ambiguous (a
+# candidate's fp64 p within 2^-17 of a bf16 midpoint), bound about 5x.  Worst row against fp64: x 9.1e-3, k2 9.1e-3,
+# v2 8.7e-3, last logits 7.6e-3, bounds about 5x.  The counters' minimums are about 80 % of the counts measured there
+# (unambiguous 15912, top-p cuts 89, top_k 1 / 2 / 20 / 64: 644 / 3404 / 6325 / 5539, ties 3998, EOS rows 665, 8-step
+# events 316, 2-step events 25); the masked, not-live and fp64 counts follow from the case set alone.
+@bounded([
+    ("pt_ws_layout_error", 0.0), ("pt_k_loop_mismatch", 0.0), ("pt_v_loop_mismatch", 0.0), ("pt_logits_loop_mismatch", 0.0),
+    ("pt_nan_read", 0.0), ("pt_draw_mismatch", 0.0), ("pt_ambiguous_frac", 0.15), ("pt_n_steps_error", 0.0),
+    ("pt_not_live_token_not_pad", 0.0), ("pt_seq_mismatch", 0.0), ("pt_ev_in_mismatch", 0.0), ("pt_pos_advance_error", 0.0),
+    ("pt_counter_advance_error", 0.0), ("pt_row_last_error", 0.0), ("pt_other_slots_changed", 0.0),
+    ("pt_f64_x_row", 4.5e-2), ("pt_f64_k_row", 4.5e-2), ("pt_f64_v_row", 4.5e-2), ("pt_f64_logits_row", 4e-2),
+    ("min:pt_count_bm", 5.0), ("min:pt_count_unambiguous", 12000.0), ("min:pt_count_topp_cut", 60.0),
+    ("min:pt_count_topk1_draws", 500.0), ("min:pt_count_topk2_draws", 2500.0), ("min:pt_count_topk20_draws", 5000.0),
+    ("min:pt_count_topk64_draws", 4000.0), ("min:pt_count_tie", 3000.0), ("min:pt_count_eos_rows", 500.0),
+    ("min:pt_count_8_step_events", 250.0), ("min:pt_count_2_step_events", 15.0), ("min:pt_count_masked_rows", 1554.0),
+    ("min:pt_count_not_live_rows", 208.0), ("min:pt_count_f64_cases", 128.0),
+])
+def check_persist_token_exact():
+    """One event of the persistent generate kernel per launch -- b200_decode_events at several settings, _ragged, _queue
+    with rows that are not live, _queue_rows with per-row settings, seeds and row_first -- at every batch tile, scored step
+    by step.  The workspace is 0xFF-filled (NaN in bf16) before the launch; afterwards its x, logits, ev_t, k2 and v2
+    (decode_reference.decode_ws_layout) are read.  From the kernel's own x and tokens, the launch-per-phase loop's calls
+    (RMSNorm, inner_input, the token-level step, the fused lm_head) must reproduce every token-level k / v and the last
+    logits bit for bit; every sampling decision must be decode_reference.logits_sample of the loop's logits in the
+    restated grammar range with the restated uniform; the step count, commit, positions, counter, row_last and pool
+    slots must be the restated ones; x, k2 / v2 and the logits are anchored to an fp64 event step and token steps."""
+    import ctypes
+    import decode_reference as DR
+    W = _Worst("pt_")
+    cnt = {k: 0 for k in ("unambiguous", "topp_cut", "topk1_draws", "topk2_draws", "topk20_draws", "topk64_draws", "tie",
+                          "eos_rows", "8_step_events", "2_step_events", "masked_rows", "not_live_rows", "f64_cases")}
+    bms, n_dec, n_amb = set(), 0, 0
+    for mname, model in _pt_models().items():
+        V = model.tokenizer.vocab_size
+        for B in PT_SIZES:
+            key, gg = model._checkout_generator(B, PT_MAX_LEN, 1.0, 0.98, 20, None)
+            d, ws, _ = gg._persistent()
+            scalar = (d.temp, d.top_p, d.top_k)
+            try:
+                assert gg.persistent_ok()
+                gg.alloc_rows()
+                bms.add(1 if B <= 1 else 2 if B <= 2 else 4 if B <= 4 else 8 if B <= 8 else 16)
+                L = DR.decode_ws_layout(d.batch, d.H, d.I_outer, d.I_inner, d.pitch, d.nh_outer, d.n_inner)
+                W.add("", f"B{B}", {"ws_layout_error": abs(L["total"] - lib.load().b200_decode_events_workspace_bytes(
+                    ctypes.byref(d)))})
+                kv, g = gg.kv1, gg.g
+                lut, eos, pad, n_ty = g.lut.cpu().numpy(), g.eos, g.pad, g.n_event_types
+                H, n_in = d.H, d.n_inner
+                nh2, D2 = gg.inner.eng.cfg.n_head, gg.inner.eng.cfg.head_dim
+                nl = len(kv.k)
+                for pos in PT_POS:
+                    gen = torch.Generator(device=DEV).manual_seed(pos * 17 + B)
+                    prompt = torch.randint(0, V, (B, pos + 1, 8), generator=gen, device=DEV)
+                    gg._set_lengths(prompt, None)
+                    gg._set_state(prompt)
+                    pools0 = [t.clone() for t in kv.k + kv.v]
+                    variants = [("plain", s) for s in PT_PLAIN] + [("ragged", PT_RAGGED), ("queue", PT_QUEUE), ("rows", None)]
+                    for vi, (kind, sc) in enumerate(variants):
+                        case = f"{mname} B{B} pos{pos} {kind}{vi}"
+                        offs = [0] * B if kind == "plain" else _ragged_offsets(B, pos)
+                        queue = kind in ("queue", "rows")
+                        live = [not (queue and b % 3 == 2) for b in range(B)]
+                        ctx = [pos + o for o in offs]
+                        c0 = 3 + pos + vi
+                        pre = _pt_state(gg, pools0, prompt, pos, offs, live, c0)
+                        kinds = [(b + vi + pos) % 4 for b in range(B)]
+                        _pt_masks(gg, kinds, seed=pos + 31 * vi + B)
+                        if kind == "rows":
+                            settings = [(PT_ROW_TEMP[(b + vi) % 3], PT_ROW_TOP_P[(b + pos) % 4], PT_ROW_TOP_K[(b + pos // 2) % 4])
+                                        for b in range(B)]
+                            first = [max(0, ctx[b] - (3 * b + pos) % 11) for b in range(B)]
+                            seeds = [(1000003 * (b + 1) + 7919 * pos + vi) & ((1 << 62) - 1) for b in range(B)]
+                            gg.row_temp.copy_(torch.tensor([s[0] for s in settings]))
+                            gg.row_top_p.copy_(torch.tensor([s[1] for s in settings]))
+                            gg.row_top_k.copy_(torch.tensor([s[2] for s in settings], dtype=torch.int32))
+                            gg.row_seed.copy_(torch.tensor(seeds, dtype=torch.int64))
+                            gg.row_first.copy_(torch.tensor(first, dtype=torch.int32))
+                        else:
+                            settings = [sc] * B
+                            d.temp, d.top_p, d.top_k = sc
+                        row_end = [ctx[b] + 1 if b % 4 == 1 else PT_MAX_LEN - 1 for b in range(B)]
+                        row_last = [-1 if live[b] else (-2 if b % 2 else ctx[b]) for b in range(B)]
+                        gg.row_end.copy_(torch.tensor(row_end, dtype=torch.int32))
+                        gg.row_last.copy_(torch.tensor(row_last, dtype=torch.int32))
+                        ev_in0, mask_np = gg.ev_in.clone(), gg.mask.cpu().numpy()
+                        ws.fill_(255)
+                        _pt_launch(gg, kind, 1)
+                        torch.cuda.synchronize()
+                        x = _pt_ws(ws, L, "x", BF, (B, H))
+                        lg = _pt_ws(ws, L, "logits", BF, (B, d.pitch))[:, :V]
+                        evt = _pt_ws(ws, L, "ev_t", torch.int64, (8, B))
+                        k2 = _pt_ws(ws, L, "k2", BF, (n_in, B, 8, H))
+                        v2 = _pt_ws(ws, L, "v2", BF, (n_in, B, 8, H))
+                        evt_np = evt.cpu().numpy()
+                        n = 0
+                        while n < 8 and (evt_np[n] != -1).all():
+                            n += 1
+                        n_want = DR.event_n_steps(evt_np[0], live, lut, eos, n_ty)
+                        lv = torch.tensor(live, device=DEV)
+                        m = {"n_steps_error": abs(n - n_want),
+                             "nan_read": float(torch.isnan(x[lv]).sum() + torch.isnan(lg[lv]).sum()
+                                               + torch.isnan(k2[:, lv, :n]).sum() + torch.isnan(v2[:, lv, :n]).sum()),
+                             "not_live_token_not_pad": float((evt_np[:n][:, ~np.array(live)] != pad).sum())}
+                        # ---- 1. the token-level half against the launch-per-phase kernels, bit for bit
+                        kv2, llog = _pt_loop(gg, x, evt, max(n, 1))
+                        for nm, pools, kern in (("k", kv2.k, k2), ("v", kv2.v, v2)):
+                            bad = 0.0
+                            for li in range(n_in):
+                                lp = pools[li].view(B, nh2, 8, D2).permute(0, 2, 1, 3).reshape(B, 8, H)
+                                bad += _ne(kern[li][lv, :n], lp[lv, :n])
+                            m[f"{nm}_loop_mismatch"] = bad
+                        m["logits_loop_mismatch"] = _ne(lg[lv], llog[max(n, 1) - 1][lv])
+                        # ---- 2. every sampling decision
+                        if kind == "rows":
+                            u = DR.event_uniforms("rows", B, max(n, 1), pos=pos, row_off=offs, row_first=first, row_seed=seeds)
+                        else:
+                            u = DR.event_uniforms(kind, B, max(n, 1), c0=c0, seed=gg.seed)
+                        dec_ = DR.event_decisions(llog.float().cpu().numpy(), evt_np, n, live, settings, mask_np, u, lut,
+                                                  eos, pad, n_ty)
+                        isdec = dec_["id"] >= 0
+                        clear = isdec & ~dec_["amb"]
+                        m["draw_mismatch"] = float((clear & (dec_["id"] != evt_np[:n])).sum())
+                        n_dec += int(isdec.sum())
+                        n_amb += int((isdec & dec_["amb"]).sum())
+                        cnt["unambiguous"] += int(clear.sum())
+                        cnt["topp_cut"] += int((clear & dec_["cut"]).sum())
+                        cnt["tie"] += int((clear & dec_["tie"]).sum())
+                        for k_ in PT_ROW_TOP_K:
+                            cnt[f"topk{k_}_draws"] += int(clear[:, [s[2] == k_ for s in settings]].sum())
+                        # ---- 3. event bookkeeping
+                        _, seq_w, ev_w = DR.event_commit_rows(evt_np, n_want, live, np.full((B, PT_MAX_LEN, 8), -5),
+                                                              ev_in0.cpu().numpy(), pos, offs, pad)
+                        m["seq_mismatch"] = float((gg.seq.cpu().numpy() != seq_w).sum())
+                        m["ev_in_mismatch"] = float((gg.ev_in.cpu().numpy() != ev_w).sum())
+                        m["pos_advance_error"] = abs(int(gg.pos) - pos - 1)
+                        m["counter_advance_error"] = abs(int(gg.counter[0]) - c0 - 8) + abs(int(gg.counter[1]) - gg.seed)
+                        if queue:
+                            want_last = [(ctx[b] + 1 if evt_np[0, b] == eos or ctx[b] + 1 >= row_end[b] else -1)
+                                         if live[b] else row_last[b] for b in range(B)]
+                            m["row_last_error"] = float(sum(a != w_ for a, w_ in zip(gg.row_last.tolist(), want_last)))
+                        slot = DR.slot_mask(pre[0].shape, kv.block_table, kv.page, [(b, ctx[b]) for b in range(B) if live[b]])
+                        m["other_slots_changed"] = sum(float((~_same(p_, s_) & ~slot).sum()) for p_, s_ in zip(kv.k + kv.v, pre))
+                        W.add("", case, m)
+                        cnt["eos_rows"] += sum(1 for b in range(B) if live[b] and evt_np[0, b] == eos)
+                        cnt["8_step_events"] += int(n == 8)
+                        cnt["2_step_events"] += int(n == 2)
+                        cnt["masked_rows"] += sum(1 for b in range(B) if live[b] and kinds[b] != 0)
+                        cnt["not_live_rows"] += B - sum(live)
+                        # ---- 4. fp64 anchors (the first plain setting and the per-row kernel)
+                        if vi == 0 or kind == "rows":
+                            cnt["f64_cases"] += 1
+                            e = ops.embed_sum(ev_in0, gg.outer.eng.embed)
+                            _, x64 = _event_step64(gg.outer.eng, e, pre[:nl], pre[nl:], kv.block_table, kv.page, ctx,
+                                                   gg.outer.cos, gg.outer.sin, want_x=True)
+                            k64, v64, lg64 = _token_steps64(gg.inner.eng, gg.lm_head, gg.outer.eng.norm, x, evt, max(n, 1),
+                                                            gg.inner.cos, gg.inner.sin)
+                            f = {"x_row": P.row_worst(x[lv], x64[lv]),
+                                 "logits_row": P.row_worst(lg[lv], lg64[lv, max(n, 1) - 1])}
+                            for nm, kern, ref in (("k", k2, k64), ("v", v2, v64)):
+                                got = kern[:, lv, :n].reshape(n_in, -1, n, nh2, D2)
+                                f[f"{nm}_row"] = P.row_worst(got, ref[:, lv, :n])
+                            W.add("f64", case, f)
+            finally:
+                d.temp, d.top_p, d.top_k = scalar
+                gg.set_deny(())
+                model._return_generator(key, gg)
+    out = W.report()
+    out["pt_ambiguous_frac"] = n_amb / max(n_dec, 1)
+    out["pt_count_bm"] = float(len(bms))
+    for k_, v_ in cnt.items():
+        out[f"pt_count_{k_}"] = float(v_)
+    for k_ in sorted(out):
+        if k_.startswith("pt_count") or k_ == "pt_ambiguous_frac":
+            print(f"  {k_} = {out[k_]:.4g}")
+    return out
+
+
+@bounded([("min:pm_count_cases", 12.0), ("min:pm_count_in_kernel_exits", 6.0), ("pm_", 0.0)])
+def check_persist_multi_event():
+    """One launch of 3 events of the persistent kernel against three launches of one, from the same state, for the plain,
+    ragged and per-row kernels: seq, ev_in, every pool, pos, the RNG counter and row_last must agree bit for bit.  This is
+    the in-kernel hand-over between events (cur_ev, pos++, the counter with events_done, rows that finish); a snapshot at
+    pos = max_len - 3 runs the in-kernel `pos + 1 >= max_len` exit inside the launch."""
+    W = _Worst("pm_")
+    model = _pt_models(("peaked",))["peaked"]
+    V = model.tokenizer.vocab_size
+    n_cases = n_exits = 0
+    for B in (3, 16):
+        key, gg = model._checkout_generator(B, PT_MAX_LEN, 1.0, 0.98, 20, None)
+        try:
+            gg.alloc_rows()
+            kv = gg.kv1
+            for pos in (65, PT_MAX_LEN - 3):
+                gen = torch.Generator(device=DEV).manual_seed(pos + 5 * B)
+                prompt = torch.randint(0, V, (B, pos + 1, 8), generator=gen, device=DEV)
+                gg._set_lengths(prompt, None)
+                gg._set_state(prompt)
+                pools0 = [t.clone() for t in kv.k + kv.v]
+                for kind in ("plain", "ragged", "rows"):
+                    offs = [0] * B if kind == "plain" else _ragged_offsets(B, pos)
+                    live = [not (kind == "rows" and b % 3 == 2) for b in range(B)]
+                    ctx = [pos + o for o in offs]
+                    _pt_state(gg, pools0, prompt, pos, offs, live, c0=11 + pos)
+                    # row 0 never finishes (no EOS, no budget), so every launch has a live row
+                    _pt_masks(gg, [0] + [b % 4 for b in range(1, B)], seed=pos + B)
+                    gg.mask[0, gg.g.eos] = 0
+                    if kind == "rows":
+                        gg.row_temp.copy_(torch.tensor([PT_ROW_TEMP[b % 3] for b in range(B)]))
+                        gg.row_top_p.copy_(torch.tensor([PT_ROW_TOP_P[b % 4] for b in range(B)]))
+                        gg.row_top_k.copy_(torch.tensor([PT_ROW_TOP_K[(b + 2) % 4] for b in range(B)], dtype=torch.int32))
+                        gg.row_seed.copy_(torch.tensor([977 * b + pos for b in range(B)], dtype=torch.int64))
+                        gg.row_first.copy_(torch.tensor([max(0, c - b % 5) for b, c in enumerate(ctx)], dtype=torch.int32))
+                        gg.row_end.copy_(torch.tensor([c + 2 if b % 4 == 1 else PT_MAX_LEN - 1 for b, c in enumerate(ctx)],
+                                                      dtype=torch.int32))
+                        gg.row_last.copy_(torch.tensor([-1 if live[b] else -2 for b in range(B)], dtype=torch.int32))
+                    state = kv.k + kv.v + [gg.seq, gg.ev_in, gg.pos, gg.counter, gg.row_last]
+                    snap = [t.clone() for t in state]
+                    runs = []
+                    for split in (False, True):
+                        for t, s in zip(state, snap):
+                            t.copy_(s)
+                        for _ in range(3 if split else 1):
+                            _pt_launch(gg, kind, 1 if split else 3)
+                        torch.cuda.synchronize()
+                        runs.append([t.clone() for t in state])
+                    one, three = runs
+                    n_run = int(one[-3]) - pos
+                    W.add("", f"B{B} pos{pos} {kind}", {
+                        "one_vs_three_mismatch": sum(float((~_same(a, b_)).sum()) for a, b_ in zip(one, three)),
+                        "events_run_error": abs(n_run - min(3, PT_MAX_LEN - 1 - pos))})
+                    n_cases += 1
+                    n_exits += int(n_run < 3)
+        finally:
+            gg.set_deny(())
+            model._return_generator(key, gg)
+    out = W.report()
+    out["pm_count_cases"], out["pm_count_in_kernel_exits"] = float(n_cases), float(n_exits)
     return out
 
 
@@ -3058,6 +3459,7 @@ GROUPS = {
     "gemm_matrix": check_gemm_matrix, "gemm_epilogues": check_gemm_epilogues, "attn_edges": check_attn_edges,
     "gemv_matrix": check_gemv_conformance, "decode_attn_edges": check_decode_attn_conformance,
     "sampler_exact": check_sampler_conformance, "persist_vs_phase": check_persist_vs_phase,
+    "persist_token_exact": check_persist_token_exact, "persist_multi_event": check_persist_multi_event,
     "embed_exact": check_embed_conformance, "rmsnorm_exact": check_rmsnorm_conformance, "rope_exact": check_rope_conformance,
     "swiglu_exact": check_swiglu_conformance, "attn_tiny_exact": check_attn_tiny_conformance,
     "loss_optim_exact": check_loss_optim_conformance,

@@ -340,6 +340,26 @@ def test_decode_descriptor_mirror_matches_the_header():
     assert names == [f[0] for f in lib.DecodeDesc._fields_]
 
 
+def test_decode_workspace_layout_restatement():
+    """decode_reference.decode_ws_layout, through which the persistent kernel's conformance group reads x, logits, ev_t
+    and the token-level k / v out of the workspace, gives the size b200_decode_events_workspace_bytes computes, for
+    descriptors of several batch sizes, token-level depths and MLP widths (a layout change fails here, not as a read of
+    the wrong bytes)."""
+    import ctypes
+    import decode_reference as DR
+    lib = _built()
+    for B, n_inner, I_outer, I_inner, pitch in ((1, 1, 4096, 1024, 3408), (2, 2, 4096, 1024, 3408),
+                                                (9, 2, 2048, 4096, 3408), (16, 3, 4096, 5120, 4096)):
+        d = lib.DecodeDesc()
+        d.batch, d.n_inner, d.I_outer, d.I_inner, d.pitch = B, n_inner, I_outer, I_inner, pitch
+        d.H, d.nh_outer, d.nh_inner, d.V, d.n_outer = 1024, 16, 4, 3406, 2
+        L = DR.decode_ws_layout(B, d.H, I_outer, I_inner, pitch, d.nh_outer, n_inner)
+        assert L["total"] == lib.query("b200_decode_events_workspace_bytes", ctypes.byref(d)), (B, n_inner, I_outer)
+        offs = [v for k, v in L.items() if k != "total"]
+        assert offs == sorted(offs) and all(o % 256 == 0 for o in offs) and L["bar"] == 0
+        assert L["k2"] + n_inner * B * 8 * d.H * 2 <= L["v2"]
+
+
 def test_generate_loop_modes():
     import midi_model as mm
     assert mm._loop_mode("persist") == "persist"
