@@ -275,7 +275,7 @@ int b200_event_commit_queue(const long long* ev_t, long long* seq, long long* ev
 /*      per-request queue (generate_many with per-request settings or seeds):
  *        sample_from_logits_rows: b200_sample_from_logits with row r's settings from row_temp, row_top_p, row_top_k (device
  *          float / float / int32 [rows]).  Preconditions (the caller's: checking device values would need a sync): row_temp[r]
- *          > 0 and row_top_k[r] >= 1.  top_k > 64 takes the general path, as in b200_sample_from_logits.
+ *          > 0 and row_top_k[r] >= 1.  top_k > 128 takes the general path, as in b200_sample_from_logits.
  *        uniform_fill_rows: u[b] = hash(row_seed[b], 8 j + step, 0) with j = *pos_dev + row_off[b] - row_first[b] (row_first:
  *          device int32 [B], seq index of the request's last prompt event; row_seed: device uint64 [B]), i.e. the draw that
  *          b200_uniform_fill makes for a batch-1 loop seeded row_seed[b] at its new event j, token step `step`.  The position
@@ -316,7 +316,7 @@ typedef struct b200_decode_desc {
     const int* lut;             /* [n_event_types][8][2] parameter id ranges (midi_tokenizer.py:517-535) */
     int n_event_types, eos_id, pad_id;
     float temp, top_p;
-    int top_k, batch;
+    int top_k /* 1..128 */, batch /* 1..16; 1..32 for the _queue_rows and _queue_stream entries */;
     unsigned long long* prof;   /* may be NULL.  Tuning hook: device array of 128 counters; [i] += SM cycles CTA 0 spent in phase i
                                    (incl. the closing barrier), [32 + i] += 1; phases: qkv, attention, combine, o_proj, gate|up,
                                    down of the event-level stack (0-5) and of the token-level stack (6-10, no combine),
@@ -346,7 +346,8 @@ int b200_decode_events_queue(const b200_decode_desc* d, const int* row_off, cons
  *      and rng_state seed are not used for draws.  Row b's event-level attention is cut into chunks exactly as the batch-1
  *      kernel cuts it at row b's own length, so with the same pages, position, settings, seed and mask row, row b commits
  *      bit for bit what b200_decode_events at batch 1 commits.  Preconditions (the caller's): every live row has
- *      row_temp > 0, 0 < row_top_p <= 1 and 1 <= row_top_k <= 64. */
+ *      row_temp > 0, 0 < row_top_p <= 1 and 1 <= row_top_k <= 128.  Batch 1..32: a launch of more than 16 rows
+ *      runs every per-row phase on two groups of at most 16 rows, each with the arithmetic of a 16-row launch. */
 int b200_decode_events_queue_rows(const b200_decode_desc* d, const int* row_off, const int* row_end, int* row_last,
                                   int exit_on_done, int n_events, void* workspace, size_t workspace_bytes,
                                   const float* row_temp, const float* row_top_p, const int* row_top_k,

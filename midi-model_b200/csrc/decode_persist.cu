@@ -78,7 +78,7 @@ struct PDQueue : PDRagged {
 // settings and RNG key; row b's new event j = pos + row_off[b] - row_first[b] draws hash(row_seed[b], 8 j + t, 0)
 struct PDRows : PDQueue {
     const float *row_temp, *row_top_p;   // [B]
-    const int* row_top_k;                // [B], 1..64
+    const int* row_top_k;                // [B], 1..128
     const unsigned long long* row_seed;  // [B]
     const int* row_first;                // [B]: seq index of the request's last prompt event
 };
@@ -694,6 +694,14 @@ __device__ __forceinline__ float rng_uniform(unsigned long long seed, unsigned l
     return smp::counter_uniform(seed, c, (unsigned long long)i);
 }
 
+// Row group g of a launch whose per-row phases run in NG groups of at most BM rows: its first row b0 and its row count
+// (<= 0: no such group).  With one group it is the whole batch.
+template <int BM, int NG>
+__device__ __forceinline__ int row_group(int g, int B, int& b0) {
+    b0 = g * BM;
+    return NG > 1 ? min(BM, B - b0) : B;
+}
+
 // =================================================================================================================
 // QUEUE (implies RAGGED): each row stops on its own.  A live row finishes at the commit of an event that is EOS or lands on
 // row_end[b]; a row that is not live commits nothing, takes no part in the token-step count and skips its attention items.
@@ -705,11 +713,17 @@ __device__ __forceinline__ float rng_uniform(unsigned long long seed, unsigned l
 // reads that word after the commit barrier and, when it is nonzero, leaves after this event's commit through the same
 // uniform exit as exit_on_done.  No CTA reads ctl itself: CTAs that saw different values would deadlock at the next
 // grid barrier.  The kernel only samples ctl, it never waits on host memory.
+// Batch: 1..16 rows; ROWS (and STREAM) take 1..32.  A ROWS launch of more than 16 rows runs with BM = 16 and every phase
+// that holds rows in shared memory or registers (the staging and norm blocks, the projections with their residual and
+// SwiGLU stores) runs twice, once per group of 16 rows, each time with the code of a 16-row launch: row b's arithmetic is
+// that of the same row at any batch.  Each group re-reads the phase's weights (the token-level ones from L2).  Attention,
+// the sampler CTAs (one per row) and the commit loop over all B rows directly.
 template <int BM, bool RAGGED, bool QUEUE = false, bool ROWS = false, bool STREAM = false>
 __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDArg<RAGGED, QUEUE, ROWS, STREAM> p) {
     static_assert(!QUEUE || RAGGED, "the queue kernel positions its rows through row_off");
     static_assert(!ROWS || QUEUE, "per-request rows are queue rows");
     static_assert(!STREAM || ROWS, "the streaming kernel is the per-request queue kernel");
+    constexpr int NG = (ROWS && BM == 16) ? 2 : 1;                                 // row groups (row_group)
     extern __shared__ __align__(16) uint8_t pd_smem[];
     const DD& d = p.d;
     const int B = d.batch, H = d.H;
@@ -721,7 +735,7 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
     float* q_all = s_red + 64;                                                      // [PD_WARPS][64]
     bf16* kn_all = reinterpret_cast<bf16*>(q_all + PD_WARPS * 64);                  // [PD_WARPS][64]
     bf16* vn_all = kn_all + PD_WARPS * 64;
-    int* cur_ev = reinterpret_cast<int*>(vn_all + PD_WARPS * 64);                   // [BM][8] event fed to the event-level stack
+    int* cur_ev = reinterpret_cast<int*>(vn_all + PD_WARPS * 64);                   // [B][8] event fed to the event-level stack
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ngw = gridDim.x * PD_WARPS;
     const int gw = warp * gridDim.x + blockIdx.x;      // interleave the CTAs: consecutive row pairs land on different SMs
@@ -755,40 +769,48 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
             // ---- norm + QKV
             prefetch_rows<false>(pre, w.qkv, H, 3 * H, gwv, lane, pol_stream);
             if (l > 0) { grid_sync(gb); prof.mark(PH_DOWN_O); }   // layer 0 reads only this CTA's copy of the event: no wait
-            if (warp < B) {
-                bf16* row = xs + (size_t)warp * H;
-                if (l == 0) {
-                    // embed_tokens(x).sum(-2) (midi_model.py:145-146): fp32 accumulate over the 8 ids, one rounding
-                    for (int v = lane; v < H / 8; v += 32) {
-                        uint4 er[PD_T];
+            for (int g = 0; g < NG; g++) {
+                int b0;
+                const int Bg = row_group<BM, NG>(g, B, b0);
+                if (NG > 1 && Bg <= 0) break;
+                if (NG > 1 && g > 0) __syncthreads();        // the previous group's projection has read xs
+                if (warp < Bg) {
+                    const int rb = b0 + warp;
+                    bf16* row = xs + (size_t)warp * H;
+                    if (l == 0) {
+                        // embed_tokens(x).sum(-2) (midi_model.py:145-146): fp32 accumulate over the 8 ids, one rounding
+                        for (int v = lane; v < H / 8; v += 32) {
+                            uint4 er[PD_T];
 #pragma unroll
-                        for (int t = 0; t < PD_T; t++) {      // the 8 embedding rows of the event: loads in flight together
-                            const int id = cur_ev[warp * PD_T + t];
-                            er[t] = make_uint4(0, 0, 0, 0);
-                            if (id >= 0 && id < d.V) er[t] = *reinterpret_cast<const uint4*>(d.emb_outer + (size_t)id * H + v * 8);
+                            for (int t = 0; t < PD_T; t++) {      // the 8 embedding rows of the event: loads in flight together
+                                const int id = cur_ev[rb * PD_T + t];
+                                er[t] = make_uint4(0, 0, 0, 0);
+                                if (id >= 0 && id < d.V) er[t] = *reinterpret_cast<const uint4*>(d.emb_outer + (size_t)id * H + v * 8);
+                            }
+                            float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll
+                            for (int t = 0; t < PD_T; t++) {
+                                float f[8];
+                                unpack8(er[t], f);
+#pragma unroll
+                                for (int j = 0; j < 8; j++) acc[j] += f[j];
+                            }
+                            *reinterpret_cast<uint4*>(row + v * 8) = pack8(acc);
                         }
-                        float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll
-                        for (int t = 0; t < PD_T; t++) {
-                            float f[8];
-                            unpack8(er[t], f);
-#pragma unroll
-                            for (int j = 0; j < 8; j++) acc[j] += f[j];
-                        }
-                        *reinterpret_cast<uint4*>(row + v * 8) = pack8(acc);
+                        __syncwarp();
+                        if (blockIdx.x == 0) copy_row_to_global(p.x + (size_t)rb * H, row, H, lane);
+                    } else {
+                        copy_row_from_global(row, p.x + (size_t)rb * H, H, lane);
                     }
                     __syncwarp();
-                    if (blockIdx.x == 0) copy_row_to_global(p.x + (size_t)warp * H, row, H, lane);
-                } else {
-                    copy_row_from_global(row, p.x + (size_t)warp * H, H, lane);
+                    norm_row_inplace(row, H, w.ln1, d.eps, lane);
                 }
-                __syncwarp();
-                norm_row_inplace(row, H, w.ln1, d.eps, lane);
+                __syncthreads();
+                prof.sub(PH_QKV_O, 0);
+                gemv_pairs<BM, false>(xs, H, w.qkv, H, 3 * H, Bg, nullptr, 0, p.qkv + (size_t)b0 * 3 * H, 3 * H, gwv, ngwv,
+                                      lane, pre, pol_stream);
+                prof.sub(PH_QKV_O, 1);
             }
-            __syncthreads();
-            prof.sub(PH_QKV_O, 0);
-            gemv_pairs<BM, false>(xs, H, w.qkv, H, 3 * H, B, nullptr, 0, p.qkv, 3 * H, gwv, ngwv, lane, pre, pol_stream);
-            prof.sub(PH_QKV_O, 1);
             // ---- RoPE + KV append + attention over positions 0..pos
             grid_sync(gb);
             prof.mark(PH_QKV_O);
@@ -809,34 +831,55 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
                 prof.mark(PH_ATT_O);
             }
             // ---- o_proj + residual
-            if (warp < B) copy_row_from_global(xs + (size_t)warp * H, p.attn + (size_t)warp * H, H, lane);
-            __syncthreads();
-            prof.sub(PH_OPROJ_O, 0);
-            gemv_pairs<BM, false>(xs, H, w.o, H, H, B, p.x, H, p.h, H, gwv, ngwv, lane, pre, pol_stream);
-            prof.sub(PH_OPROJ_O, 1);
+            for (int g = 0; g < NG; g++) {
+                int b0;
+                const int Bg = row_group<BM, NG>(g, B, b0);
+                if (NG > 1 && Bg <= 0) break;
+                if (NG > 1 && g > 0) __syncthreads();
+                if (warp < Bg) copy_row_from_global(xs + (size_t)warp * H, p.attn + (size_t)(b0 + warp) * H, H, lane);
+                __syncthreads();
+                prof.sub(PH_OPROJ_O, 0);
+                gemv_pairs<BM, false>(xs, H, w.o, H, H, Bg, p.x + (size_t)b0 * H, H, p.h + (size_t)b0 * H, H, gwv, ngwv, lane,
+                                      pre, pol_stream);
+                prof.sub(PH_OPROJ_O, 1);
+            }
             // ---- norm + gate|up + SwiGLU
             prefetch_rows<true>(pre, w.gu, H, d.I_outer, gwv, lane, pol_stream);
             grid_sync(gb);
             prof.mark(PH_OPROJ_O);
-            if (warp < B) {
-                copy_row_from_global(xs + (size_t)warp * H, p.h + (size_t)warp * H, H, lane);
-                __syncwarp();
-                norm_row_inplace(xs + (size_t)warp * H, H, w.ln2, d.eps, lane);
+            for (int g = 0; g < NG; g++) {
+                int b0;
+                const int Bg = row_group<BM, NG>(g, B, b0);
+                if (NG > 1 && Bg <= 0) break;
+                if (NG > 1 && g > 0) __syncthreads();
+                if (warp < Bg) {
+                    copy_row_from_global(xs + (size_t)warp * H, p.h + (size_t)(b0 + warp) * H, H, lane);
+                    __syncwarp();
+                    norm_row_inplace(xs + (size_t)warp * H, H, w.ln2, d.eps, lane);
+                }
+                __syncthreads();
+                prof.sub(PH_GU_O, 0);
+                gemv_pairs<BM, true>(xs, H, w.gu, H, d.I_outer, Bg, nullptr, 0, p.act + (size_t)b0 * d.I_outer, d.I_outer, gwv,
+                                     ngwv, lane, pre, pol_stream);
+                prof.sub(PH_GU_O, 1);
             }
-            __syncthreads();
-            prof.sub(PH_GU_O, 0);
-            gemv_pairs<BM, true>(xs, H, w.gu, H, d.I_outer, B, nullptr, 0, p.act, d.I_outer, gwv, ngwv, lane, pre, pol_stream);
-            prof.sub(PH_GU_O, 1);
             // ---- down + residual
             prefetch_rows<false>(pre, w.down, d.I_outer, H, gwv, lane, pol_stream);
             grid_sync(gb);
             prof.mark(PH_GU_O);
-            __syncthreads();
-            if (warp < B) copy_row_from_global(xs + (size_t)warp * d.I_outer, p.act + (size_t)warp * d.I_outer, d.I_outer, lane);
-            __syncthreads();
-            prof.sub(PH_DOWN_O, 0);
-            gemv_pairs<BM, false>(xs, d.I_outer, w.down, d.I_outer, H, B, p.h, H, p.x, H, gwv, ngwv, lane, pre, pol_stream);
-            prof.sub(PH_DOWN_O, 1);
+            for (int g = 0; g < NG; g++) {
+                int b0;
+                const int Bg = row_group<BM, NG>(g, B, b0);
+                if (NG > 1 && Bg <= 0) break;
+                __syncthreads();
+                if (warp < Bg)
+                    copy_row_from_global(xs + (size_t)warp * d.I_outer, p.act + (size_t)(b0 + warp) * d.I_outer, d.I_outer, lane);
+                __syncthreads();
+                prof.sub(PH_DOWN_O, 0);
+                gemv_pairs<BM, false>(xs, d.I_outer, w.down, d.I_outer, H, Bg, p.h + (size_t)b0 * H, H, p.x + (size_t)b0 * H, H,
+                                      gwv, ngwv, lane, pre, pol_stream);
+                prof.sub(PH_DOWN_O, 1);
+            }
         }
         // =============================== token-level stack: up to 8 steps =========================================
         int n_steps = PD_T;
@@ -865,30 +908,38 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
                     }
                     n_steps = min(PD_T, need);
                 }
-                if (warp < B) {
-                    bf16* row = xs + (size_t)warp * H;
-                    if (l == 0) {
-                        if (i == 0) {          // hidden = final norm of the event-level stack (hf :421), midi_model.py:126
-                            copy_row_from_global(row, p.x + (size_t)warp * H, H, lane);
+                for (int g = 0; g < NG; g++) {
+                    int b0;
+                    const int Bg = row_group<BM, NG>(g, B, b0);
+                    if (NG > 1 && Bg <= 0) break;
+                    if (NG > 1 && g > 0) __syncthreads();
+                    if (warp < Bg) {
+                        const int rb = b0 + warp;
+                        bf16* row = xs + (size_t)warp * H;
+                        if (l == 0) {
+                            if (i == 0) {          // hidden = final norm of the event-level stack (hf :421), midi_model.py:126
+                                copy_row_from_global(row, p.x + (size_t)rb * H, H, lane);
+                                __syncwarp();
+                                norm_row_inplace(row, H, d.outer_norm, d.eps, lane);
+                            } else {               // embedding of the token sampled at the previous step (midi_model.py:128)
+                                long long id = __ldcg(p.ev_t + (size_t)(i - 1) * B + rb);
+                                if (id < 0 || id >= d.V) id = 0;
+                                copy_row_from_global(row, d.emb_inner + (size_t)id * H, H, lane);
+                            }
                             __syncwarp();
-                            norm_row_inplace(row, H, d.outer_norm, d.eps, lane);
-                        } else {               // embedding of the token sampled at the previous step (midi_model.py:128)
-                            long long id = __ldcg(p.ev_t + (size_t)(i - 1) * B + warp);
-                            if (id < 0 || id >= d.V) id = 0;
-                            copy_row_from_global(row, d.emb_inner + (size_t)id * H, H, lane);
+                            if (blockIdx.x == 0) copy_row_to_global(p.x2 + (size_t)rb * H, row, H, lane);
+                        } else {
+                            copy_row_from_global(row, p.x2 + (size_t)rb * H, H, lane);
                         }
                         __syncwarp();
-                        if (blockIdx.x == 0) copy_row_to_global(p.x2 + (size_t)warp * H, row, H, lane);
-                    } else {
-                        copy_row_from_global(row, p.x2 + (size_t)warp * H, H, lane);
+                        norm_row_inplace(row, H, w.ln1, d.eps, lane);
                     }
-                    __syncwarp();
-                    norm_row_inplace(row, H, w.ln1, d.eps, lane);
+                    __syncthreads();
+                    prof.sub(PH_QKV_I, 0);
+                    gemv_pairs<BM, false>(xs, H, w.qkv, H, 3 * H, Bg, nullptr, 0, p.qkv + (size_t)b0 * 3 * H, 3 * H, gwv, ngwv,
+                                          lane, pre, pol_keep);
+                    prof.sub(PH_QKV_I, 1);
                 }
-                __syncthreads();
-                prof.sub(PH_QKV_I, 0);
-                gemv_pairs<BM, false>(xs, H, w.qkv, H, 3 * H, B, nullptr, 0, p.qkv, 3 * H, gwv, ngwv, lane, pre, pol_keep);
-                prof.sub(PH_QKV_I, 1);
                 grid_sync(gb);
                 prof.mark(PH_QKV_I);
                 inner_attention(p, l, i, B, gw, ngw, lane);
@@ -896,45 +947,75 @@ __global__ void __launch_bounds__(PD_THREADS, 1) decode_events_kernel(const PDAr
                 prefetch_rows<false>(pre, w.o, H, H, gwv, lane, pol_keep);
                 grid_sync(gb);
                 prof.mark(PH_ATT_I);
-                if (warp < B) copy_row_from_global(xs + (size_t)warp * H, p.attn + (size_t)warp * H, H, lane);
-                __syncthreads();
-                prof.sub(PH_OPROJ_I, 0);
-                gemv_pairs<BM, false>(xs, H, w.o, H, H, B, p.x2, H, p.h2, H, gwv, ngwv, lane, pre, pol_keep);
-                prof.sub(PH_OPROJ_I, 1);
+                for (int g = 0; g < NG; g++) {
+                    int b0;
+                    const int Bg = row_group<BM, NG>(g, B, b0);
+                    if (NG > 1 && Bg <= 0) break;
+                    if (NG > 1 && g > 0) __syncthreads();
+                    if (warp < Bg) copy_row_from_global(xs + (size_t)warp * H, p.attn + (size_t)(b0 + warp) * H, H, lane);
+                    __syncthreads();
+                    prof.sub(PH_OPROJ_I, 0);
+                    gemv_pairs<BM, false>(xs, H, w.o, H, H, Bg, p.x2 + (size_t)b0 * H, H, p.h2 + (size_t)b0 * H, H, gwv, ngwv,
+                                          lane, pre, pol_keep);
+                    prof.sub(PH_OPROJ_I, 1);
+                }
                 prefetch_rows<true>(pre, w.gu, H, d.I_inner, gwv, lane, pol_keep);
                 grid_sync(gb);
                 prof.mark(PH_OPROJ_I);
-                if (warp < B) {
-                    copy_row_from_global(xs + (size_t)warp * H, p.h2 + (size_t)warp * H, H, lane);
-                    __syncwarp();
-                    norm_row_inplace(xs + (size_t)warp * H, H, w.ln2, d.eps, lane);
+                for (int g = 0; g < NG; g++) {
+                    int b0;
+                    const int Bg = row_group<BM, NG>(g, B, b0);
+                    if (NG > 1 && Bg <= 0) break;
+                    if (NG > 1 && g > 0) __syncthreads();
+                    if (warp < Bg) {
+                        copy_row_from_global(xs + (size_t)warp * H, p.h2 + (size_t)(b0 + warp) * H, H, lane);
+                        __syncwarp();
+                        norm_row_inplace(xs + (size_t)warp * H, H, w.ln2, d.eps, lane);
+                    }
+                    __syncthreads();
+                    prof.sub(PH_GU_I, 0);
+                    gemv_pairs<BM, true>(xs, H, w.gu, H, d.I_inner, Bg, nullptr, 0, p.act + (size_t)b0 * d.I_inner, d.I_inner,
+                                         gwv, ngwv, lane, pre, pol_keep);
+                    prof.sub(PH_GU_I, 1);
                 }
-                __syncthreads();
-                prof.sub(PH_GU_I, 0);
-                gemv_pairs<BM, true>(xs, H, w.gu, H, d.I_inner, B, nullptr, 0, p.act, d.I_inner, gwv, ngwv, lane, pre, pol_keep);
-                prof.sub(PH_GU_I, 1);
                 prefetch_rows<false>(pre, w.down, d.I_inner, H, gwv, lane, pol_keep);
                 grid_sync(gb);
                 prof.mark(PH_GU_I);
-                if (warp < B) copy_row_from_global(xs + (size_t)warp * d.I_inner, p.act + (size_t)warp * d.I_inner, d.I_inner, lane);
-                __syncthreads();
-                prof.sub(PH_DOWN_I, 0);
-                gemv_pairs<BM, false>(xs, d.I_inner, w.down, d.I_inner, H, B, p.h2, H, p.x2, H, gwv, ngwv, lane, pre, pol_keep);
-                prof.sub(PH_DOWN_I, 1);
+                for (int g = 0; g < NG; g++) {
+                    int b0;
+                    const int Bg = row_group<BM, NG>(g, B, b0);
+                    if (NG > 1 && Bg <= 0) break;
+                    if (NG > 1 && g > 0) __syncthreads();
+                    if (warp < Bg)
+                        copy_row_from_global(xs + (size_t)warp * d.I_inner, p.act + (size_t)(b0 + warp) * d.I_inner, d.I_inner,
+                                             lane);
+                    __syncthreads();
+                    prof.sub(PH_DOWN_I, 0);
+                    gemv_pairs<BM, false>(xs, d.I_inner, w.down, d.I_inner, H, Bg, p.h2 + (size_t)b0 * H, H,
+                                          p.x2 + (size_t)b0 * H, H, gwv, ngwv, lane, pre, pol_keep);
+                    prof.sub(PH_DOWN_I, 1);
+                }
             }
             // ---- final norm + lm_head
             prefetch_rows<false>(pre, d.lm_head, H, d.V, gwv, lane, pol_keep);
             grid_sync(gb);
             prof.mark(PH_DOWN_I);
-            if (warp < B) {
-                copy_row_from_global(xs + (size_t)warp * H, p.x2 + (size_t)warp * H, H, lane);
-                __syncwarp();
-                norm_row_inplace(xs + (size_t)warp * H, H, d.inner_norm, d.eps, lane);
+            for (int g = 0; g < NG; g++) {
+                int b0;
+                const int Bg = row_group<BM, NG>(g, B, b0);
+                if (NG > 1 && Bg <= 0) break;
+                if (NG > 1 && g > 0) __syncthreads();
+                if (warp < Bg) {
+                    copy_row_from_global(xs + (size_t)warp * H, p.x2 + (size_t)(b0 + warp) * H, H, lane);
+                    __syncwarp();
+                    norm_row_inplace(xs + (size_t)warp * H, H, d.inner_norm, d.eps, lane);
+                }
+                __syncthreads();
+                prof.sub(PH_LMHEAD, 0);
+                gemv_pairs<BM, false>(xs, H, d.lm_head, H, d.V, Bg, nullptr, 0, p.logits + (size_t)b0 * d.pitch, d.pitch, gwv,
+                                      ngwv, lane, pre, pol_keep);
+                prof.sub(PH_LMHEAD, 1);
             }
-            __syncthreads();
-            prof.sub(PH_LMHEAD, 0);
-            gemv_pairs<BM, false>(xs, H, d.lm_head, H, d.V, B, nullptr, 0, p.logits, d.pitch, gwv, ngwv, lane, pre, pol_keep);
-            prof.sub(PH_LMHEAD, 1);
             // ---- sample (one CTA per row): temperature softmax, grammar range, top-p / top-k, draw
             grid_sync(gb);
             prof.mark(PH_LMHEAD);
@@ -1074,13 +1155,15 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, const int* r
     B200_CHECK_ARG(!ROWS || (rows != nullptr && rows->temp != nullptr && rows->top_p != nullptr && rows->top_k != nullptr &&
                              rows->seed != nullptr && rows->first != nullptr),
                    "decode_events_queue_rows: row_temp, row_top_p, row_top_k, row_seed and row_first required");
-    B200_CHECK_ARG(d.batch >= 1 && d.batch <= 16, "decode_events: batch %d outside 1..16", d.batch);
+    constexpr int max_batch = ROWS ? 32 : 16;           // per-request rows: two groups of 16 (decode_events_kernel)
+    B200_CHECK_ARG(d.batch >= 1 && d.batch <= max_batch, "decode_events: batch %d outside 1..%d", d.batch, max_batch);
     B200_CHECK_ARG(d.H == 1024 && d.nh_outer * 64 == d.H && d.nh_inner * 256 == d.H,
                    "decode_events: built for hidden 1024 (16 x 64 event-level heads, 4 x 256 token-level heads)");
     B200_CHECK_ARG(d.I_outer % 256 == 0 && d.I_inner % 256 == 0, "decode_events: MLP widths must be multiples of 256");
     B200_CHECK_ARG(d.V <= smp::SMP_MAXV && d.pitch >= d.V, "decode_events: vocabulary %d unsupported", d.V);
     B200_CHECK_ARG(d.page % 32 == 0, "decode_events: KV page size must be a multiple of 32");
-    B200_CHECK_ARG(d.temp > 0.f && d.top_k >= 1 && d.top_k <= 64, "decode_events: temperature must be positive and 1 <= top_k <= 64");
+    B200_CHECK_ARG(d.temp > 0.f && d.top_k >= 1 && d.top_k <= smp::FAST_MAXK,
+                   "decode_events: temperature must be positive and 1 <= top_k <= %d", smp::FAST_MAXK);
     if (n_events <= 0) return B200_OK;
     const WsLayout L = ws_layout(d);
     B200_CHECK_ARG(workspace != nullptr && workspace_bytes >= L.total && ((uintptr_t)workspace % 256 == 0),
@@ -1134,7 +1217,7 @@ int decode_events(const b200_decode_desc* desc, const int* row_off, const int* r
     }
     const int bm = d.batch <= 1 ? 1 : d.batch <= 2 ? 2 : d.batch <= 4 ? 4 : d.batch <= 8 ? 8 : 16;
     const size_t smem = (size_t)bm * p.k_max * 2 + (size_t)smp::SMP_MAXV * 8 + (PD_THREADS + 8) * 4 + 64 * 4 +
-                        PD_WARPS * 64 * (4 + 2 + 2) + (size_t)bm * PD_T * 4 + 64;
+                        PD_WARPS * 64 * (4 + 2 + 2) + (size_t)(bm > d.batch ? bm : d.batch) * PD_T * 4 + 64;   // cur_ev: [B][8]
     void* args[] = {(void*)&pk};
     const void* fn = nullptr;
     switch (bm) {

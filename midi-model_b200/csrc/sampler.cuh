@@ -183,19 +183,22 @@ __device__ int preselect_topk(float* s_p, int* s_i, int n, int top_k, int* s_his
 //   the softmax output, so the denominator covers every id); ids outside [lo, hi) or masked out get p = 0;
 //   candidates sorted by (p desc, id asc); only the first min(n, top_k) can be drawn (midi_model.py:157-159); top-p on the
 //   un-renormalised cumulative mass (:153-156); renormalise; draw with the uniform u (:161-164).
-// Fast path (top_k <= 64, the default is 20): the top-k set is found with a 4-pass radix select over the 16-bit bf16
+// Fast path (top_k <= 128, the default is 20): the top-k set is found with a 4-pass radix select over the 16-bit bf16
 // patterns of p (per-warp shared-memory histograms), ties at the k-th value are resolved towards the lowest ids with a
-// block-wide exclusive scan in id order, the <= 64 survivors are rank-sorted, one thread walks them.  ~17 block barriers
-// instead of the ~60 (and three serial single-thread scans) of compaction + two histogram passes + a 256-wide bitonic sort.
-// Results are identical to the general path (sample_tail on the compacted candidates), which remains for top_k > 64.
-// Scratch: s_p [SMP_MAXV] floats, s_i [SMP_MAXV] ints, s_cnt [NT + 8] ints, s_red [64] floats.
+// block-wide exclusive scan in id order, the <= 128 survivors are rank-sorted, one thread walks them.  ~17 block barriers
+// instead of the ~60 (and three serial single-thread scans) of compaction + two histogram passes + a full bitonic sort.
+// Results are identical to the general path (sample_tail on the compacted candidates), which remains for top_k > 128.
+// Scratch: s_p [SMP_MAXV] floats, s_i [SMP_MAXV] ints, s_cnt [NT + 8] ints, s_red [64] floats; NT >= FAST_MAXK.
 // ---------------------------------------------------------------------------------------------
+constexpr int FAST_MAXK = 128;                          // largest top_k of the fast path
+
 template <int NT, bool FAST_ONLY = false>
 __device__ int sample_logits_row(const bf16* __restrict__ logits, int V, float temp, float top_p, int top_k, int lo, int hi,
                                  const unsigned char* __restrict__ mrow, float u, float* s_p, int* s_i, int* s_cnt,
                                  float* s_red, bool coherent_loads) {
     constexpr int NW = NT / 32;
     constexpr int PER = SMP_MAXV / NT;                 // ids per thread (consecutive: thread t owns [t * PER, t * PER + PER))
+    static_assert(NT >= FAST_MAXK && 4 * NW * 16 + 4 * FAST_MAXK <= SMP_MAXV, "fast path: rank sort or survivors do not fit");
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     float mx = -INFINITY;
     {
@@ -238,7 +241,7 @@ __device__ int sample_logits_row(const bf16* __restrict__ logits, int V, float t
     for (int w = 0; w < NW; w++) sum += s_red[32 + w];
     const float inv = 1.f / sum;
 
-    if (!FAST_ONLY && top_k > 64) {                    // general path
+    if (!FAST_ONLY && top_k > FAST_MAXK) {             // general path
         __syncthreads();
         for (int i = tid; i < V; i += NT) {
             bool ok = (i >= lo && i < hi);
@@ -345,10 +348,11 @@ __device__ int sample_logits_row(const bf16* __restrict__ logits, int V, float t
     for (int w = 0; w < warp; w++) base += ctl[8 + w];
     const int excl = base + incl - packed;
     int gt_before = excl & 0xFFFF, eq_before = excl >> 16;
-    float* sel_p = s_red;                               // [64] (block reductions are done)
-    int* sel_i = s_cnt + 8 + NW + 8;                    // [64]
-    float* srt_p = reinterpret_cast<float*>(s_cnt + 8 + NW + 8 + 64);   // [64]
-    int* srt_i = s_cnt + 8 + NW + 8 + 128;              // [64]
+    // survivors in s_i past the digit histograms (read for the last time before the scan's barrier)
+    float* sel_p = reinterpret_cast<float*>(hist + 4 * NW * 16);          // [FAST_MAXK]
+    int* sel_i = hist + 4 * NW * 16 + FAST_MAXK;                          // [FAST_MAXK]
+    float* srt_p = reinterpret_cast<float*>(hist + 4 * NW * 16 + 2 * FAST_MAXK);   // [FAST_MAXK]
+    int* srt_i = hist + 4 * NW * 16 + 3 * FAST_MAXK;                      // [FAST_MAXK]
 #pragma unroll
     for (int j = 0; j < PER; j++) {
         const unsigned k = key[j];

@@ -456,9 +456,12 @@ class GraphGenerator:
 
     # ------------------------------------------------------------------ persistent kernel (csrc/decode_persist.cu)
     def persistent_ok(self) -> bool:
+        """Whether the persistent kernel runs this loop's current call: at most 32 slots in per-request mode (the `_rows`
+        kernels run their rows in groups of 16), 16 otherwise, every top_k in 1..128, and a model it is built for."""
         c1, c2 = self.outer.eng.cfg, self.inner.eng.cfg
         top_ks = self.req_top_k if self.rows else [self.top_k]
-        return (self.B <= 16 and all(1 <= k <= 64 for k in top_ks) and c1.hidden == 1024 and c2.hidden == 1024 and c1.head_dim == 64 and c2.head_dim == 256
+        return (self.B <= (32 if self.rows else 16) and all(1 <= k <= 128 for k in top_ks)
+                and c1.hidden == 1024 and c2.hidden == 1024 and c1.head_dim == 64 and c2.head_dim == 256
                 and c1.inner % 256 == 0 and c2.inner % 256 == 0 and self.T == 8 and self.kv1.page % 32 == 0)
 
     def _persistent(self):
@@ -784,7 +787,7 @@ class GraphGenerator:
         `settings` (per-request mode): one (temp, top_p, top_k, seed, denied token ids) per request, with temp > 0,
         0 < top_p <= 1, top_k >= 1 (checked by the caller).  Request i then samples with its own settings and mask row and
         draws what a batch-1 loop seeded `seed` draws, through the `_rows` entries; the persistent kernel needs every top_k
-        <= 64.  Without it, every slot shares this loop's settings, seed stream and mask.
+        <= 128 and at most 32 slots.  Without it, every slot shares this loop's settings, seed stream and mask.
 
         Requests with equal prompts of at least 65 events (`_share_keys`) share the KV pages of the prompt's whole pages
         (SharedPages): the first one resident is prefilled, a later one only copies the prompt's tail page from a live

@@ -17,11 +17,11 @@ has the same prompt), and the rows are rebased (pos = the largest live position,
 persistent kernel each launch is `b200_decode_events_queue_stream` over at most 64 events, with exit_on_done while requests
 wait; the worker polls the pinned `committed` array about every millisecond and hands each new event to its request.  The
 launch also ends when the host sets `ctl`: a request submitted while a slot is free, a cancellation, or close.  Where the
-persistent kernel does not apply (more than 16 slots, a live request with top_k > 64, or a model it is not built for) the
+persistent kernel does not apply (more than 32 slots, a live request with top_k > 128, or a model it is not built for) the
 server runs the graph loop (or the host-issued one, B200_GENERATE=nograph), one event per step, and streams after every
 event.
 
-Guarantee: on the persistent kernel (batch_size <= 16, every top_k <= 64), a request that is not cancelled streams bit for
+Guarantee: on the persistent kernel (batch_size <= 32, every top_k <= 128), a request that is not cancelled streams bit for
 bit the events of generate_stream(prompt, batch_size=1, max_len=L + max_new, temp, top_p, top_k, grammar options,
 generator=g), g being a generator whose first draw is the request's seed, for prompts of at most 4096 events; whatever the
 arrival times, submitting threads, slots, cancellations and other requests.  A cancelled request streams a prefix of those
@@ -419,7 +419,7 @@ class GenerateServer:
                 self._launch_stream(gg, n, waiting, live)
                 state = torch.cat([gg.pos, gg.row_last]).cpu()
             else:
-                # the graph loop, or for a persistent server's event with a live top_k > 64 request its launches issued
+                # the graph loop, or for a persistent server's event with a live top_k > 128 request its launches issued
                 # from the host (a graph captured now would have to run an event of its own)
                 if self._graph:
                     gg.graph_queue_rows.replay()

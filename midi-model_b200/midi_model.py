@@ -1140,8 +1140,8 @@ class MIDIModel(PreTrainedModel):
         list of one entry (None or a list of channels) per request: request i samples with its own settings and grammar
         options and draws, at its new event j and token step t, hash(seeds[i], 8 j + t, 0) -- the draw of generate's loop
         at batch 1 seeded seeds[i].  Without `seeds`, seed i is torch.randint(0, 2**62, (1,), generator=generator), drawn
-        once per request in input order.  On the persistent kernel (B200_GENERATE=persist, batch_size <= 16, every top_k
-        <= 64) request i's attention is also summed as at batch 1, so its result is bit for bit
+        once per request in input order.  On the persistent kernel (B200_GENERATE=persist, batch_size <= 32, every top_k
+        <= 128) request i's attention is also summed as at batch 1, so its result is bit for bit
         generate(prompt_i, batch_size=1, max_len=L_i + max_new_i, temp_i, top_p_i, top_k_i, generator=g_i), g_i being a
         generator whose first draw is seeds[i] (with grammar options: the events generate_stream yields at batch 1, for
         prompts of at most 4096 events), whatever batch_size, slot, order and other requests.  On the graph and
