@@ -62,6 +62,25 @@ int b200_batch_to_xy_i16(const void* batch, int B, int S1, int T, long long* x, 
    column.  No other batch row is read. */
 int b200_batch_to_xy_packed_i16(const void* batch, int T, const int* src, int n_rows, int pad_id, long long* x, long long* y,
                                 cudaStream_t s);
+/* train.py's augmentation (MIDITokenizerV2.augment, midi_tokenizer.py:1023-1102; track shift 0 as train.py draws it) of
+   an int16 batch [B, L, T] in place (T >= 7, the v2 token layout).  aug is device int32 [B, B200_AUG_COLS], one row per
+   sample: skip (non-zero: the sample is left untouched -- the reference's abort when a non-drum note leaves 0..127, or no
+   augmentation at all), the pitch / velocity / cc value / bpm / channel shifts, and the 128-bit mask of the file's
+   drum-only tracks (bit tr % 32 of word tr / 32), whose key signatures get sf = 0.  Rows whose token 0 is not an event id
+   are untouched. */
+#define B200_AUG_SKIP 0
+#define B200_AUG_PITCH 1
+#define B200_AUG_VELOCITY 2
+#define B200_AUG_CC_VALUE 3
+#define B200_AUG_BPM 4
+#define B200_AUG_CHANNEL 5
+#define B200_AUG_DRUM 6
+#define B200_AUG_COLS 10
+typedef struct b200_augment_ids {
+    int note, patch_change, control_change, set_tempo, key_signature;        /* event ids */
+    int track, channel, pitch, velocity, controller, value, bpm, sf, mi;     /* first id of each parameter */
+} b200_augment_ids;
+int b200_augment_i16(void* batch, int B, int L, int T, const int* aug, const b200_augment_ids* ids /*host*/, cudaStream_t s);
 size_t b200_embed_bwd_workspace_bytes(int n_ids, int V, int H);
 /* id i reads gradient row (i / per_row) * row_stride + (i % per_row) * row_inner + row_off; pad row gets 0 */
 int b200_embed_bwd(const long long* ids, int n_ids, const void* dout, void* dtable, int V, int H, int per_row,

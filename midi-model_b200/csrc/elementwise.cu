@@ -5,6 +5,7 @@
 // accesses, one 128-thread CTA per row (rows are 2 KB at hidden=1024), grids sized in rows.
 #include "common.cuh"
 #include "rope.cuh"
+#include "../../include/midi_b200.h"
 
 namespace {
 
@@ -723,6 +724,70 @@ extern "C" int b200_batch_to_xy_packed_i16(const void* batch, int T, const int* 
     if (n == 0) return B200_OK;
     batch_to_xy_packed_kernel<<<grid_for((size_t)n, 256), 256, 0, stream>>>((const short*)batch, src, x, y, n, T, pad_id);
     B200_CHECK_LAUNCH("batch_to_xy_packed");
+    return B200_OK;
+}
+
+// train.py's augmentation (MIDITokenizerV2.augment, midi_tokenizer.py:1023-1102) of a cropped int16 batch, in place, one
+// thread per token row.  The host draws the shifts and decides the two rules that need the whole file (corpus metadata):
+// whether any non-drum note would leave 0..127 (then the sample is skipped entirely) and which tracks are drum-only.
+// Python's % is floored and the pitch / sf operands can be negative, hence floor_mod.  Zero shifts still clamp.
+namespace {
+__device__ __forceinline__ int floor_mod(int a, int m) {
+    const int r = a % m;
+    return r < 0 ? r + m : r;
+}
+
+__device__ __forceinline__ int clamp_i(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
+
+__global__ void augment_kernel(short* __restrict__ b, const int* __restrict__ aug, long long n_rows, int L, int T,
+                               b200_augment_ids id) {
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n_rows; r += (long long)gridDim.x * blockDim.x) {
+        const int* a = aug + (r / L) * B200_AUG_COLS;
+        if (a[B200_AUG_SKIP]) continue;
+        short* t = b + r * T;
+        const int ev = t[0];
+        if (ev == id.note || ev == id.patch_change || ev == id.control_change) {
+            // every v2 event with a channel has it at position 4
+            const int s = a[B200_AUG_CHANNEL];
+            const int c0 = t[4] - id.channel;
+            int c = floor_mod(c0 + s, 16);
+            if (c0 == 9) c = 9;
+            else if (c == 9) c = floor_mod(9 + s, 16);
+            t[4] = (short)(id.channel + c);
+            if (ev == id.note) {
+                int p = t[5] - id.pitch;
+                if (c0 != 9) p += a[B200_AUG_PITCH];
+                t[5] = (short)(id.pitch + p);
+                t[6] = (short)(id.velocity + clamp_i(t[6] - id.velocity + a[B200_AUG_VELOCITY], 1, 127));
+            } else if (ev == id.control_change) {
+                const int cc = t[5] - id.controller;
+                if (cc == 1 || cc == 2 || cc == 7 || cc == 11)
+                    t[6] = (short)(id.value + clamp_i(t[6] - id.value + a[B200_AUG_CC_VALUE], 1, 127));
+            }
+        } else if (ev == id.set_tempo) {
+            t[4] = (short)(id.bpm + clamp_i(t[4] - id.bpm + a[B200_AUG_BPM], 1, 383));
+        } else if (ev == id.key_signature) {
+            const int tr = t[3] - id.track;
+            const int mi = t[5] - id.mi;
+            const int k = floor_mod(floor_mod((t[4] - id.sf - 7) * 7, 12) + a[B200_AUG_PITCH], 12);   // sf2key, shift
+            int sf = (k * 7) % 12;                                                                    // key2sf
+            if (sf > 6 || (mi == 1 && sf >= 5)) sf -= 12;
+            if (tr >= 0 && tr < 128 && ((unsigned)a[B200_AUG_DRUM + (tr >> 5)] >> (tr & 31) & 1u)) sf = 0;
+            t[4] = (short)(id.sf + sf + 7);
+        }
+    }
+}
+}   // namespace
+
+extern "C" int b200_augment_i16(void* batch, int B, int L, int T, const int* aug, const b200_augment_ids* ids,
+                                cudaStream_t stream) {
+    B200_CHECK_ARG(B >= 0 && L >= 0 && T >= 7, "augment: bad shape (%d, %d, %d)", B, L, T);
+    B200_CHECK_ARG(ids != nullptr, "augment: null id table");
+    const long long n = (long long)B * L;
+    if (n == 0) return B200_OK;
+    B200_CHECK_ARG(batch && aug, "augment: null pointer");
+    augment_kernel<<<grid_for((size_t)n, 256), 256, 0, stream>>>((short*)batch, aug, n, L, T, *ids);
+    B200_CHECK_LAUNCH("augment");
     return B200_OK;
 }
 

@@ -18,6 +18,9 @@ batches, `b200_batch_to_xy_packed_i16` packs the rows that have a target):
     lengths = [len(s) for s in samples]
     batch = collate(samples, pad_id)
     loss = model.training_loss(batch.to("cuda"), lengths=lengths)     # lengths stay on the host
+
+A pre-tokenised corpus (midi_b200/corpus.py) yields `(tokens, lengths, aug)` tuples; `augment_(tokens, aug)` then runs
+train.py's augmentation on the device batch.
 """
 from __future__ import annotations
 
@@ -57,10 +60,13 @@ class Prefetcher:
 
     for batch in Prefetcher(loader, device):         # batch: int16 [B, L, T] on `device`
         loss = model.training_loss(batch)
+
+    An item may also be a tuple, such as the `(tokens, lengths, aug)` of `Corpus.batches`: each tensor in it is copied,
+    everything else (`lengths`, a list that stays on the host) is passed through, and the tuple is yielded.
     """
 
-    def __init__(self, batches: Iterable[torch.Tensor], device, depth: int = 2):
-        self.it: Iterator[torch.Tensor] = iter(batches)
+    def __init__(self, batches: Iterable, device, depth: int = 2):
+        self.it: Iterator = iter(batches)
         self.device = torch.device(device)
         self.depth = max(1, int(depth))
         self.copy_stream = torch.cuda.Stream(device=self.device)
@@ -68,25 +74,57 @@ class Prefetcher:
 
     def _issue(self) -> bool:
         try:
-            host = next(self.it)
+            item = next(self.it)
         except StopIteration:
             return False
-        if not host.is_pinned():
-            host = host.pin_memory()
+        parts = item if isinstance(item, tuple) else (item,)
+        host = tuple(p.pin_memory() if isinstance(p, torch.Tensor) and not p.is_pinned() else p for p in parts)
         with torch.cuda.stream(self.copy_stream):
-            dev = host.to(self.device, non_blocking=True)
+            dev = tuple(p.to(self.device, non_blocking=True) if isinstance(p, torch.Tensor) else p for p in host)
             ev = torch.cuda.Event()
             ev.record(self.copy_stream)
-        self.queue.append((dev, ev, host))          # `host` stays referenced until its copy has been consumed
+        self.queue.append((dev, ev, host, isinstance(item, tuple)))   # `host` stays referenced until its copy is consumed
         return True
 
     def __iter__(self):
         while len(self.queue) < self.depth and self._issue():
             pass
         while self.queue:
-            dev, ev, _host = self.queue.pop(0)
+            dev, ev, _host, is_tuple = self.queue.pop(0)
             cur = torch.cuda.current_stream(self.device)
             cur.wait_event(ev)
-            dev.record_stream(cur)                  # allocated on the copy stream, consumed on the compute stream
+            for p in dev:
+                if isinstance(p, torch.Tensor):
+                    p.record_stream(cur)            # allocated on the copy stream, consumed on the compute stream
             self._issue()
-            yield dev
+            yield dev if is_tuple else dev[0]
+
+
+_AUG_IDS = None
+
+
+def augment_ids(tok=None):
+    """The `lib.AugmentIds` of the v2 token layout (event ids and first parameter ids)."""
+    from . import lib
+    from .tokenizer_tables import TokenizerTables
+    tok = tok or TokenizerTables("v2")
+    if tok.version != "v2":
+        raise lib.B200Error(f"augment: the {tok.version} tokenizer is not supported (its augment differs); v2 only")
+    ev, pid = tok.event_ids, tok.parameter_ids
+    return lib.AugmentIds(*(ev[e] for e in ("note", "patch_change", "control_change", "set_tempo", "key_signature")),
+                          *(pid[p][0] for p in ("track", "channel", "pitch", "velocity", "controller", "value", "bpm", "sf",
+                                                "mi")))
+
+
+def augment_(batch: torch.Tensor, aug: torch.Tensor) -> torch.Tensor:
+    """train.py's `MIDITokenizerV2.augment` of every sample of a device int16 batch `[B, L, T]`, in place, with the draws
+    of `aug` (int32 `[B, 10]` on the same device, as `Corpus.batches` yields it).  Returns `batch`.
+
+    The corpus metadata carries the two rules that depend on the whole file (the abort when a pitch shift moves a non-drum
+    note out of 0..127, and sf = 0 on drum-only tracks), so augmenting a crop gives, row for row, the crop of the
+    reference's augmented file.  Pad, BOS and EOS rows are left alone."""
+    global _AUG_IDS
+    from . import ops
+    if _AUG_IDS is None:
+        _AUG_IDS = augment_ids()
+    return ops.augment_(batch, aug, _AUG_IDS)

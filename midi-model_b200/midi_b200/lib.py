@@ -30,6 +30,7 @@ SIGNATURES = {
     "b200_inner_input_rows_bwd_hidden": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "b200_batch_to_xy_i16": (i32, [vp, i32, i32, i32, vp, vp, vp]),
     "b200_batch_to_xy_packed_i16": (i32, [vp, i32, vp, i32, i32, vp, vp, vp]),
+    "b200_augment_i16": (i32, [vp, i32, i32, i32, vp, vp, vp]),
     "b200_embed_bwd_workspace_bytes": (sz, [i32, i32, i32]),
     "b200_embed_bwd": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, sz, vp]),
     "b200_rmsnorm_fwd": (i32, [vp, vp, vp, vp, i32, i32, f32, vp]),
@@ -107,6 +108,15 @@ class DecodeDesc(C.Structure):
                 ("rng_state", vp), ("dense_mask", vp), ("lut", vp),
                 ("n_event_types", i32), ("eos_id", i32), ("pad_id", i32),
                 ("temp", f32), ("top_p", f32), ("top_k", i32), ("batch", i32), ("prof", vp)]
+
+
+AUG_SKIP, AUG_PITCH, AUG_VELOCITY, AUG_CC_VALUE, AUG_BPM, AUG_CHANNEL, AUG_DRUM, AUG_COLS = 0, 1, 2, 3, 4, 5, 6, 10
+
+
+class AugmentIds(C.Structure):
+    """b200_augment_ids of include/midi_b200.h (field for field): event ids and the first id of each parameter."""
+    _fields_ = [(n, i32) for n in ("note", "patch_change", "control_change", "set_tempo", "key_signature", "track",
+                                   "channel", "pitch", "velocity", "controller", "value", "bpm", "sf", "mi")]
 
 
 class B200Error(RuntimeError):

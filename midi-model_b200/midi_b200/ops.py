@@ -5,6 +5,7 @@ Only shapes, pointer extraction and workspace management live here; the arithmet
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 from typing import Optional
 
@@ -115,6 +116,22 @@ def batch_to_xy_packed(batch: torch.Tensor, src: torch.Tensor, pad_id: int):
     lib.call("b200_batch_to_xy_packed_i16", batch.data_ptr(), T, src.data_ptr(), src.shape[0], int(pad_id), x.data_ptr(),
              y.data_ptr(), lib.stream())
     return x, y
+
+
+def augment_(batch: torch.Tensor, aug: torch.Tensor, ids) -> torch.Tensor:
+    """train.py's augmentation of an int16 [B, L, T] batch in place; aug int32 [B, lib.AUG_COLS] on the batch's device
+    (include/midi_b200.h), ids a `lib.AugmentIds`."""
+    lib.require_cuda(batch, "augment_: batch")
+    lib.require_cuda(aug, "augment_: aug")
+    if batch.dtype != torch.int16 or batch.dim() != 3 or not batch.is_contiguous():
+        raise lib.B200Error(f"augment_: expected a contiguous int16 [B, L, T] batch, got {batch.dtype} {tuple(batch.shape)}")
+    B, L, T = batch.shape
+    if aug.dtype != torch.int32 or tuple(aug.shape) != (B, lib.AUG_COLS) or not aug.is_contiguous() \
+            or aug.device != batch.device:
+        raise lib.B200Error(f"augment_: aug must be contiguous int32 [{B}, {lib.AUG_COLS}] on {batch.device}, got "
+                            f"{aug.dtype} {tuple(aug.shape)} on {aug.device}")
+    lib.call("b200_augment_i16", batch.data_ptr(), B, L, T, aug.data_ptr(), C.byref(ids), lib.stream())
+    return batch
 
 
 def embed_bwd(ids: torch.Tensor, dout: torch.Tensor, dtable: torch.Tensor, per_row: int, row_stride: int, row_inner: int,
