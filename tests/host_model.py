@@ -1,5 +1,6 @@
-"""Shared fixtures of the CPU tests that run the fused trainer's host logic over the mock kernel layer
-(tests/mock_kernels.py): a tiny model, synthetic batches, LoRA set-up, gradient read-out and the oracle's autograd."""
+"""Shared fixtures of the CPU tests that run host logic over the mock kernel layer (tests/mock_kernels.py): a tiny model,
+synthetic batches, LoRA set-up, gradient read-out and the oracle's autograd for the fused trainer; the installed layer, a
+generate loop and prompts for the generate tests."""
 import torch
 
 BF = torch.bfloat16
@@ -12,6 +13,22 @@ def tiny_model(seed=0):
     torch.manual_seed(seed)
     cfg = mm.MIDIModelConfig.get_config("v2", True, n_layer=4, n_head=4, n_embd=256, n_inner=512)
     return mm.MIDIModel(cfg).to(BF).train()
+
+
+def generate_model(monkeypatch, loop):
+    """The tiny model in eval mode over the mock kernel layer, generating on `loop` (B200_GENERATE): "nograph" for the
+    host-issued loop, "persist" for the persistent kernel's launch protocol."""
+    import mock_kernels
+    mock_kernels.install(monkeypatch, persist=loop == "persist")
+    monkeypatch.setenv("B200_GENERATE", loop)
+    return tiny_model(0).eval()
+
+
+def prompts(model, lengths, seed):
+    """Prompts of `lengths` events (int64 [L, T] arrays), cut from one synthetic batch."""
+    from midi_b200.synth import synth_batch
+    batch = synth_batch(model.tokenizer, len(lengths), max(lengths), seed=seed).numpy()
+    return [batch[i, :L] for i, L in enumerate(lengths)]
 
 
 def make_batch(model, B=2, S1=10, seed=1, pad_tail=0, lengths=None):

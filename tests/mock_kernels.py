@@ -3,7 +3,9 @@ so that the HOST LOGIC of the engine -- the per-layer forward / backward schedul
 they land in the flat buffers, the LoRA composition, the optimizer span, the autograd Functions -- runs in the CPU test
 suite and is compared with the oracle's autograd.  It is installed by monkeypatching inside a test and nowhere else; the
 product has no such switch (test_no_cpu_fallback).  It says nothing about the CUDA kernels themselves: those are compared
-with the oracle on the GPU (tests/gpu_checks.py).
+with the oracle on the GPU (tests/gpu_checks.py).  The stand-ins of the generate path's C-ABI entries are in
+tests/mock_decode.py; `install` is the one entry point of the whole layer, for the trainer's tests and the generate tests
+alike.
 
 Semantics follow the kernels' contracts in include/midi_b200.h: bf16 storage, fp32 arithmetic, one rounding per stored
 value; packed layouts, row pitches and in-place behaviour as the engine relies on them.
@@ -133,13 +135,21 @@ def _rot(x, cos, sin, backward):
     return torch.cat((x1 * cos + x2 * sin, x2 * cos - x1 * sin), -1)
 
 
-def rope_qk_(qkv, cos, sin, S, H, D, backward=False, pos0=0, pos0_dev=None):
+def rope_qk_(qkv, cos, sin, S, H, D, backward=False, pos0=0, pos0_dev=None, row_off=None):
     rows = qkv.shape[0]
     pos = pos0 + torch.arange(rows) % S
+    if pos0_dev is not None:                                            # the device-side position base
+        pos = pos + int(pos0_dev.reshape(-1)[0])
+    if row_off is not None:                                             # ragged: row b's S rows at + row_off[b]
+        pos = pos + row_off.long().repeat_interleave(S)
     c, s = cos.float()[pos][:, None], sin.float()[pos][:, None]          # [rows, 1, D/2]
     for col0 in (0, H):
         blk = _f(qkv[:, col0:col0 + H]).view(rows, H // D, D)
         qkv[:, col0:col0 + H] = _rot(blk, c, s, backward).reshape(rows, H).to(BF)
+
+
+def rope_qk_ragged_(qkv, cos, sin, S, H, D, row_off, pos0=0, pos0_dev=None):
+    rope_qk_(qkv, cos, sin, S, H, D, pos0=pos0, pos0_dev=pos0_dev, row_off=row_off)
 
 
 def _segments(tiles):
@@ -320,132 +330,42 @@ def ce_bwd_(logits, targets, lse, lac, V, ignore_index, grad_scale=1.0, grad_sca
 
 
 
-# ------------------------------------------------------------------ decode-step entry points (pointer level)
-def _bfmat(ptr, rows, cols, ld):
-    t = _from_ptr(ptr, (rows - 1) * ld + cols, BF)
-    return torch.as_strided(t, (rows, cols), (ld, 1))
+# ------------------------------------------------------------------ raw C-ABI calls the host code issues itself
+def _inner_input_bwd_hidden(dx_ptr, dh_ptr, n_events, Tin, H, _s):
+    dx = _from_ptr(dx_ptr, n_events * Tin * H, BF).view(n_events, Tin, H)
+    _from_ptr(dh_ptr, n_events * H, BF).view(n_events, H).copy_(dx[:, 0])
 
 
-def _pool(ptr, batch, max_pages, nh, page, D):
-    return _from_ptr(ptr, batch * max_pages * nh * page * D, BF).view(batch * max_pages, nh, page, D)
+def _grad_clip_coef(gptr, n, max_norm, nc_ptr, _a, _b, _s):
+    g = _from_ptr(gptr, n, BF).float()
+    norm = float(g.pow(2).sum().sqrt())
+    nc = _from_ptr(nc_ptr, 2, torch.float32)
+    nc[0] = norm
+    nc[1] = min(1.0, max_norm / (norm + 1e-6))
 
 
-def _gemv_bf16(x, W, res, y, B, N, K, ldx, ldw, ldr, ldy, _s):
-    acc = _f(_bfmat(x, B, K, ldx)) @ _f(_bfmat(W, N, K, ldw)).t()
-    if res:
-        acc = acc.to(BF).float() + _f(_bfmat(res, B, N, ldr))
-    out = _bfmat(y, B, ldy if ldy >= N else N, ldy)
-    out[:, :N] = acc.to(BF)
-    out[:, N:] = 0
+def _adamw_step(pptr, gptr, mptr, vptr, fptr, n, lr, b1, b2, eps, wd, step, nc_ptr, _s):
+    p, g = _from_ptr(pptr, n, BF), _from_ptr(gptr, n, BF).float()
+    m, v = _from_ptr(mptr, n, torch.float32), _from_ptr(vptr, n, torch.float32)
+    flags = _from_ptr(fptr, (n + 255) // 256, torch.uint8)
+    g = g * float(_from_ptr(nc_ptr, 2, torch.float32)[1])
+    m.mul_(b1).add_(g, alpha=1 - b1)
+    v.mul_(b2).addcmul_(g, g, value=1 - b2)
+    decay = torch.where(flags.repeat_interleave(256)[:n] != 0, torch.ones(()), torch.tensor(1.0 - lr * wd))
+    upd = (m / (1 - b1 ** step)) / ((v / (1 - b2 ** step)).sqrt() + eps)
+    p.copy_((p.float() * decay - lr * upd).to(BF))
 
 
-def _gemv_fused(x, ids, ids_stride, table, V, norm_w, eps, W, res, y, B, N_out, K, ldx, ldw, ldr, ldy, swiglu_, _s):
-    assert not ids, "mock kernel layer: the ids/table input of b200_gemv_fused is used by the graph loop only"
-    h = _bfmat(x, B, K, ldx).clone()
-    if norm_w:
-        h = rmsnorm(h, _from_ptr(norm_w, K, BF), eps)
-    rows_w = 2 * N_out if swiglu_ else N_out
-    z = (_f(h) @ _f(_bfmat(W, rows_w, K, ldw)).t())
-    if swiglu_:
-        z = _f(swiglu(z.to(BF)))
-    if res:
-        z = z.to(BF).float() + _f(_bfmat(res, B, N_out, ldr))
-    _bfmat(y, B, N_out, ldy).copy_(z.to(BF))
+CALLS = {"b200_inner_input_bwd_hidden": _inner_input_bwd_hidden, "b200_grad_clip_coef": _grad_clip_coef,
+         "b200_adamw_step": _adamw_step}
 
 
-def _dev_int(ptr):
-    return int(_from_ptr(ptr, 1, torch.int32)[0]) if ptr else 0
-
-
-def _kv_append(qkv, k_pool, v_pool, bt, max_pages, page, nh, D, batch, s_new, pos0, pos0_dev, ld, _s):
-    pos0 = pos0 + _dev_int(pos0_dev)
-    H = nh * D
-    q = _bfmat(qkv, batch * s_new, 3 * H, ld)
-    kp, vp = _pool(k_pool, batch, max_pages, nh, page, D), _pool(v_pool, batch, max_pages, nh, page, D)
-    table = _from_ptr(bt, batch * max_pages, torch.int32).view(batch, max_pages)
-    for b in range(batch):
-        for i in range(s_new):
-            pos = pos0 + i
-            pg = int(table[b, pos // page])
-            row = q[b * s_new + i]
-            kp[pg, :, pos % page] = row[H:2 * H].view(nh, D)
-            vp[pg, :, pos % page] = row[2 * H:].view(nh, D)
-
-
-def _gather_kv(pool, table, b, n_pos, page):
-    pages = [pool[int(table[b, j])] for j in range((n_pos + page - 1) // page)]          # each [nh, page, D]
-    return torch.cat(pages, 1)[:, :n_pos]                                               # [nh, n_pos, D]
-
-
-def _attend(q, k, v, scale):
-    # q [nh, D], k/v [nh, T, D] (fp32) -> [nh, D], probabilities rounded to bf16 before P.V like the kernels
-    p = torch.softmax((k @ q[:, :, None])[:, :, 0] * scale, -1)
-    return (p.to(BF).float()[:, None, :] @ v)[:, 0]
-
-
-def _attn_decode(q, k_pool, v_pool, bt, max_pages, page, out, batch, s_q, nh, D, past, past_dev, max_T, ldq, ldo, scale,
-                 n_split, _ws, _wsb, _s):
-    past = past + _dev_int(past_dev)
-    H = nh * D
-    qm, om = _bfmat(q, batch * s_q, H, ldq), _bfmat(out, batch * s_q, H, ldo)
-    kp, vp = _pool(k_pool, batch, max_pages, nh, page, D), _pool(v_pool, batch, max_pages, nh, page, D)
-    table = _from_ptr(bt, batch * max_pages, torch.int32).view(batch, max_pages)
-    for b in range(batch):
-        for i in range(s_q):
-            n_pos = past + i + 1
-            k, v = _f(_gather_kv(kp, table, b, n_pos, page)), _f(_gather_kv(vp, table, b, n_pos, page))
-            om[b * s_q + i] = _attend(_f(qm[b * s_q + i]).view(nh, D), k, v, scale).reshape(H).to(BF)
-
-
-def _attn_decode_fused(qkv, k_pool, v_pool, bt, max_pages, page, cos_t, sin_t, out, batch, nh, D, pos0, pos_dev, max_T, ldq,
-                       ldo, scale, n_split, _ws, _wsb, _s):
-    pos0 = pos0 + _dev_int(pos_dev)
-    H, half = nh * D, D // 2
-    q = _bfmat(qkv, batch, 3 * H, ldq)
-    c = _from_ptr(cos_t + pos0 * half * 2, half, BF).float()[None, None]
-    s_ = _from_ptr(sin_t + pos0 * half * 2, half, BF).float()[None, None]
-    for col0 in (0, H):
-        q[:, col0:col0 + H] = _rot(_f(q[:, col0:col0 + H]).view(batch, nh, D), c, s_, False).reshape(batch, H).to(BF)
-    _kv_append(qkv, k_pool, v_pool, bt, max_pages, page, nh, D, batch, 1, pos0, None, ldq, None)
-    _attn_decode(qkv, k_pool, v_pool, bt, max_pages, page, out, batch, 1, nh, D, pos0, None, max_T, ldq, ldo, scale, n_split,
-                 None, 0, None)
-
-
-def _sample_from_logits(logits, rows, V, ld, temp, top_p, top_k, step, event_tok, lut, n_event_types, eos_id, pad_id,
-                        dense_mask, uniforms, out, out_stride, _s):
-    assert top_k == 1, "mock kernel layer: greedy sampling only"
-    lg = _f(_bfmat(logits, rows, V, ld)).clone()
-    if dense_mask:                                    # app.py:73-87 options: [rows, V] uint8, ANDed with the grammar range
-        lg[_from_ptr(dense_mask, rows * V, torch.uint8).view(rows, V) == 0] = float("-inf")
-    table = _from_ptr(lut, n_event_types * 8 * 2, torch.int32).view(n_event_types, 8, 2)
-    ev = _from_ptr(event_tok, rows, torch.int64)
-    o = _from_ptr(out, (rows - 1) * out_stride + 1, torch.int64)
-    for r in range(rows):
-        if step == 0:
-            lo, hi = eos_id, eos_id + 1 + n_event_types
-        else:
-            e = int(ev[r]) - (eos_id + 1)
-            if int(ev[r]) == eos_id or e < 0 or e >= n_event_types:
-                lo, hi = pad_id, pad_id + 1
-            else:
-                lo, hi = int(table[e, step - 1, 0]), int(table[e, step - 1, 1])
-                if hi <= lo:
-                    lo, hi = pad_id, pad_id + 1
-        o[r * out_stride] = lo + int(torch.argmax(lg[r, lo:hi]))
-
-
-def _uniform_fill(u, n, seed, state, _s):
-    _from_ptr(state, 2, torch.int64)[0] += 1          # greedy mock: the draws themselves are never used
-
-
-def _event_commit(ev_t, seq, ev_next, pos_dev, B, T, max_len, _s):
-    pos = _from_ptr(pos_dev, 1, torch.int32)
-    p = int(pos[0])
-    ev = _from_ptr(ev_t, T * B, torch.int64).view(T, B).t()                # [B, T]
-    if p + 1 < max_len:
-        _from_ptr(seq, B * max_len * T, torch.int64).view(B, max_len, T)[:, p + 1] = ev
-    _from_ptr(ev_next, B * T, torch.int64).view(B, T).copy_(ev)
-    pos[0] = p + 1
+def _query(name, *args):
+    if name == "b200_gradnorm_parts":
+        return 1
+    if name == "b200_attn_decode_workspace_bytes":
+        return 256
+    raise AssertionError(f"mock kernel layer: unexpected C-ABI query {name}")
 
 
 class _NoStream:
@@ -458,69 +378,52 @@ class _NoStream:
         pass
 
 
-_DECODE_CALLS = {"b200_uniform_fill": _uniform_fill, "b200_event_commit": _event_commit, "b200_gemv_bf16": _gemv_bf16, "b200_gemv_fused": _gemv_fused, "b200_kv_append": _kv_append,
-                 "b200_attn_decode": _attn_decode, "b200_attn_decode_fused": _attn_decode_fused,
-                 "b200_sample_from_logits": _sample_from_logits}
+class _Event:
+    """torch.cuda.Event stand-in: the mock kernels have finished when their call returns."""
 
+    def __init__(self, *a, **k):
+        pass
 
-# ------------------------------------------------------------------ raw C-ABI calls the host code issues itself
-def _call(name, *args):
-    if name in _DECODE_CALLS:
-        return _DECODE_CALLS[name](*args)
-    if name == "b200_inner_input_bwd_hidden":
-        dx_ptr, dh_ptr, n_events, Tin, H, _ = args
-        dx = _from_ptr(dx_ptr, n_events * Tin * H, BF).view(n_events, Tin, H)
-        _from_ptr(dh_ptr, n_events * H, BF).view(n_events, H).copy_(dx[:, 0])
-        return
-    if name == "b200_grad_clip_coef":
-        gptr, n, max_norm, nc_ptr, _, _, _ = args
-        g = _from_ptr(gptr, n, BF).float()
-        norm = float(g.pow(2).sum().sqrt())
-        nc = _from_ptr(nc_ptr, 2, torch.float32)
-        nc[0] = norm
-        nc[1] = min(1.0, max_norm / (norm + 1e-6))
-        return
-    if name == "b200_adamw_step":
-        pptr, gptr, mptr, vptr, fptr, n, lr, b1, b2, eps, wd, step, nc_ptr, _ = args
-        p, g = _from_ptr(pptr, n, BF), _from_ptr(gptr, n, BF).float()
-        m, v = _from_ptr(mptr, n, torch.float32), _from_ptr(vptr, n, torch.float32)
-        flags = _from_ptr(fptr, (n + 255) // 256, torch.uint8)
-        g = g * float(_from_ptr(nc_ptr, 2, torch.float32)[1])
-        m.mul_(b1).add_(g, alpha=1 - b1)
-        v.mul_(b2).addcmul_(g, g, value=1 - b2)
-        decay = torch.where(flags.repeat_interleave(256)[:n] != 0, torch.ones(()), torch.tensor(1.0 - lr * wd))
-        upd = (m / (1 - b1 ** step)) / ((v / (1 - b2 ** step)).sqrt() + eps)
-        p.copy_((p.float() * decay - lr * upd).to(BF))
-        return
-    raise AssertionError(f"mock kernel layer: unexpected C-ABI call {name}")
+    def record(self, stream=None):
+        pass
 
-
-def _query(name, *args):
-    if name == "b200_gradnorm_parts":
-        return 1
-    if name == "b200_attn_decode_workspace_bytes":
-        return 256
-    raise AssertionError(f"mock kernel layer: unexpected C-ABI query {name}")
+    def query(self):
+        return True
 
 
 # the `midi_b200.ops` wrappers the host code calls, each replaced by the stand-in of the same name above
 OPS = ("embed_sum", "inner_input", "inner_input_rows", "inner_input_rows_bwd_hidden", "batch_to_xy", "batch_to_xy_packed",
-       "embed_bwd", "rmsnorm", "add_rmsnorm", "rmsnorm_bwd", "rope_table", "rope_qk_", "rope_qk_seg_", "swiglu", "swiglu_bwd",
-       "scale", "gemm", "linear_swiglu", "linear_rope", "linear_rope_seg", "attn_causal_fwd", "attn_causal_bwd",
-       "attn_causal_fwd_seg", "attn_causal_bwd_seg", "attn_tiny_fwd", "attn_tiny_bwd", "ce_fwd", "argmax_hits", "ce_bwd_")
+       "embed_bwd", "rmsnorm", "add_rmsnorm", "rmsnorm_bwd", "rope_table", "rope_qk_", "rope_qk_seg_", "rope_qk_ragged_",
+       "swiglu", "swiglu_bwd", "scale", "gemm", "linear_swiglu", "linear_rope", "linear_rope_seg", "attn_causal_fwd",
+       "attn_causal_bwd", "attn_causal_fwd_seg", "attn_causal_bwd_seg", "attn_tiny_fwd", "attn_tiny_bwd", "ce_fwd",
+       "argmax_hits", "ce_bwd_")
 
 
-def install(monkeypatch):
-    """Route the host code's kernel calls to the CPU stand-ins above for the duration of one test."""
-    from midi_b200 import engine, lib, ops
+def install(monkeypatch, persist=False):
+    """Route the host code's kernel calls to the CPU stand-ins above and those of tests/mock_decode.py for the duration
+    of one test.  `persist`: let the generate loops take the persistent kernel's path (mock_decode.decode_events) for the
+    tiny test model, whose shapes the kernel is not built for."""
+    import contextlib
+
+    import mock_decode
+    from midi_b200 import decode, engine, lib, ops, serve
     g = globals()
     for name in OPS:
         monkeypatch.setattr(ops, name, g[name])
     monkeypatch.setattr(ops, "_ws", lambda key, nbytes, device, zero=False: torch.zeros(max(nbytes, 256), dtype=torch.uint8))
     monkeypatch.setattr(ops, "GEMM_PROFILE", None)
-    monkeypatch.setattr(lib, "load", lambda: None)
-    monkeypatch.setattr(lib, "call", _call)
+    calls = {**CALLS, **mock_decode.CALLS}
+
+    def call(name, *args):
+        if name not in calls:
+            raise AssertionError(f"mock kernel layer: unexpected C-ABI call {name}")
+        return calls[name](*args)
+
+    monkeypatch.setattr(lib, "call", call)
     monkeypatch.setattr(lib, "query", _query)
+    monkeypatch.setattr(lib, "load", lambda: mock_decode.LIB if persist else None)
+    if persist:
+        monkeypatch.setattr(decode.GraphGenerator, "persistent_ok", lambda self: True)
     monkeypatch.setattr(lib, "stream", lambda: None)
     monkeypatch.setattr(lib, "require_cuda", lambda t, what="tensor": None)
     def require_bf16(n, p, dev):                 # the dtype half of the product's check stays; only `is_cuda` is waived
@@ -529,10 +432,13 @@ def install(monkeypatch):
 
     monkeypatch.setattr(engine, "_require_device", require_bf16)
     monkeypatch.setattr(engine, "WGRAD_STREAM", False)
-    import contextlib
+    monkeypatch.setattr(serve, "_pinned", lambda shape, dtype: torch.zeros(shape, dtype=dtype))
     monkeypatch.setattr(torch.cuda, "Stream", _NoStream)
+    monkeypatch.setattr(torch.cuda, "Event", _Event)
     monkeypatch.setattr(torch.cuda, "current_stream", lambda *a, **k: _NoStream())
     monkeypatch.setattr(torch.cuda, "stream", lambda s: contextlib.nullcontext())
+    for record in (mock_decode.DRAWS, mock_decode.LAUNCHES, mock_decode.ON_EVENT, mock_decode._KEYS):
+        record.clear()
 
 
 def trace(monkeypatch, fn, names=None):

@@ -1,7 +1,7 @@
 """Request queue (`generate_many`): the host scheduler -- admission with a batch-1 prefill into a slot, the rebase of the
-shared counter, per-row stop, refill and output order -- over the CPU stand-in for the kernel layer (tests/mock_kernels.py,
-tests/mock_ragged.py, tests/mock_queue.py), on the host-issued loop (B200_GENERATE=nograph) and on the persistent kernel's
-launch protocol.  The kernels themselves are checked on the GPU (tests/test_gpu_generate_many.py)."""
+shared counter, per-row stop, refill and output order -- over the CPU stand-in for the kernel layer (tests/mock_kernels.py),
+on the host-issued loop (B200_GENERATE=nograph) and on the persistent kernel's launch protocol.  The kernels themselves
+are checked on the GPU (tests/test_gpu_generate_many.py)."""
 import inspect
 
 import numpy as np
@@ -9,7 +9,6 @@ import pytest
 import torch
 
 import host_model
-import mock_queue
 
 
 def test_generate_many_signature():
@@ -21,15 +20,7 @@ def test_generate_many_signature():
 
 @pytest.fixture(params=["nograph", "persist"])
 def model(request, monkeypatch):
-    mock_queue.install(monkeypatch, persist=request.param == "persist")
-    monkeypatch.setenv("B200_GENERATE", request.param)
-    return host_model.tiny_model(0).eval()
-
-
-def _prompts(model, lengths, seed):
-    from midi_b200.synth import synth_batch
-    batch = synth_batch(model.tokenizer, len(lengths), max(lengths), seed=seed).numpy()
-    return [batch[i, :L] for i, L in enumerate(lengths)]
+    return host_model.generate_model(monkeypatch, request.param)
 
 
 def _bos(model):
@@ -55,27 +46,27 @@ def _check_solo(model, prompts, budgets, got):
 
 def test_more_requests_than_slots_with_mixed_budgets(model):
     lengths, budgets = [5, 2, 9, 3, 7, 4, 2], [6, 1, 3, 8, 2, 5, 4]
-    prompts = _prompts(model, lengths, seed=11)
+    prompts = host_model.prompts(model, lengths, seed=11)
     got = model.generate_many(prompts, budgets, batch_size=3, top_k=1)
     _check_solo(model, prompts, budgets, got)
 
 
 def test_fewer_requests_than_slots_and_one_request(model):
-    prompts = _prompts(model, [4, 6], seed=12)
+    prompts = host_model.prompts(model, [4, 6], seed=12)
     _check_solo(model, prompts, [5, 3], model.generate_many(prompts, [5, 3], batch_size=8, top_k=1))
     one = prompts[:1]
     _check_solo(model, one, [4], model.generate_many(one, 4, batch_size=1, top_k=1))
 
 
 def test_one_new_event_and_bos_only_prompts(model):
-    prompts = [_bos(model)] + _prompts(model, [3, 5], seed=13) + [_bos(model)]
+    prompts = [_bos(model)] + host_model.prompts(model, [3, 5], seed=13) + [_bos(model)]
     _check_solo(model, prompts, [1] * 4, model.generate_many(prompts, 1, batch_size=2, top_k=1))
     _check_solo(model, prompts, [5, 2, 1, 3], model.generate_many(prompts, [5, 2, 1, 3], batch_size=2, top_k=1))
 
 
 def test_request_filling_the_pools(model):
     """L + max_new = 64 = the capacity of one 64-position page: the longest request uses its last KV slot."""
-    prompts = _prompts(model, [52, 3, 6], seed=14)
+    prompts = host_model.prompts(model, [52, 3, 6], seed=14)
     budgets = [12, 4, 2]
     from midi_b200 import decode
     seen = []
@@ -104,7 +95,7 @@ def test_one_batch1_prefill_per_request_in_input_order(model, monkeypatch):
         return orig(self, x, kv, s_new, pos_dev, *a, **k)
 
     lengths = [4, 7, 2, 5, 3]
-    prompts = _prompts(model, lengths, seed=15)
+    prompts = host_model.prompts(model, lengths, seed=15)
     model.generate_many(prompts[:1], 1, top_k=1)                    # runtime set-up outside the count
     monkeypatch.setattr(decode.CachedStack, "step", spy)
     model.generate_many(prompts, [3, 1, 4, 2, 2], batch_size=2, top_k=1)
@@ -116,7 +107,7 @@ def test_one_batch1_prefill_per_request_in_input_order(model, monkeypatch):
 
 def test_input_errors_raise(model, monkeypatch):
     from midi_b200.lib import B200Error
-    good = _prompts(model, [3, 4], seed=16)
+    good = host_model.prompts(model, [3, 4], seed=16)
     bad_prompts = [[], (), "ab", [good[0][:0]], [good[0][0]], [good[0][None]], [good[0].astype(np.float32)],
                    [torch.from_numpy(good[0]).to("meta")], [None], good[0]]
     for prompts in bad_prompts:
@@ -134,7 +125,7 @@ def test_input_errors_raise(model, monkeypatch):
 
 
 def test_cpu_tensor_prompts_and_budgets(model):
-    prompts = _prompts(model, [3, 6, 2], seed=17)
+    prompts = host_model.prompts(model, [3, 6, 2], seed=17)
     ref = model.generate_many(prompts, [2, 3, 4], batch_size=2, top_k=1)
     got = model.generate_many([torch.from_numpy(p) for p in prompts], torch.tensor([2, 3, 4]), batch_size=2, top_k=1)
     assert all((a == b).all() and a.shape == b.shape for a, b in zip(ref, got))

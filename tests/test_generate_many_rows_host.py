@@ -1,8 +1,8 @@
 """Per-request mode of the request queue (`generate_many_requests`, and `generate_many` with per-request settings): the host
 side -- each slot's settings, RNG key and mask row written at admission, the `_rows` entries issued, the scalar call left
-as it was, input checks -- over the CPU stand-in for the kernel layer (tests/mock_kernels.py, tests/mock_ragged.py,
-tests/mock_queue.py, tests/mock_rows.py), on the host-issued loop (B200_GENERATE=nograph) and on the persistent kernel's
-launch protocol.  The kernels themselves are checked on the GPU (tests/test_gpu_generate_many_rows.py)."""
+as it was, input checks -- over the CPU stand-in for the kernel layer (tests/mock_kernels.py), on the host-issued loop
+(B200_GENERATE=nograph) and on the persistent kernel's launch protocol.  The kernels themselves are checked on the GPU
+(tests/test_gpu_generate_many_rows.py)."""
 import inspect
 
 import numpy as np
@@ -10,8 +10,9 @@ import pytest
 import torch
 
 import host_model
-import mock_ragged
-import mock_rows
+import mock_decode
+import mock_kernels
+from decode_reference import counter_uniform
 
 LENGTHS, BUDGETS = [5, 2, 9, 3, 7, 4, 1], [6, 4, 4, 8, 5, 5, 4]      # >= 4: generate runs its device loop
 TEMPS, TOP_PS, TOP_KS = [1.3, 0.7, 1.0, 1.0, 0.9, 1.2, 1.0], [0.9, 1.0, 0.5, 0.98, 1.0, 0.8, 1.0], [64, 5, 20, 1, 3, 8, 2]
@@ -31,15 +32,7 @@ def test_generate_many_requests_signature():
 
 @pytest.fixture(params=["nograph", "persist"])
 def model(request, monkeypatch):
-    mock_rows.install(monkeypatch, persist=request.param == "persist")
-    monkeypatch.setenv("B200_GENERATE", request.param)
-    return host_model.tiny_model(0).eval()
-
-
-def _prompts(model, lengths, seed):
-    from midi_b200.synth import synth_batch
-    batch = synth_batch(model.tokenizer, len(lengths), max(lengths), seed=seed).numpy()
-    return [batch[i, :L] for i, L in enumerate(lengths)]
+    return host_model.generate_model(monkeypatch, request.param)
 
 
 def _deny(model, i):
@@ -72,17 +65,17 @@ def _solo(model, p, n, i):
 def test_every_draw_is_the_requests_own(model, batch_size):
     """Each sampler call of request i gets hash(seeds[i], 8 j + t, 0), its own settings and its own mask row, whatever
     slot holds it; the same request set permuted gives each request the same events."""
-    prompts = _prompts(model, LENGTHS, seed=21)
+    prompts = host_model.prompts(model, LENGTHS, seed=21)
     order = list(range(len(prompts)))
     got = model.generate_many_requests(prompts, BUDGETS, batch_size=batch_size, **_kwargs(order))
     by_seed = {SEEDS[i]: i for i in order}
     seen = {i: set() for i in order}
     n_new = [got[i].shape[0] - LENGTHS[i] for i in order]
-    for d in mock_rows.DRAWS:
+    for d in mock_decode.DRAWS:
         i = by_seed.get(d["seed"])
         if i is None or not 0 <= d["j"] < n_new[i]:
             continue                                               # an empty slot's row: its draw is never committed
-        assert d["u"] == mock_rows.counter_uniform(SEEDS[i], 8 * d["j"] + d["step"], 0), d
+        assert d["u"] == counter_uniform(SEEDS[i], 8 * d["j"] + d["step"], 0), d
         assert (d["temp"], d["top_k"]) == (np.float32(TEMPS[i]), TOP_KS[i]) and d["top_p"] == np.float32(TOP_PS[i]), d
         assert d["deny"] == _deny(model, i), d
         seen[i].add((d["j"], d["step"]))
@@ -96,7 +89,7 @@ def test_every_draw_is_the_requests_own(model, batch_size):
 
 
 def test_one_slot_equals_generate_seeded_as_specified(model):
-    prompts = _prompts(model, LENGTHS, seed=22)
+    prompts = host_model.prompts(model, LENGTHS, seed=22)
     order = list(range(len(prompts)))
     got = model.generate_many_requests(prompts, BUDGETS, batch_size=1, **_kwargs(order))
     for i, (p, n) in enumerate(zip(prompts, BUDGETS)):
@@ -107,7 +100,7 @@ def test_one_slot_equals_generate_seeded_as_specified(model):
 
 
 def test_greedy_requests_in_a_mixed_queue_equal_generating_alone(model):
-    prompts = _prompts(model, LENGTHS, seed=23)
+    prompts = host_model.prompts(model, LENGTHS, seed=23)
     top_k = [1 if i % 2 == 0 else 20 for i in range(len(prompts))]
     got = model.generate_many(prompts, BUDGETS, batch_size=3, top_k=top_k, temp=1.3, top_p=0.9)   # per-request top_k
     for i in range(0, len(prompts), 2):
@@ -120,11 +113,11 @@ def test_greedy_requests_in_a_mixed_queue_equal_generating_alone(model):
 def test_scalar_call_issues_no_rows_entry(model, monkeypatch):
     """Scalar settings without seeds keep the scalar queue: the same kernel calls, none of the `_rows` entries, and scalar
     grammar options only in every row's mask."""
-    prompts = _prompts(model, [4, 2, 6], seed=24)
+    prompts = host_model.prompts(model, [4, 2, 6], seed=24)
     model.generate_many_requests(prompts[:1], 1, top_k=1)                     # runtime set-up outside the trace
     def trace(**kw):
         with pytest.MonkeyPatch.context() as mp:
-            return mock_ragged.trace(mp, lambda: model.generate_many_requests(prompts, [3, 2, 4], batch_size=2, top_k=1, **kw))
+            return mock_kernels.trace(mp, lambda: model.generate_many_requests(prompts, [3, 2, 4], batch_size=2, top_k=1, **kw))
 
     plain = trace()
     assert plain and plain == trace(disable_patch_change=True, disable_channels=[2, 3])
@@ -134,7 +127,7 @@ def test_scalar_call_issues_no_rows_entry(model, monkeypatch):
 
 def test_per_request_input_errors_raise(model):
     from midi_b200.lib import B200Error
-    good = _prompts(model, [3, 4], seed=25)
+    good = host_model.prompts(model, [3, 4], seed=25)
     bad = [dict(temp=[1.0]), dict(temp=[1.0, 0.0]), dict(temp=[1.0, -1.0]), dict(temp=[1.0, float("nan")]),
            dict(top_p=[0.9, 0.0]), dict(top_p=[0.9, 1.5]), dict(top_k=[1, 0]), dict(top_k=[1, 2.5]), dict(top_k=[1, 2, 3]),
            dict(seeds=[1]), dict(seeds=[1, 2, 3]), dict(seeds=[1, -1]), dict(seeds=[1, 2 ** 62]), dict(seeds=[1, 2.0]),

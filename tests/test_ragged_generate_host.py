@@ -1,13 +1,13 @@
 """Ragged prompts (`generate_ragged` / `generate_stream_ragged`): the host logic of the device-resident loop (ragged state,
 rectangular prefill, per-row offsets handed to the `_ragged` kernel entries, per-row stop check and output layout) over
-the CPU stand-in for the kernel layer (tests/mock_kernels.py, tests/mock_ragged.py), B200_GENERATE=nograph.  The kernels themselves are
-checked on the GPU (tests/test_gpu_ragged_generate.py)."""
+the CPU stand-in for the kernel layer (tests/mock_kernels.py), B200_GENERATE=nograph.  The kernels themselves are checked on
+the GPU (tests/test_gpu_ragged_generate.py)."""
 import numpy as np
 import pytest
 import torch
 
 import host_model
-import mock_ragged
+import mock_kernels
 
 
 def test_ragged_signatures():
@@ -26,10 +26,7 @@ def test_ragged_signatures():
 
 @pytest.fixture
 def model(monkeypatch):
-    mock_ragged.install(monkeypatch)
-    monkeypatch.setenv("B200_GENERATE", "nograph")
-    m = host_model.tiny_model(0).eval()
-    return m
+    return host_model.generate_model(monkeypatch, "nograph")
 
 
 def _prompt(model, B, P, seed):
@@ -75,7 +72,7 @@ def test_few_new_events_still_use_the_device_loop(model, monkeypatch):
     lengths = torch.tensor([3, 5, 1])
     prompt = _prompt(model, 3, P, seed=4)
     with monkeypatch.context() as mp:
-        names = mock_ragged.trace(mp, lambda: model.generate_ragged(prompt=prompt, batch_size=3, max_len=P + 2, top_k=1,
+        names = mock_kernels.trace(mp, lambda: model.generate_ragged(prompt=prompt, batch_size=3, max_len=P + 2, top_k=1,
                                                                      lengths=lengths))
     assert "b200_event_commit_ragged" in names
     ids = model.generate_ragged(prompt=prompt, batch_size=3, max_len=P + 2, top_k=1, lengths=lengths)
@@ -96,9 +93,9 @@ def test_full_lengths_match_rectangular_call_for_call(model, monkeypatch):
     out = {}
     model.generate(**kw)                                       # one-time set-up (RoPE tables, grammar) outside the traces
     with monkeypatch.context() as mp:
-        rect = mock_ragged.trace(mp, lambda: out.setdefault("rect", model.generate(**kw)))
+        rect = mock_kernels.trace(mp, lambda: out.setdefault("rect", model.generate(**kw)))
     with monkeypatch.context() as mp:
-        ragged = mock_ragged.trace(mp, lambda: out.setdefault("ragged", model.generate_ragged(**kw, lengths=[P] * B)))
+        ragged = mock_kernels.trace(mp, lambda: out.setdefault("ragged", model.generate_ragged(**kw, lengths=[P] * B)))
     assert (out["rect"] == out["ragged"]).all() and out["rect"].shape == out["ragged"].shape
     assert not [n for n in rect if "ragged" in n]
     assert [n.replace("_ragged", "") for n in ragged] == rect

@@ -1,8 +1,8 @@
-"""The serving queue (midi_b200/serve.py: GenerateServer) over the CPU stand-in for the kernel layer (tests/mock_kernels.py
-... tests/mock_stream.py), on the host-issued loop (B200_GENERATE=nograph) and on the streaming persistent kernel's launch
-protocol: requests submitted from several threads while the server runs, cancellations, the stream against result(), the
-budget and EOS, input errors, a worker failure, the app-shaped helper, and generate_many's kernel calls left as they were.
-The kernel itself is checked on the GPU (tests/test_gpu_serve.py)."""
+"""The serving queue (midi_b200/serve.py: GenerateServer) over the CPU stand-in for the kernel layer (tests/mock_kernels.py),
+on the host-issued loop (B200_GENERATE=nograph) and on the streaming persistent kernel's launch protocol: requests
+submitted from several threads while the server runs, cancellations, the stream against result(), the budget and EOS,
+input errors, a worker failure, the app-shaped helper, and generate_many's kernel calls left as they were.  The kernel
+itself is checked on the GPU (tests/test_gpu_serve.py)."""
 import os
 import shutil
 import subprocess
@@ -14,8 +14,8 @@ import pytest
 import torch
 
 import host_model
-import mock_ragged
-import mock_stream
+import mock_decode
+import mock_kernels
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LENGTHS = [5, 2, 9, 3, 7, 4, 1, 6, 3, 8, 2, 5]
@@ -28,17 +28,9 @@ CHANNELS = [None, [0, 9], None, None, None, [3], None, None, None, None, None, [
 
 @pytest.fixture(params=["nograph", "persist"])
 def model(request, monkeypatch):
-    mock_stream.install(monkeypatch, persist=request.param == "persist")
-    monkeypatch.setenv("B200_GENERATE", request.param)
-    m = host_model.tiny_model(0).eval()
+    m = host_model.generate_model(monkeypatch, request.param)
     m.loop = request.param
     return m
-
-
-def _prompts(model, lengths, seed):
-    from midi_b200.synth import synth_batch
-    batch = synth_batch(model.tokenizer, len(lengths), max(lengths), seed=seed).numpy()
-    return [batch[i, :L] for i, L in enumerate(lengths)]
 
 
 def _kw(i):
@@ -62,7 +54,7 @@ def _solo_greedy(model, p, n):
 @pytest.mark.parametrize("slots", [2, 4])
 def test_requests_from_three_threads_with_cancellations(model, slots):
     from midi_b200.serve import GenerateServer
-    prompts = _prompts(model, LENGTHS, seed=31)
+    prompts = host_model.prompts(model, LENGTHS, seed=31)
     cancel = {3, 7}
     streamed, results, errors = {}, {}, []
 
@@ -110,19 +102,19 @@ def test_requests_from_three_threads_with_cancellations(model, slots):
         deny = set(model._deny_ids(False, False, CHANNELS[i]))
         assert not any(deny & set(row.tolist()) for row in new), i
     if model.loop == "persist":
-        assert mock_stream.LAUNCHES and all(n <= 64 for n, _, _, _ in mock_stream.LAUNCHES)
+        assert mock_decode.LAUNCHES and all(n <= 64 for n, _, _, _ in mock_decode.LAUNCHES)
 
 
 def test_cancel_ends_a_running_launch(model):
     """A cancellation while a launch runs ends it after the event in which ctl is seen; the slot then serves the next
     request, whose result is unchanged."""
     from midi_b200.serve import GenerateServer
-    prompts = _prompts(model, [4, 3], seed=32)
+    prompts = host_model.prompts(model, [4, 3], seed=32)
     with GenerateServer(model, batch_size=1, max_len=64) as server:
         seen = []
         long = server.submit(prompts[0], 40, top_k=1, seed=1)
         if model.loop == "persist":
-            mock_stream.ON_EVENT.append(lambda k: seen.append(k) if k == 3 and not long.cancelled and long.cancel() is None
+            mock_decode.ON_EVENT.append(lambda k: seen.append(k) if k == 3 and not long.cancelled and long.cancel() is None
                                         else None)
         else:
             it = iter(long)
@@ -133,7 +125,7 @@ def test_cancel_ends_a_running_launch(model):
         got_long, got_next = long.result(), nxt.result()
     assert prompts[0].shape[0] + 3 <= got_long.shape[0] < prompts[0].shape[0] + 40
     if model.loop == "persist":
-        first = mock_stream.LAUNCHES[0]
+        first = mock_decode.LAUNCHES[0]
         assert first[3] and first[2] == 3                                    # left after the event that saw ctl
     solo = _solo_greedy(model, prompts[1], 5)
     assert got_next.shape == solo.shape and (got_next == solo).all()
@@ -144,7 +136,7 @@ def test_cancel_ends_a_running_launch(model):
 def test_submit_checks_raise_in_the_callers_thread(model):
     from midi_b200.lib import B200Error
     from midi_b200.serve import GenerateServer
-    p = _prompts(model, [4], seed=33)[0]
+    p = host_model.prompts(model, [4], seed=33)[0]
     bad = [dict(max_new=0), dict(max_new=2.0), dict(max_new=True), dict(max_new=13), dict(temp=0.0), dict(temp=-1.0),
            dict(temp=float("nan")), dict(top_p=0.0), dict(top_p=1.5), dict(top_k=0), dict(top_k=2.5), dict(seed=-1),
            dict(seed=2 ** 62), dict(seed=2.0), dict(seed=True), dict(disable_channels=[16]), dict(disable_channels=[-1]),
@@ -172,7 +164,7 @@ def test_submit_checks_raise_in_the_callers_thread(model):
 def test_weights_changed_since_start_raise(model):
     from midi_b200.lib import B200Error
     from midi_b200.serve import GenerateServer
-    p = _prompts(model, [3], seed=34)[0]
+    p = host_model.prompts(model, [3], seed=34)[0]
     with GenerateServer(model, batch_size=1, max_len=16) as server:
         server.submit(p, 2, top_k=1).result()
         with torch.no_grad():
@@ -185,7 +177,7 @@ def test_worker_error_reaches_every_iterator(model, monkeypatch):
     from midi_b200 import lib
     from midi_b200.lib import B200Error
     from midi_b200.serve import GenerateServer
-    prompts = _prompts(model, [3, 4, 5, 2, 6], seed=35)
+    prompts = host_model.prompts(model, [3, 4, 5, 2, 6], seed=35)
     call = lib.call
 
     def failing(name, *a):                # the first event fails, with two requests resident and three waiting
@@ -214,7 +206,7 @@ def test_helper_rows_and_pad_layout(model):
     the i-th draw of the generator."""
     from midi_b200.serve import GenerateServer
     tok = model.tokenizer
-    prompt = _prompts(model, [5], seed=36)[0]
+    prompt = host_model.prompts(model, [5], seed=36)[0]
     B, max_len = 3, 12
     with GenerateServer(model, batch_size=2, max_len=64) as server:
         # EOS is likely for some rows with a sampled step 0: check the pad layout whenever a row ends early
@@ -242,12 +234,12 @@ def test_helper_rows_and_pad_layout(model):
 
 def test_generate_many_trace_is_unchanged_by_a_server(model):
     from midi_b200.serve import GenerateServer
-    prompts = _prompts(model, [4, 2, 6], seed=37)
+    prompts = host_model.prompts(model, [4, 2, 6], seed=37)
     model.generate_many_requests(prompts[:1], 1, top_k=1)
 
     def trace():
         with pytest.MonkeyPatch.context() as mp:
-            return mock_ragged.trace(mp, lambda: model.generate_many_requests(prompts, [3, 2, 4], batch_size=2, top_k=1,
+            return mock_kernels.trace(mp, lambda: model.generate_many_requests(prompts, [3, 2, 4], batch_size=2, top_k=1,
                                                                              seeds=[1, 2, 3]))
 
     before = trace()

@@ -1,30 +1,21 @@
 """Shared prompts in the request queue (`generate_many`, `generate_many_requests`): requests with equal prompts of at least
 65 events prefill once and read the prompt's whole pages from the same KV pages (decode.SharedPages).  Over the CPU
-stand-in for the kernel layer (tests/mock_shared.py and the mocks below it), on the host-issued loop and on the persistent
-kernel's launch protocol, greedy and per-request sampled.  Every call is compared with the same call with sharing off, and
-spies check the page assignment at every launch."""
+stand-in for the kernel layer (tests/mock_kernels.py), on the host-issued loop and on the persistent kernel's launch
+protocol, greedy and per-request sampled.  Every call is compared with the same call with sharing off, and spies check
+the page assignment at every launch."""
 import numpy as np
 import pytest
 import torch
 
 import host_model
-import mock_ragged
-import mock_shared
+import mock_kernels
 
 LAUNCHES = ("b200_event_commit_queue", "b200_decode_events_queue", "b200_decode_events_queue_rows")
 
 
 @pytest.fixture(params=["nograph", "persist"])
 def model(request, monkeypatch):
-    mock_shared.install(monkeypatch, persist=request.param == "persist")
-    monkeypatch.setenv("B200_GENERATE", request.param)
-    return host_model.tiny_model(0).eval()
-
-
-def _prompts(model, lengths, seed):
-    from midi_b200.synth import synth_batch
-    batch = synth_batch(model.tokenizer, len(lengths), max(lengths), seed=seed).numpy()
-    return [batch[i, :L] for i, L in enumerate(lengths)]
+    return host_model.generate_model(monkeypatch, request.param)
 
 
 class Spy:
@@ -131,7 +122,7 @@ def _check(model, prompts, budgets, batch_size, sampled):
 
 @pytest.mark.parametrize("sampled", [False, True])
 def test_duplicates_admitted_together(model, sampled):
-    a, c = _prompts(model, [70, 90], seed=31)
+    a, c = host_model.prompts(model, [70, 90], seed=31)
     prompts = [a, a, c, a]
     got, spy = _check(model, prompts, [5, 3, 4, 6], 4, sampled)
     assert sorted(spy.prefills) == [70, 90]                 # one prefill of the shared prompt
@@ -142,7 +133,7 @@ def test_duplicates_admitted_together(model, sampled):
 def test_duplicates_admitted_apart_and_finishing_at_different_events(model, sampled):
     """Two slots: the second copy of `a` joins the first while it is live, at its own position; the later copies join the
     second; after the last sharer finishes, `a` is prefilled again."""
-    a, c, d, e = _prompts(model, [80, 66, 75, 68], seed=32)
+    a, c, d, e = host_model.prompts(model, [80, 66, 75, 68], seed=32)
     prompts = [a, c, a, a, d, a, e]
     budgets = [9, 2, 3, 8, 9, 1, 2]
     got, spy = _check(model, prompts, budgets, 2, sampled)
@@ -154,7 +145,7 @@ def test_duplicates_admitted_apart_and_finishing_at_different_events(model, samp
 def test_page_boundaries(model, L):
     """L - 1 = 63 shares nothing (no whole page).  L - 1 = 64 and 128 share one and two pages, and their tail pages hold no
     prompt position; L - 1 = 65 shares one page and copies a tail page holding one prompt position."""
-    a, c = _prompts(model, [L, 67], seed=33)
+    a, c = host_model.prompts(model, [L, 67], seed=33)
     prompts = [a, c, a, a]
     got, spy = _check(model, prompts, [4, 2, 5, 3], 3, False)
     if L - 1 < 64:
@@ -167,7 +158,7 @@ def test_page_boundaries(model, L):
 def test_empty_slot_while_sharers_are_live(model, sampled):
     """The distinct request finishes first and no request waits: its slot stays empty (and, on the host-issued loop, keeps
     appending) while the sharers run on."""
-    a, c = _prompts(model, [72, 5], seed=34)
+    a, c = host_model.prompts(model, [72, 5], seed=34)
     got, spy = _check(model, [a, c, a], [7, 1, 6], 3, sampled)
     assert spy.shared_launches > 0
 
@@ -175,7 +166,7 @@ def test_empty_slot_while_sharers_are_live(model, sampled):
 @pytest.mark.parametrize("sampled", [False, True])
 def test_refilled_slot_prefills_beside_shared_pages(model, sampled):
     """Slot 1 is refilled with distinct prompts while the sharers of `a` are live: their prefills go to free pages."""
-    a, c, d, e = _prompts(model, [100, 3, 70, 90], seed=35)
+    a, c, d, e = host_model.prompts(model, [100, 3, 70, 90], seed=35)
     got, spy = _check(model, [a, c, d, a, e], [10, 1, 2, 9, 2], 3, sampled)
     assert spy.prefills.count(100) == 1 and spy.shared_launches > 0
 
@@ -185,7 +176,7 @@ def test_call_without_a_shared_prompt_keeps_its_trace(model):
     launch sees the identity block table, every prefill goes through the slot's own pages (PagedKV.row), and the kernel
     calls are those of the call with sharing patched off."""
     from midi_b200 import decode
-    prompts = _prompts(model, [64, 70, 5], seed=36)
+    prompts = host_model.prompts(model, [64, 70, 5], seed=36)
     prompts = [prompts[0], prompts[1], prompts[0], prompts[2]]
     model.generate_many(prompts[:1], 1, top_k=1)                        # runtime set-up outside the trace
 
@@ -195,7 +186,7 @@ def test_call_without_a_shared_prompt_keeps_its_trace(model):
                 mp.setattr(decode, "_share_keys", lambda prompts, page: [None] * len(prompts))
             mp.setattr(decode.PagedKV, "table_row", lambda *a: pytest.fail("a prefill through the block table"))
             spy = Spy(model, mp)
-            names = mock_ragged.trace(mp, lambda: model.generate_many(prompts, [3, 2, 4, 2], batch_size=2, top_k=1))
+            names = mock_kernels.trace(mp, lambda: model.generate_many(prompts, [3, 2, 4, 2], batch_size=2, top_k=1))
         assert spy.pages is None and spy.launches > 0
         return names
 
