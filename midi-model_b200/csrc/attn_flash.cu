@@ -154,6 +154,7 @@ flash_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const b
     cp_async_commit();
 
     float m_i[2] = {-INFINITY, -INFINITY}, l_i[2] = {0.f, 0.f};
+    float msc[2] = {0.f, 0.f};   // m_i * scale * log2(e), rounded once: every exponent of the row is taken against it
     float oacc[8][4];
 #pragma unroll
     for (int i = 0; i < 8; i++)
@@ -207,12 +208,16 @@ flash_fwd_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k, const b
             mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
             mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
         }
-        float alpha[2], msc[2], rs[2] = {0.f, 0.f};
+        float alpha[2], rs[2] = {0.f, 0.f};
 #pragma unroll
         for (int r = 0; r < 2; r++) {
             const float mnew = mx[r];
-            msc[r] = (mnew == -INFINITY) ? 0.f : mnew * sl2;
-            alpha[r] = (m_i[r] == -INFINITY) ? 0.f : exp2f(m_i[r] * sl2 - msc[r]);
+            // The rescale is the difference of the old and new rounded reference points, so it is exactly 1 while the
+            // max stays.  __fmul_rn keeps the product out of an FMA: m_old * sl2 - msc contracted to one FMA would be
+            // 2^(rounding error of msc) instead, compounding over every key tile (1.9e-4 in the LSE at 64 tiles).
+            const float ms = (mnew == -INFINITY) ? 0.f : __fmul_rn(mnew, sl2);
+            alpha[r] = (m_i[r] == -INFINITY) ? 0.f : exp2f(msc[r] - ms);
+            msc[r] = ms;
             m_i[r] = mnew;
         }
 #pragma unroll

@@ -1689,24 +1689,107 @@ def check_gemm_epilogues():
     return W.report()
 
 
+def _attn_ref64_parts(q, k, v, do, off, scale, o_in=None):
+    """P.attn_ref64 of (B, h, S, D) tensors, on the whole tensors when their fp64 [Sq, Sk] score matrices fit in 2^26
+    elements (0.5 GB), else one batch row and as many heads as fit at a time: materialised at once, a (8, 2048) or
+    (1, 4096) case at 16 heads would take tens of GB of fp64 temporaries."""
+    B, nh, Sq, _ = q.shape
+    Sk = k.shape[2]
+    cap = 1 << 26
+    if B * nh * Sq * Sk <= cap:
+        return P.attn_ref64(q, k, v, do, off, scale, o_in)
+    hg = max(1, cap // (Sq * Sk))
+    out = None
+    for b in range(B):
+        for h0 in range(0, nh, hg):
+            i = (slice(b, b + 1), slice(h0, h0 + hg))
+            part = P.attn_ref64(q[i], k[i], v[i], do[i], off, scale, None if o_in is None else o_in[i])
+            if out is None:
+                out = [torch.empty((B, nh) + t.shape[2:], dtype=t.dtype, device=t.device) for t in part]
+            for t, r in zip(out, part):
+                t[i] = r
+    return tuple(out)
+
+
+def _attn_case(W, case, ins, new_out, B, Sq, Sk, nh, cos, sin, scale=0.125, floor=1e-3):
+    """One case of the attention conformance groups: b200_attn_causal_fwd{_wgmma,} and, from each implementation's own
+    o and lse, b200_attn_causal_bwd{_wgmma,} plain and with the RoPE backward fused into dq / dk, all through the C ABI.
+    Scored per (batch, head, row) against fp64 attention and its fp64 gradient given the o each backward receives, and
+    wgmma against mma on the same inputs.  The mma backward needs n_heads % 4 == 0, so other head counts run its
+    forward only.
+
+    ins    : {"q", "k", "v", "do"} -> (data pointer, [batch, row, head] element strides, (B, nh, S, D) view)
+    new_out: "o" -> fresh NaN output buffers for o, "dqkv" -> for dq, dk, dv, as ([(buffer, region the kernel must
+             write)], [(data pointer, strides, (B, nh, S, D) view)] of each output)."""
+    D = 64
+    off = Sk - Sq
+    q, k, v, do = (ins[n][2] for n in ("q", "k", "v", "do"))
+    o64, lse64, _, _, _ = _attn_ref64_parts(q, k, v, do, off, scale)
+    atol = 1e-3 * float(do.double().norm(dim=-1).median())   # row-norm floor on the scale of the inputs
+    st_in = [s for n in ("q", "k", "v") for s in ins[n][1]]
+    rows = {}
+    for impl, sfx in (("wg", "_wgmma"), ("mma", "")):
+        obufs, ((o_ptr, o_st, o),) = new_out("o")
+        n_lse = B * nh * Sq
+        lse = torch.full((n_lse + 64,), float("nan"), device=DEV)
+        stt = torch.tensor(st_in + o_st, dtype=torch.int64)
+        lib.call("b200_attn_causal_fwd" + sfx, ins["q"][0], ins["k"][0], ins["v"][0], o_ptr, lse.data_ptr(),
+                 stt.data_ptr(), B, nh, Sq, Sk, D, scale, lib.stream())
+        rows[(impl, "o")] = P.row_worst(o, o64, atol=atol)
+        W.add(impl, case, {"lse_abs": float((lse[:n_lse].view(B, nh, Sq).double() - lse64).abs().max())})
+        for buf, region in obufs:
+            W.add("", case, P.sentinel_report(buf, region))
+        W.add("", case, P.sentinel_report(lse, (slice(0, n_lse),)))
+        if impl == "mma" and nh % 4:
+            continue
+        _, _, dq64, dk64, dv64 = _attn_ref64_parts(q, k, v, do, off, scale, o_in=o)
+        dq64r = P.rope_bwd64(dq64, cos, sin, torch.arange(Sq, device=DEV) + off)
+        dk64r = P.rope_bwd64(dk64, cos, sin, torch.arange(Sk, device=DEV))
+        for rope in (False, True):
+            gbufs, parts = new_out("dqkv")
+            delta = torch.empty(n_lse, device=DEV)
+            stb = torch.tensor(st_in + o_st + ins["do"][1] + [s for p in parts for s in p[1]], dtype=torch.int64)
+            lib.call("b200_attn_causal_bwd" + sfx, ins["q"][0], ins["k"][0], ins["v"][0], o_ptr, ins["do"][0],
+                     lse.data_ptr(), delta.data_ptr(), parts[0][0], parts[1][0], parts[2][0], stb.data_ptr(), B, nh, Sq,
+                     Sk, D, scale, cos.data_ptr() if rope else None, sin.data_ptr() if rope else None, lib.stream())
+            g = {n: p[2] for n, p in zip(("dq", "dk", "dv"), parts)}
+            if rope:
+                W.add(impl, case, {"rope_dq_row": P.row_worst(g["dq"], dq64r, atol=atol),
+                                   "rope_dk_row": P.row_worst(g["dk"], dk64r, atol=atol),
+                                   "rope_dv_mismatch": float((g["dv"] != dv_plain).sum())})
+            else:
+                for n, ref in (("dq", dq64), ("dk", dk64), ("dv", dv64)):
+                    rows[(impl, n)] = P.row_worst(g[n], ref, atol=atol)
+                dv_plain = g["dv"].clone()
+            for buf, region in gbufs:
+                W.add("", case, P.sentinel_report(buf, region))
+    for (impl, n), val in rows.items():
+        W.add(impl, case, {f"{n}_row": val})
+        if impl == "wg" and ("mma", n) in rows:
+            # same semantics, so the wgmma worst row should stay near the mma worst row on the same inputs
+            W.add("wg_over_mma", case, {n: val / (1.5 * rows[("mma", n)] + floor)})
+
+
+def _attn_bounds(p):
+    """The bound table of an attention conformance group whose metrics _attn_case names with prefix p."""
+    return [(f"{p}sentinels_changed", 0.0), (f"{p}nan_in_range", 0.0), (f"{p}wg_rope_dv_mismatch", 0.0),
+            (f"{p}mma_rope_dv_mismatch", 0.0), (f"{p}wg_over_mma_", 1.0), (f"{p}wg_lse_abs", AE_LSE_ABS),
+            (f"{p}mma_lse_abs", AE_LSE_ABS),
+            *[(f"{p}{i}_{n}_row", AE_ROW) for i in ("wg", "mma") for n in ("o", "dq", "dk", "dv", "rope_dq", "rope_dk")]]
+
+
 # same card: worst row 3.4e-3 (o), 4.4e-3 / 4.6e-3 / 4.5e-3 (dq / dk / dv, with or without the fused RoPE backward),
 # equal for both implementations; wgmma / (1.5 mma + 1e-3) <= 0.58; LSE 4.8e-5 (saturated softmax)
 AE_ROW, AE_LSE_ABS = 1e-2, 1e-4
 
 
-@bounded([
-    ("ae_sentinels_changed", 0.0), ("ae_nan_in_range", 0.0), ("ae_wg_rope_dv_mismatch", 0.0),
-    ("ae_mma_rope_dv_mismatch", 0.0), ("ae_wg_over_mma_", 1.0), ("ae_wg_lse_abs", AE_LSE_ABS), ("ae_mma_lse_abs", AE_LSE_ABS),
-    *[(f"ae_{i}_{n}_row", AE_ROW) for i in ("wg", "mma") for n in ("o", "dq", "dk", "dv", "rope_dq", "rope_dk")],
-])
+@bounded(_attn_bounds("ae_"))
 def check_attn_edges():
-    """Both attention implementations through the C ABI with explicit strides: separate q / k / v / dO buffers with a
-    batch pitch of S + 3 rows and a row pitch of H + 16 (all padding NaN), outputs inside NaN buffers; S from 1 to 320,
-    Sq < Sk, one head, saturated softmax.  Scored per (batch, head, row) against fp64 attention and its fp64 gradient
-    given the o each backward receives, and wgmma against mma on the same inputs.  The mma backward needs n_heads % 4 == 0, so one-head cases run its forward
-    only."""
+    """Both attention implementations through the C ABI with explicit strides (_attn_case): separate q / k / v / dO
+    buffers with a batch pitch of S + 3 rows and a row pitch of H + 16 (all padding NaN), outputs inside NaN buffers; S
+    from 1 to 320, Sq < Sk, one head, saturated softmax."""
     W = _Worst("ae_")
-    D, scale, floor = 64, 0.125, 1e-3
+    D, scale = 64, 0.125
     cases = [(3, S, S, nh, 1.0) for S in (1, 2, 17, 63, 64, 65, 127, 129, 320) for nh in (1, 4)]
     cases += [(3, Sq, Sk, 4, 1.0) for Sq, Sk in ((1, 300), (5, 70), (64, 129), (65, 200))]
     cases += [(2, 129, 129, 4, 8.0)]
@@ -1714,73 +1797,224 @@ def check_attn_edges():
     for ci, (B, Sq, Sk, nh, amp) in enumerate(cases):
         H = nh * D
         ld = H + 16
-        off = Sk - Sq
         case = f"B{B} Sq{Sq} Sk{Sk} h{nh}" + (f" x{amp:g}" if amp != 1.0 else "")
-
-        def buf(S, seed, a=1.0):
-            vals = randn(B, S, H, scale=a, seed=seed)
-            t = P.nan_buffer((B, S + 3, ld), device=DEV)
-            t[:, :S, :H] = vals
-            return vals.view(B, S, nh, D).transpose(1, 2), t
 
         def st(S):
             return [(S + 3) * ld, ld, D]
 
-        q, qb = buf(Sq, 3000 + 4 * ci, amp)
-        k, kb = buf(Sk, 3001 + 4 * ci, amp)
-        v, vb = buf(Sk, 3002 + 4 * ci)
-        do, dob = buf(Sq, 3003 + 4 * ci)
-        o64, lse64, _, _, _ = P.attn_ref64(q, k, v, do, off, scale)
-        atol = 1e-3 * float(do.double().norm(dim=-1).median())   # row-norm floor on the scale of the inputs
+        def buf(S):
+            t = P.nan_buffer((B, S + 3, ld), device=DEV)
+            return t, (t.data_ptr(), st(S), t[:, :S, :H].view(B, S, nh, D).transpose(1, 2))
+
+        def operand(S, seed, a=1.0):
+            t, desc = buf(S)
+            t[:, :S, :H] = randn(B, S, H, scale=a, seed=seed)
+            return desc
+
+        def new_out(kind):
+            made = [buf(Sq)] if kind == "o" else [buf(Sq), buf(Sk), buf(Sk)]
+            return [(t, (slice(None), slice(0, d[2].shape[2]), slice(0, H))) for t, d in made], [d for _, d in made]
+
+        ins = {"q": operand(Sq, 3000 + 4 * ci, amp), "k": operand(Sk, 3001 + 4 * ci, amp), "v": operand(Sk, 3002 + 4 * ci),
+               "do": operand(Sq, 3003 + 4 * ci)}
         cos, sin = ops.rope_table(inv, Sk)
-        rows = {}
-        for impl, sfx in (("wg", "_wgmma"), ("mma", "")):
-            ob = P.nan_buffer((B, Sq + 3, ld), device=DEV)
-            n_lse = B * nh * Sq
-            lse = torch.full((n_lse + 64,), float("nan"), device=DEV)
-            stt = torch.tensor(st(Sq) + st(Sk) + st(Sk) + st(Sq), dtype=torch.int64)
-            lib.call("b200_attn_causal_fwd" + sfx, qb.data_ptr(), kb.data_ptr(), vb.data_ptr(), ob.data_ptr(), lse.data_ptr(),
-                     stt.data_ptr(), B, nh, Sq, Sk, D, scale, lib.stream())
-            o = ob[:, :Sq, :H].view(B, Sq, nh, D).transpose(1, 2)
-            rows[(impl, "o")] = P.row_worst(o, o64, atol=atol)
-            W.add(impl, case, {"lse_abs": float((lse[:n_lse].view(B, nh, Sq).double() - lse64).abs().max())})
-            W.add("", case, P.sentinel_report(ob, (slice(None), slice(0, Sq), slice(0, H))))
-            W.add("", case, P.sentinel_report(lse, (slice(0, n_lse),)))
-            if impl == "mma" and nh % 4:
-                continue
-            # backward (plain and with the RoPE backward fused into dq / dk), from this implementation's o and lse; the
-            # fp64 reference is the gradient given that o
-            _, _, dq64, dk64, dv64 = P.attn_ref64(q, k, v, do, off, scale, o_in=o)
-            dq64r = P.rope_bwd64(dq64, cos, sin, torch.arange(Sq, device=DEV) + off)
-            dk64r = P.rope_bwd64(dk64, cos, sin, torch.arange(Sk, device=DEV))
-            for rope in (False, True):
-                dq = P.nan_buffer((B, Sq + 3, ld), device=DEV)
-                dk = P.nan_buffer((B, Sk + 3, ld), device=DEV)
-                dv = P.nan_buffer((B, Sk + 3, ld), device=DEV)
-                delta = torch.empty(n_lse, device=DEV)
-                stb = torch.tensor(st(Sq) + st(Sk) + st(Sk) + st(Sq) + st(Sq) + st(Sq) + st(Sk) + st(Sk), dtype=torch.int64)
-                lib.call("b200_attn_causal_bwd" + sfx, qb.data_ptr(), kb.data_ptr(), vb.data_ptr(), ob.data_ptr(),
-                         dob.data_ptr(), lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
-                         stb.data_ptr(), B, nh, Sq, Sk, D, scale, cos.data_ptr() if rope else None,
-                         sin.data_ptr() if rope else None, lib.stream())
-                g = {n: t[:, :S, :H].view(B, S, nh, D).transpose(1, 2) for n, t, S in (("dq", dq, Sq), ("dk", dk, Sk),
-                                                                                    ("dv", dv, Sk))}
-                if rope:
-                    W.add(impl, case, {"rope_dq_row": P.row_worst(g["dq"], dq64r, atol=atol),
-                                       "rope_dk_row": P.row_worst(g["dk"], dk64r, atol=atol),
-                                       "rope_dv_mismatch": float((g["dv"] != dv_plain).sum())})
-                else:
-                    for n, ref in (("dq", dq64), ("dk", dk64), ("dv", dv64)):
-                        rows[(impl, n)] = P.row_worst(g[n], ref, atol=atol)
-                    dv_plain = g["dv"].clone()
-                for t, S in ((dq, Sq), (dk, Sk), (dv, Sk)):
-                    W.add("", case, P.sentinel_report(t, (slice(None), slice(0, S), slice(0, H))))
-        for (impl, n), val in rows.items():
-            W.add(impl, case, {f"{n}_row": val})
-            if impl == "wg" and ("mma", n) in rows:
-                # same semantics, so the wgmma worst row should stay near the mma worst row on the same inputs
-                W.add("wg_over_mma", case, {n: val / (1.5 * rows[("mma", n)] + floor)})
+        _attn_case(W, case, ins, new_out, B, Sq, Sk, nh, cos, sin, scale)
     return W.report()
+
+
+# The score families of the long-context groups, shaped through one "carrier" column of every head: column 31, the
+# slowest-rotating RoPE pair, so that the decode kernel's rotation of the new q (cos >= 0.85 up to position 4095) keeps
+# each family's shape.  Every value is exact in bf16 (powers of two and small integers).
+AL_FAMILIES = ("amp1", "amp4", "sink", "late", "flat")
+_CARRIER = 31
+
+
+def _score_family(fam, q, k, sink_key=64.0):
+    """q, k [..., S, n_heads, D] bf16 (the key position is the index along dim -3) shaped into a score family:
+    "amp1" as given; "amp4" both x4, saturating rows; "sink" q[c] = 2 and k[c] = sink_key at key 0, 0 elsewhere, so
+    key 0 leads every query by about sink_key / 4 - 4 nats; "late" q[c] = 16 and k[c] = (key // 64) / 2, so the scores
+    rise by one nat per 64-key tile (over 0.17 nats of noise) and the running max moves in every tile; "flat" q = 0:
+    every score is 0, attention is uniform and P is exactly 1.
+
+    "late" keeps q's and k's random parts in disjoint RoPE pairs (q x4 where k = 0, k x8 where q / 32), so the ramp
+    carries no noise and neither operand is dominated by the component all rows share.  Both backward kernels round dS
+    to bf16 before dS.K and dS^T.Q: with the ramp's magnitude on k alone, the sum over a dq row, whose dS cancel, scaled
+    that rounding into a worst dq row of 0.1 at S = 4096; on q alone every dk row lay along the carrier and some were
+    near zero (worst 0.48).  Pairs stay within their class under the decode kernel's rotation of q, and the carrier's
+    partner column is 0 in both."""
+    if fam == "amp1":
+        return q, k
+    if fam == "amp4":
+        return q * 4, k * 4
+    if fam == "flat":
+        return torch.zeros_like(q), k
+    kpos = torch.arange(k.shape[-3], device=k.device).view(-1, 1)
+    if fam == "sink":
+        q, k = q.clone(), k.clone()
+        q[..., _CARRIER] = 2.0
+        k[..., _CARRIER] = torch.where(kpos == 0, sink_key, 0.0).to(k.dtype)
+        return q, k
+    D = q.shape[-1]
+    col = torch.arange(D, device=q.device) % (D // 2)
+    q_own = col < D // 4                                   # pairs 0 .. 15: q's random part, k = 0
+    k_own = ~q_own & (col != _CARRIER)                     # pairs 16 .. 30: k's random part, q / 32
+    q = torch.where(q_own, q * 4, q / 32)
+    k = torch.where(k_own, k * 8, torch.zeros_like(k))
+    q[..., _CARRIER], q[..., _CARRIER + D // 2] = 16.0, 0.0
+    k[..., _CARRIER] = (kpos // 64).to(k.dtype) / 2
+    return q, k
+
+
+# Segment layouts the ragged trainer can produce beyond those of tests/test_gpu_ragged.py: 32 one-tile segments; short
+# segments before two long ones, which the longest-first order table interleaves; one 4096-row segment (64 key tiles)
+AL_SEGMENTS = ([64] * 32, [64] * 8 + [1984, 2048], [4096])
+
+
+# measured on an NVIDIA H100 80GB HBM3 at 700 W, both implementations alike: worst row 3.7e-3 (o, B8 S2048 amp1),
+# 7.7e-3 (dq, B8 S2048 sink), 7.3e-3 (dk, B1 S4096 late), 5.0e-3 (dv, B8 S2048 amp4), RoPE backward within 5 %; LSE
+# 2.2e-5 (wgmma) / 2.0e-5 (mma), both at amp4; wgmma / (1.5 mma + 1e-3) <= 0.61; segment mode bit-identical, rows <= 5.0e-3,
+# LSE 1.3e-6.  The row error does not grow with S: the attn_edges bounds stand.  30 s, 3.9 GiB peak device memory.
+@bounded([
+    *_attn_bounds("al_"),
+    ("al_seg_seg_mismatch", 0.0), ("al_seg_sentinels_changed", 0.0), ("al_seg_nan_in_range", 0.0),
+    ("al_seg_row", AE_ROW), ("al_seg_lse_abs", AE_LSE_ABS),
+    ("min:al_key_tiles", 64.0), ("min:al_batched_long_cases", 1.0), ("min:al_families_at_4096", 4.0),
+])
+def check_attn_long():
+    """The attention conformance of attn_edges (_attn_case) at the lengths training runs: the benchmark shape (8, 2048),
+    (2, 2047), (2, 2049), (3, 1000) and (1, 4096) at 16 heads, with q / k / v column views of one packed qkv buffer of
+    row pitch 3H + 64, o / dO / dqkv at their own padded pitches, as ops.attn_causal_fwd / _bwd lay them out (all
+    padding NaN, spare NaN rows under every output); at (8, 2048) and (1, 4096) also the peaked score families of
+    _score_family.  Plus the segment kernels on AL_SEGMENTS, bit-identical per segment to the unsegmented kernel and
+    scored against fp64 (seg_attention_case)."""
+    W = _Worst("al_")
+    D, nh, scale = 64, 16, 0.125
+    H = nh * D
+    ldq, ldo, ldd, lddo = 3 * H + 64, H + 24, 3 * H + 56, H + 40
+    cases = [(8, 2048, f) for f in AL_FAMILIES] + [(1, 4096, f) for f in AL_FAMILIES]
+    cases += [(2, 2047, "amp1"), (2, 2049, "amp1"), (3, 1000, "amp1")]
+    inv = O.default_inv_freq(D).to(BF).to(DEV)
+    key_tiles, batched_long, fams_4096 = 0, 0, set()
+    for ci, (B, S, fam) in enumerate(cases):
+        case = f"B{B} S{S} {fam}"
+        R = B * S
+        vals = randn(B, S, 3, nh, D, seed=7000 + ci)
+        q, k = _score_family(fam, vals[:, :, 0], vals[:, :, 1])
+        qkv = P.nan_buffer((R + 64, ldq), device=DEV)
+        for c, t in enumerate((q, k, vals[:, :, 2])):
+            qkv[:R, c * H:(c + 1) * H] = t.reshape(R, H)
+        dob = P.poisoned(randn(R, H, seed=7100 + ci), R + 64, lddo)
+
+        def desc(t, col, ld):
+            return t.data_ptr() + 2 * col, [S * ld, ld, D], t[:R, col:col + H].view(B, S, nh, D).transpose(1, 2)
+
+        def new_out(kind):
+            if kind == "o":
+                t = P.nan_buffer((R + 64, ldo), device=DEV)
+                return [(t, (slice(0, R), slice(0, H)))], [desc(t, 0, ldo)]
+            t = P.nan_buffer((R + 64, ldd), device=DEV)
+            return [(t, (slice(0, R), slice(0, 3 * H)))], [desc(t, c * H, ldd) for c in range(3)]
+
+        ins = {"q": desc(qkv, 0, ldq), "k": desc(qkv, H, ldq), "v": desc(qkv, 2 * H, ldq), "do": desc(dob, 0, lddo)}
+        cos, sin = ops.rope_table(inv, S)
+        _attn_case(W, case, ins, new_out, B, S, S, nh, cos, sin, scale)
+        key_tiles = max(key_tiles, (S + 63) // 64)
+        batched_long += int(B > 1 and S >= 2048)
+        if S == 4096 and fam != "amp1":
+            fams_4096.add(fam)
+    for segs in AL_SEGMENTS:
+        W.add("seg", f"segments {segs[0]} x{len(segs)}" if len(set(segs)) == 1 else f"segments {segs}",
+              seg_attention_case(segs, nh))
+        key_tiles = max(key_tiles, max(segs) // 64)
+    out = W.report()
+    out["al_key_tiles"], out["al_batched_long_cases"] = float(key_tiles), float(batched_long)
+    out["al_families_at_4096"] = float(len(fams_4096))
+    return out
+
+
+def seg_attention_case(segs, nh):
+    """b200_attn_causal_{fwd,bwd}_seg_wgmma on one packed batch of segments of the given row counts (multiples of 64),
+    nh heads, with the fused RoPE backward and without, outputs in NaN-sentinel buffers: every segment must be
+    bit-identical to b200_attn_causal_{fwd,bwd}_wgmma run on that segment alone (in segment mode the kernels run the same
+    tiles in the same order on the same operands), and is scored per row against fp64.  Returns the metrics without a
+    case tag: sentinel counts, seg_mismatch_* (differing elements), row_* (worst row) and lse_abs."""
+    import midi_model as mm
+    D = 64
+    H = nh * D
+    N = sum(segs)
+    ldq, ldo = 3 * H + 64, H + 64
+    g = torch.Generator(device=DEV).manual_seed(7)
+    rnd = lambda *s: torch.randn(*s, generator=g, device=DEV).to(BF)
+    qkvb = P.poisoned(rnd(N, 3 * H), N + 64, ldq)
+    dob = P.poisoned(rnd(N, H), N + 64, ldo)
+    seg = mm._ragged_layout(list(segs), 1, torch.device(DEV))[1]
+    cos, sin = ops.rope_table(O.default_inv_freq(D).to(BF).to(DEV), max(segs))
+    st_f = torch.tensor([ldq, D] * 3 + [ldo, D], dtype=torch.int64)
+    st_b = torch.tensor([ldq, D] * 3 + [ldo, D] * 2 + [ldq, D] * 3, dtype=torch.int64)
+    nb = lambda r, c: P.nan_buffer((r, c), device=DEV)
+    m = {}
+    # ---- segment mode
+    q, k, v = (qkvb.data_ptr() + 2 * i * H for i in range(3))
+    ob = nb(N + 64, ldo)
+    lse = torch.full((nh * N + 64,), float("nan"), device=DEV)
+    lib.call("b200_attn_causal_fwd_seg_wgmma", q, k, v, ob.data_ptr(), lse.data_ptr(), st_f.data_ptr(), N // 64, nh, D,
+             0.125, seg.tiles.data_ptr(), seg.order.data_ptr(), lib.stream())
+    m.update({f"{k_}_fwd": v_ for k_, v_ in P.sentinel_report(ob, (slice(0, N), slice(0, H))).items()})
+    m.update({f"{k_}_lse": v_ for k_, v_ in P.sentinel_report(lse, (slice(0, nh * N),)).items()})
+    grads = {}
+    for rope in (False, True):
+        dq = nb(N + 64, ldq)
+        delta = torch.empty(nh * N, device=DEV)
+        lib.call("b200_attn_causal_bwd_seg_wgmma", q, k, v, ob.data_ptr(), dob.data_ptr(), lse.data_ptr(), delta.data_ptr(),
+                 dq.data_ptr(), dq.data_ptr() + 2 * H, dq.data_ptr() + 4 * H, st_b.data_ptr(), N // 64, nh, D, 0.125,
+                 cos.data_ptr() if rope else None, sin.data_ptr() if rope else None, seg.tiles.data_ptr(),
+                 seg.order.data_ptr(), lib.stream())
+        m.update({f"{k_}_bwd_rope{int(rope)}": v_
+                  for k_, v_ in P.sentinel_report(dq, (slice(0, N), slice(0, 3 * H))).items()})
+        grads[rope] = dq
+    lse = lse[:nh * N].view(nh, N)
+    # ---- each segment alone through the unsegmented kernel, and fp64
+    mism = {"o": 0, "lse": 0, "dqkv": 0, "dqkv_rope": 0}
+    worst = {}
+    r0 = 0
+    for R in segs:
+        base = qkvb.data_ptr() + r0 * ldq * 2
+        st1 = torch.tensor([R * ldq, ldq, D] * 3 + [R * ldo, ldo, D], dtype=torch.int64)
+        o1 = nb(R, ldo)
+        l1 = torch.empty(nh * R, device=DEV)
+        lib.call("b200_attn_causal_fwd_wgmma", base, base + 2 * H, base + 4 * H, o1.data_ptr(), l1.data_ptr(), st1.data_ptr(),
+                 1, nh, R, R, D, 0.125, lib.stream())
+        mism["o"] += int((o1[:, :H] != ob[r0:r0 + R, :H]).sum())
+        mism["lse"] += int((l1.view(nh, R) != lse[:, r0:r0 + R]).sum())
+        stb1 = torch.tensor([R * ldq, ldq, D] * 3 + [R * ldo, ldo, D] * 2 + [R * ldq, ldq, D] * 3, dtype=torch.int64)
+        for rope in (False, True):
+            d1 = nb(R, ldq)
+            delta = torch.empty(nh * R, device=DEV)
+            lib.call("b200_attn_causal_bwd_wgmma", base, base + 2 * H, base + 4 * H, o1.data_ptr(),
+                     dob.data_ptr() + r0 * ldo * 2, l1.data_ptr(), delta.data_ptr(), d1.data_ptr(), d1.data_ptr() + 2 * H,
+                     d1.data_ptr() + 4 * H, stb1.data_ptr(), 1, nh, R, R, D, 0.125, cos.data_ptr() if rope else None,
+                     sin.data_ptr() if rope else None, lib.stream())
+            mism["dqkv_rope" if rope else "dqkv"] += int((d1[:, :3 * H] != grads[rope][r0:r0 + R, :3 * H]).sum())
+        heads = lambda t, c0: t[r0:r0 + R, c0:c0 + H].view(R, nh, D).transpose(0, 1)
+        qs, ks, vs, dos, os_ = heads(qkvb, 0), heads(qkvb, H), heads(qkvb, 2 * H), heads(dob, 0), heads(ob, 0)
+        o64, lse64, dq64, dk64, dv64 = (t[0] for t in _attn_ref64_parts(qs[None], ks[None], vs[None], dos[None], 0, 0.125,
+                                                                         o_in=os_[None]))
+        atol = 1e-3 * float(dos.double().norm(dim=-1).median())
+        sc = {"o": P.row_worst(os_, o64, atol=atol), "lse_abs": float((lse[:, r0:r0 + R].double() - lse64).abs().max())}
+        for rope in (False, True):
+            gq, gk, gv = (heads(grads[rope], c) for c in (0, H, 2 * H))
+            rq = P.rope_bwd64(dq64, cos, sin, slice(0, R)) if rope else dq64
+            rk = P.rope_bwd64(dk64, cos, sin, slice(0, R)) if rope else dk64
+            sfx = "_rope" if rope else ""
+            sc["dq" + sfx] = P.row_worst(gq, rq, atol=atol)
+            sc["dk" + sfx] = P.row_worst(gk, rk, atol=atol)
+            sc["dv" + sfx] = P.row_worst(gv, dv64, atol=atol)
+        for n, val in sc.items():
+            worst[n] = max(worst.get(n, 0.0), val)
+        r0 += R
+    m.update({f"seg_mismatch_{n}": float(c) for n, c in mism.items()})
+    m.update({(n if n == "lse_abs" else f"row_{n}"): val for n, val in worst.items()})
+    return m
 
 
 # ------------------------------------------------------------------------------------------ decode conformance groups
@@ -1956,6 +2190,51 @@ def _same(a, b):
     return (a == b) | (torch.isnan(a.float()) & torch.isnan(b.float()))
 
 
+def _kv_append(qkv, kp, vp, bt, mp, page, nh, D, Bn, s_new, pos0, dev):
+    """b200_kv_append of s_new rows per batch row at pos0, passed by value or (dev) from the device."""
+    pd = torch.tensor([pos0], dtype=torch.int32, device=DEV) if dev else None
+    lib.call("b200_kv_append", qkv.data_ptr(), kp.data_ptr(), vp.data_ptr(), bt.data_ptr(), mp, page, nh, D, Bn, s_new,
+             0 if dev else pos0, lib.ptr(pd), qkv.stride(0), lib.stream())
+
+
+def _fused_decode_case(W, kern, case, qkv, pools, pools0, expect, bt, mp, page, cos, sin, Bn, nh, D, pos, dev, max_T,
+                       n_split, ref, atol):
+    """b200_attn_decode_fused of the new token rows qkv at position pos (by value or from the device) on the pools
+    reset to pools0: the pools must equal `expect` (the appended slots, no other slot touched) and the output must
+    match ref per (row, head); the CTA kernels must also be bit-identical to b200_rope_qk + b200_kv_append +
+    b200_attn_decode on the same inputs."""
+    kp, vp = pools
+    k0, v0 = pools0
+    kexp, vexp = expect
+    H, scale = nh * D, 1.0 / math.sqrt(D)
+    kp.copy_(k0)
+    vp.copy_(v0)
+    pdv = torch.tensor([pos], dtype=torch.int32, device=DEV) if dev else None
+    o = P.nan_buffer((Bn + 1, H + 8), device=DEV)
+    nbytes = lib.query("b200_attn_decode_workspace_bytes", Bn, nh, D, n_split)
+    ws = torch.full((nbytes // 4,), float("nan"), device=DEV)
+    lib.call("b200_attn_decode_fused", qkv.data_ptr(), kp.data_ptr(), vp.data_ptr(), bt.data_ptr(), mp, page,
+             cos.data_ptr(), sin.data_ptr(), o.data_ptr(), Bn, nh, D, 0 if dev else pos, lib.ptr(pdv), max_T,
+             qkv.stride(0), o.stride(0), scale, n_split, ws.data_ptr(), nbytes, lib.stream())
+    W.add(kern, case, {"append_mismatch": float((~_same(kp, kexp)).sum() + (~_same(vp, vexp)).sum()),
+                       "o_row": P.row_worst(o[:Bn, :H].view(Bn, nh, 1, D), ref, atol=atol)})
+    W.add(kern, case, P.sentinel_report(o, (slice(0, Bn), slice(0, H))))
+    if kern == "warp256":
+        return
+    # the unfused launches on the same inputs: b200_rope_qk + b200_kv_append + b200_attn_decode
+    q2 = qkv.clone()
+    lib.call("b200_rope_qk", q2.data_ptr(), cos.data_ptr(), sin.data_ptr(), Bn, 1, H, D, q2.stride(0), 0,
+             pos, None, lib.stream())
+    k2, v2 = k0.clone(), v0.clone()
+    _kv_append(q2, k2, v2, bt, mp, page, nh, D, Bn, 1, pos, False)
+    o2 = P.nan_buffer((Bn + 1, H + 8), device=DEV)
+    lib.call("b200_attn_decode", q2.data_ptr(), k2.data_ptr(), v2.data_ptr(), bt.data_ptr(), mp, page,
+             o2.data_ptr(), Bn, 1, nh, D, pos, None, max_T, q2.stride(0), o2.stride(0), scale, n_split,
+             ws.data_ptr(), nbytes, lib.stream())
+    W.add(kern, case, {"vs_unfused_mismatch": float((~_same(o, o2)).sum() + (~_same(kp, k2)).sum()
+                                                    + (~_same(vp, v2)).sum())})
+
+
 # same card: appends bit-exact, nothing else written; worst (row, head) against fp64 attention 3.3e-3 (b200_attn_decode,
 # head_dim 64), 2.7e-3 (256), 2.8e-3 / 2.4e-3 / 2.7e-3 (fused: 64-dim CTA, 256-dim CTA, warp kernel); fused CTA kernels
 # bit-identical to RoPE + append + b200_attn_decode; 302 splits without keys ran
@@ -1974,13 +2253,7 @@ def check_decode_attn_conformance():
     leading dimensions; outputs per (row, head) against fp64 attention over the pools."""
     import decode_reference as DR
     W = _Worst("da_")
-    floor = 1e-3
     n_empty_splits = 0
-
-    def append(qkv, kp, vp, bt, mp, page, nh, D, Bn, s_new, pos0, dev):
-        pd = torch.tensor([pos0], dtype=torch.int32, device=DEV) if dev else None
-        lib.call("b200_kv_append", qkv.data_ptr(), kp.data_ptr(), vp.data_ptr(), bt.data_ptr(), mp, page, nh, D, Bn, s_new,
-                 0 if dev else pos0, lib.ptr(pd), qkv.stride(0), lib.stream())
 
     # ---- b200_kv_append
     for nh, D, page, cap in ((16, 64, 64, 192), (4, 256, 8, 24)):
@@ -1992,7 +2265,7 @@ def check_decode_attn_conformance():
                     kp, vp, bt, mp = _paged_pools(nh, D, page, Bn, cap, seed=pos0 + s_new)
                     vals = randn(Bn * s_new, 3 * H, seed=D + s_new + pos0)
                     qkv = P.poisoned(vals, Bn * s_new + 1, 3 * H + 24)
-                    append(qkv, kp, vp, bt, mp, page, nh, D, Bn, s_new, pos0, dev)
+                    _kv_append(qkv, kp, vp, bt, mp, page, nh, D, Bn, s_new, pos0, dev)
                     v4 = vals.view(Bn, s_new, 3, nh, D)
                     bad = 0
                     for b in range(Bn):
@@ -2010,7 +2283,7 @@ def check_decode_attn_conformance():
             max_T = T if T == 2048 else T + 17               # 2048 / 2 splits: a chunk of exactly 1024 keys
             kp, vp, bt, mp = _paged_pools(nh, D, page, Bn, max_T, seed=T + D)
             hist = randn(Bn * T, 3 * H, seed=T * 3 + D)
-            append(hist, kp, vp, bt, mp, page, nh, D, Bn, T, 0, False)
+            _kv_append(hist, kp, vp, bt, mp, page, nh, D, Bn, T, 0, False)
             k0, v0 = kp.clone(), vp.clone()
             atol = 1e-3 * float(hist[:, 2 * H:].double().view(-1, D).norm(dim=-1).median())
             for s_q in (1, 5, 8):
@@ -2053,7 +2326,7 @@ def check_decode_attn_conformance():
             max_T = cap if kern != "cta64" else T + 7
             kp, vp, bt, mp = _paged_pools(nh, D, page, Bn, cap, seed=T + D + 1)
             if pos:
-                append(randn(Bn * pos, 3 * H, seed=T + D + 2), kp, vp, bt, mp, page, nh, D, Bn, pos, 0, False)
+                _kv_append(randn(Bn * pos, 3 * H, seed=T + D + 2), kp, vp, bt, mp, page, nh, D, Bn, pos, 0, False)
             k0, v0 = kp.clone(), vp.clone()
             vals = randn(Bn, 3 * H, seed=T + D + 3)
             qkv = P.poisoned(vals, Bn + 1, 3 * H + 8)
@@ -2071,35 +2344,100 @@ def check_decode_attn_conformance():
                 if (max_T + n_split - 1) // n_split > 1024:
                     continue
                 for dev in (False, True):
-                    case = f"{kern} T{T} n_split{n_split}" + (" pos_dev" if dev else "")
-                    kp.copy_(k0)
-                    vp.copy_(v0)
-                    pdv = torch.tensor([pos], dtype=torch.int32, device=DEV) if dev else None
-                    o = P.nan_buffer((Bn + 1, H + 8), device=DEV)
-                    nbytes = lib.query("b200_attn_decode_workspace_bytes", Bn, nh, D, n_split)
-                    ws = torch.full((nbytes // 4,), float("nan"), device=DEV)
-                    lib.call("b200_attn_decode_fused", qkv.data_ptr(), kp.data_ptr(), vp.data_ptr(), bt.data_ptr(), mp, page,
-                             cos.data_ptr(), sin.data_ptr(), o.data_ptr(), Bn, nh, D, 0 if dev else pos, lib.ptr(pdv), max_T,
-                             qkv.stride(0), o.stride(0), scale, n_split, ws.data_ptr(), nbytes, lib.stream())
-                    W.add(kern, case, {"append_mismatch": float((~_same(kp, kexp)).sum() + (~_same(vp, vexp)).sum()),
-                                       "o_row": P.row_worst(o[:Bn, :H].view(Bn, nh, 1, D), ref, atol=atol)})
-                    W.add(kern, case, P.sentinel_report(o, (slice(0, Bn), slice(0, H))))
-                    if kern == "warp256":
-                        continue
-                    # the unfused launches on the same inputs: b200_rope_qk + b200_kv_append + b200_attn_decode
-                    q2 = qkv.clone()
-                    lib.call("b200_rope_qk", q2.data_ptr(), cos.data_ptr(), sin.data_ptr(), Bn, 1, H, D, q2.stride(0), 0,
-                             pos, None, lib.stream())
-                    k2, v2 = k0.clone(), v0.clone()
-                    append(q2, k2, v2, bt, mp, page, nh, D, Bn, 1, pos, False)
-                    o2 = P.nan_buffer((Bn + 1, H + 8), device=DEV)
-                    lib.call("b200_attn_decode", q2.data_ptr(), k2.data_ptr(), v2.data_ptr(), bt.data_ptr(), mp, page,
-                             o2.data_ptr(), Bn, 1, nh, D, pos, None, max_T, q2.stride(0), o2.stride(0), scale, n_split,
-                             ws.data_ptr(), nbytes, lib.stream())
-                    W.add(kern, case, {"vs_unfused_mismatch": float((~_same(o, o2)).sum() + (~_same(kp, k2)).sum()
-                                                                    + (~_same(vp, v2)).sum())})
+                    _fused_decode_case(W, kern, f"{kern} T{T} n_split{n_split}" + (" pos_dev" if dev else ""), qkv,
+                                       (kp, vp), (k0, v0), (kexp, vexp), bt, mp, page, cos, sin, Bn, nh, D, pos, dev, max_T,
+                                       n_split, ref, atol)
     out = W.report()
     out["da_empty_splits_run"] = float(n_empty_splits)
+    return out
+
+# Generation's longest contexts: 4096-event pools read in n_split chunks and combined.  Measured on an NVIDIA H100 80GB
+# HBM3 at 700 W: worst (row, head) 3.7e-3 (b200_attn_decode, late T2049 B16 s_q8 n_split8), 3.1e-3 (fused, amp1 T2049
+# B16 n_split4); appends bit-exact, no other pool slot or sentinel written, fused bit-identical to the unfused launches;
+# 156672 combines with split maxima more than 20 nats apart.  3 s, 2.6 GiB peak device memory.
+DL_TS = (2049, 3000, 4095, 4096)
+DL_SPLITS = (4, 8, 16, 32)      # 4: the fewest that keep a chunk of 4096 keys at <= 1024; 16: what generate runs
+DL_FAMILIES = ("amp1", "sink", "late", "flat")
+
+
+@bounded([
+    ("dl_attn_sentinels_changed", 0.0), ("dl_attn_nan_in_range", 0.0), ("dl_attn_pool_changed", 0.0),
+    ("dl_attn_o_row", 1.5e-2), ("dl_cta64_o_row", 1.5e-2),
+    *[(f"dl_cta64_{m}", 0.0) for m in ("append_mismatch", "sentinels_changed", "nan_in_range", "vs_unfused_mismatch")],
+    ("min:dl_splits_at_4096", 4.0), ("min:dl_combines_over_20_nats", 1.0),
+])
+def check_decode_attn_long():
+    """b200_attn_decode (s_q 1 and 8) and b200_attn_decode_fused (64-dim CTA kernel) as decode_attn_edges runs them, at
+    max_T 4096 with T from 2049 to 4096, n_split 4 to 32, 1 and 16 batch rows and the score families of _score_family
+    (the sink 28 to 32 nats above every other key, so the combine scales the other splits' partials down by more than
+    20 nats).  Positions by value and from the device; outputs per (row, head) against fp64 over the pools, no pool slot
+    but the appended ones written, the fused kernel bit-identical to RoPE + append + b200_attn_decode."""
+    import decode_reference as DR
+    W = _Worst("dl_")
+    nh, D, page, max_T = 16, 64, 64, 4096
+    H, scale = nh * D, 1.0 / math.sqrt(D)
+    cos, sin = ops.rope_table(O.default_inv_freq(D).to(BF).to(DEV), max_T)
+    splits_4096, wide = set(), 0
+    for fi, fam in enumerate(DL_FAMILIES):
+        for ti, T in enumerate(DL_TS):
+            for Bn in (1, 16):
+                seed = 8000 + 100 * fi + 10 * ti + Bn
+                vals = randn(Bn, T, 3, nh, D, seed=seed)
+                q, k = _score_family(fam, vals[:, :, 0], vals[:, :, 1], sink_key=128.0)
+                qkv_t = torch.stack([q, k, vals[:, :, 2]], 2)          # [Bn, T, 3, nh, D]: the qkv row of position t
+                atol = 1e-3 * float(vals[:, :, 2].double().norm(dim=-1).median())
+                # ---- b200_attn_decode: the queries of the last s_q positions over all T keys
+                kp, vp, bt, mp = _paged_pools(nh, D, page, Bn, max_T, seed=seed)
+                _kv_append(qkv_t.reshape(Bn * T, 3 * H), kp, vp, bt, mp, page, nh, D, Bn, T, 0, False)
+                k0, v0 = kp.clone(), vp.clone()
+                for s_q in (1, 8):
+                    past, rows = T - s_q, Bn * s_q
+                    qv = q[:, past:]
+                    Q = P.poisoned(qv.reshape(rows, H), rows + 1, H + 24)
+                    ref = torch.stack([DR.paged_attention64(qv[b].transpose(0, 1), kp, vp, bt, page, b, T, scale)
+                                       for b in range(Bn)])
+                    for n_split in DL_SPLITS:
+                        for dev in (False, True):
+                            case = f"{fam} T{T} B{Bn} s_q{s_q} n_split{n_split}" + (" past_dev" if dev else "")
+                            pdv = torch.tensor([past], dtype=torch.int32, device=DEV) if dev else None
+                            o = P.nan_buffer((rows + 2, H + 16), device=DEV)
+                            nbytes = lib.query("b200_attn_decode_workspace_bytes", rows, nh, D, n_split)
+                            ws = torch.full((nbytes // 4,), float("nan"), device=DEV)
+                            lib.call("b200_attn_decode", Q.data_ptr(), kp.data_ptr(), vp.data_ptr(), bt.data_ptr(), mp,
+                                     page, o.data_ptr(), Bn, s_q, nh, D, 0 if dev else past, lib.ptr(pdv), max_T,
+                                     Q.stride(0), o.stride(0), scale, n_split, ws.data_ptr(), nbytes, lib.stream())
+                            got = o[:rows, :H].view(Bn, s_q, nh, D).transpose(1, 2)
+                            W.add("attn", case, {"o_row": P.row_worst(got, ref, atol=atol)})
+                            W.add("attn", case, P.sentinel_report(o, (slice(0, rows), slice(0, H))))
+                            # the split maxima the combine pass rescaled by: (m, l, o[D]) records per (row, head, split)
+                            m = ws[:rows * nh * n_split * (D + 2)].view(rows * nh, n_split, D + 2)[:, :, 0]
+                            wide += int((m.amax(1) - m.amin(1) > 20).sum())
+                            if T == max_T:
+                                splits_4096.add(n_split)
+                W.add("attn", f"{fam} T{T} B{Bn}", {"pool_changed": float((~_same(kp, k0)).sum() + (~_same(vp, v0)).sum())})
+                # ---- b200_attn_decode_fused: the token at position T - 1 over the T - 1 before it
+                pos = T - 1
+                kp, vp, bt, mp = _paged_pools(nh, D, page, Bn, max_T, seed=seed + 1)
+                _kv_append(qkv_t[:, :pos].reshape(Bn * pos, 3 * H), kp, vp, bt, mp, page, nh, D, Bn, pos, 0, False)
+                k0, v0 = kp.clone(), vp.clone()
+                v4 = qkv_t[:, pos]
+                qkv = P.poisoned(v4.reshape(Bn, 3 * H), Bn + 1, 3 * H + 8)
+                q64, _ = _rope_chain64(v4[:, 0], cos, sin, pos)
+                k64, _ = _rope_chain64(v4[:, 1], cos, sin, pos)
+                kexp, vexp = k0.clone(), v0.clone()
+                for b in range(Bn):
+                    pg = int(bt[b, pos // page])
+                    kexp[pg, :, pos % page] = k64[b].to(BF)
+                    vexp[pg, :, pos % page] = v4[b, 2]
+                ref = torch.stack([DR.paged_attention64(q64[b][:, None], kexp, vexp, bt, page, b, T, scale)
+                                   for b in range(Bn)])
+                for n_split in DL_SPLITS:
+                    for dev in (False, True):
+                        _fused_decode_case(W, "cta64", f"{fam} T{T} B{Bn} n_split{n_split}" + (" pos_dev" if dev else ""),
+                                           qkv, (kp, vp), (k0, v0), (kexp, vexp), bt, mp, page, cos, sin, Bn, nh, D, pos,
+                                           dev, max_T, n_split, ref, atol)
+    out = W.report()
+    out["dl_splits_at_4096"], out["dl_combines_over_20_nats"] = float(len(splits_4096)), float(wide)
     return out
 
 
@@ -3457,7 +3795,8 @@ GROUPS = {
     "gemm_exact": check_gemm_exact, "decode_paged": check_decode_paged, "lora_train": check_lora_train,
     "model_vs_hf": check_model_vs_hf, "model_medium_long": check_model_medium_long,
     "gemm_matrix": check_gemm_matrix, "gemm_epilogues": check_gemm_epilogues, "attn_edges": check_attn_edges,
-    "gemv_matrix": check_gemv_conformance, "decode_attn_edges": check_decode_attn_conformance,
+    "attn_long": check_attn_long, "gemv_matrix": check_gemv_conformance, "decode_attn_edges": check_decode_attn_conformance,
+    "decode_attn_long": check_decode_attn_long,
     "sampler_exact": check_sampler_conformance, "persist_vs_phase": check_persist_vs_phase,
     "persist_token_exact": check_persist_token_exact, "persist_multi_event": check_persist_multi_event,
     "embed_exact": check_embed_conformance, "rmsnorm_exact": check_rmsnorm_conformance, "rope_exact": check_rope_conformance,

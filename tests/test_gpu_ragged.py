@@ -54,85 +54,8 @@ def _tables(seg_rows):
 @pytest.mark.parametrize("segs", [[64], [64, 192, 64, 1216, 128], [2048]], ids=["one_tile", "mixed", "s2048"])
 @pytest.mark.parametrize("nh", [1, 16])
 def test_segment_attention_kernels(segs, nh):
-    import torch
-    import parity_metrics as P
-    from oracle import midi_oracle as O
-    from midi_b200 import lib, ops
-    torch.manual_seed(len(segs) * 100 + nh)
-    H = nh * D
-    N = sum(segs)
-    ldq, ldo = 3 * H + 64, H + 64
-    g = torch.Generator(device="cuda").manual_seed(7)
-    rnd = lambda *s: torch.randn(*s, generator=g, device="cuda").to(torch.bfloat16)
-    qkvb = P.poisoned(rnd(N, 3 * H), N + 64, ldq)
-    dob = P.poisoned(rnd(N, H), N + 64, ldo)
-    seg = _tables(segs)
-    cos, sin = ops.rope_table(O.default_inv_freq(D).to(torch.bfloat16).cuda(), max(segs))
-    st_f = torch.tensor([ldq, D] * 3 + [ldo, D], dtype=torch.int64)
-    st_b = torch.tensor([ldq, D] * 3 + [ldo, D] * 2 + [ldq, D] * 3, dtype=torch.int64)
-    nb = lambda r, c: P.nan_buffer((r, c), device="cuda")
-    m = {}
     tag = f"{'-'.join(map(str, segs))}_h{nh}"
-    # ---- segment mode
-    q, k, v = (qkvb.data_ptr() + 2 * i * H for i in range(3))
-    ob = nb(N + 64, ldo)
-    lse = torch.full((nh * N + 64,), float("nan"), device="cuda")
-    lib.call("b200_attn_causal_fwd_seg_wgmma", q, k, v, ob.data_ptr(), lse.data_ptr(), st_f.data_ptr(), N // 64, nh, D,
-             0.125, seg.tiles.data_ptr(), seg.order.data_ptr(), lib.stream())
-    m.update({f"{k_}_fwd_{tag}": v_ for k_, v_ in P.sentinel_report(ob, (slice(0, N), slice(0, H))).items()})
-    m.update({f"{k_}_lse_{tag}": v_ for k_, v_ in P.sentinel_report(lse, (slice(0, nh * N),)).items()})
-    grads = {}
-    for rope in (False, True):
-        dq = nb(N + 64, ldq)
-        delta = torch.empty(nh * N, device="cuda")
-        lib.call("b200_attn_causal_bwd_seg_wgmma", q, k, v, ob.data_ptr(), dob.data_ptr(), lse.data_ptr(), delta.data_ptr(),
-                 dq.data_ptr(), dq.data_ptr() + 2 * H, dq.data_ptr() + 4 * H, st_b.data_ptr(), N // 64, nh, D, 0.125,
-                 cos.data_ptr() if rope else None, sin.data_ptr() if rope else None, seg.tiles.data_ptr(),
-                 seg.order.data_ptr(), lib.stream())
-        m.update({f"{k_}_bwd_{tag}_rope{int(rope)}": v_ for k_, v_ in P.sentinel_report(dq, (slice(0, N), slice(0, 3 * H))).items()})
-        grads[rope] = dq
-    lse = lse[:nh * N].view(nh, N)
-    # ---- each segment alone through the unsegmented kernel, and fp64
-    mism = {"o": 0, "lse": 0, "dqkv": 0, "dqkv_rope": 0}
-    worst = {}
-    r0 = 0
-    for R in segs:
-        base = qkvb.data_ptr() + r0 * ldq * 2
-        st1 = torch.tensor([R * ldq, ldq, D] * 3 + [R * ldo, ldo, D], dtype=torch.int64)
-        o1 = nb(R, ldo)
-        l1 = torch.empty(nh * R, device="cuda")
-        lib.call("b200_attn_causal_fwd_wgmma", base, base + 2 * H, base + 4 * H, o1.data_ptr(), l1.data_ptr(), st1.data_ptr(),
-                 1, nh, R, R, D, 0.125, lib.stream())
-        mism["o"] += int((o1[:, :H] != ob[r0:r0 + R, :H]).sum())
-        mism["lse"] += int((l1.view(nh, R) != lse[:, r0:r0 + R]).sum())
-        stb1 = torch.tensor([R * ldq, ldq, D] * 3 + [R * ldo, ldo, D] * 2 + [R * ldq, ldq, D] * 3, dtype=torch.int64)
-        for rope in (False, True):
-            d1 = nb(R, ldq)
-            delta = torch.empty(nh * R, device="cuda")
-            lib.call("b200_attn_causal_bwd_wgmma", base, base + 2 * H, base + 4 * H, o1.data_ptr(),
-                     dob.data_ptr() + r0 * ldo * 2, l1.data_ptr(), delta.data_ptr(), d1.data_ptr(), d1.data_ptr() + 2 * H,
-                     d1.data_ptr() + 4 * H, stb1.data_ptr(), 1, nh, R, R, D, 0.125, cos.data_ptr() if rope else None,
-                     sin.data_ptr() if rope else None, lib.stream())
-            mism["dqkv_rope" if rope else "dqkv"] += int((d1[:, :3 * H] != grads[rope][r0:r0 + R, :3 * H]).sum())
-        heads = lambda t, c0: t[r0:r0 + R, c0:c0 + H].view(R, nh, D).transpose(0, 1)
-        qs, ks, vs, dos, os_ = heads(qkvb, 0), heads(qkvb, H), heads(qkvb, 2 * H), heads(dob, 0), heads(ob, 0)
-        o64, lse64, dq64, dk64, dv64 = P.attn_ref64(qs, ks, vs, dos, 0, o_in=os_)
-        atol = 1e-3 * float(dos.double().norm(dim=-1).median())
-        sc = {"o": P.row_worst(os_, o64, atol=atol), "lse_abs": float((lse[:, r0:r0 + R].double() - lse64).abs().max())}
-        for rope in (False, True):
-            gq, gk, gv = (heads(grads[rope], c) for c in (0, H, 2 * H))
-            rq = P.rope_bwd64(dq64, cos, sin, slice(0, R)) if rope else dq64
-            rk = P.rope_bwd64(dk64, cos, sin, slice(0, R)) if rope else dk64
-            sfx = "_rope" if rope else ""
-            sc["dq" + sfx] = P.row_worst(gq, rq, atol=atol)
-            sc["dk" + sfx] = P.row_worst(gk, rk, atol=atol)
-            sc["dv" + sfx] = P.row_worst(gv, dv64, atol=atol)
-        for n, val in sc.items():
-            worst[n] = max(worst.get(n, 0.0), val)
-        r0 += R
-    m.update({f"seg_mismatch_{n}_{tag}": float(c) for n, c in mism.items()})
-    m.update({(n if n == "lse_abs" else f"row_{n}") + f"_{tag}": val for n, val in worst.items()})
-    assert_within(m, BOUNDS)
+    assert_within({f"{k}_{tag}": v for k, v in G.seg_attention_case(segs, nh).items()}, BOUNDS)
 
 
 @pytest.mark.gpu
