@@ -4,7 +4,8 @@ attention references they are scored against, and the one check that judges ever
 
 Global norms hide localized errors: a wrong 8-column group in one row of a 1000 x 1024 GEMM, or a zeroed last row of
 one attention head, moves a relative Frobenius norm by less than its usual bound.  These helpers score the worst
-element or the worst row instead.  Pure PyTorch on any device, so tests/test_parity_metrics.py can show on the CPU that
+element or the worst row instead; grad_report does the same for every gradient of a backward pass, against the fp64
+stack (stack64, train_loss64) and as a ratio to the bf16 eager oracle's error.  Pure PyTorch on any device, so tests/test_parity_metrics.py can show on the CPU that
 each metric fails on the corruptions it is meant to catch."""
 from __future__ import annotations
 
@@ -236,3 +237,148 @@ def swiglu_bwd64(gu, dact):
     g, u, d = gu[:, :I].double(), gu[:, I:].double(), dact.double()
     sg = torch.sigmoid(g)
     return torch.cat([d * u * sg * (1 + g * (1 - sg)), d * g * sg], 1)
+
+
+# ------------------------------------------------------------------------------------------ fp64 stack, gradient report
+def stack64(sd, cfg, x, cos, sin, lengths=None):
+    """One Llama stack (hf modeling_llama.py:303-332, :421) entirely in float64 and differentiable by torch autograd:
+    RMSNorm, q/k/v, RoPE from the given tables, causal softmax over 1/sqrt(D) scores, o_proj with residual, SwiGLU MLP
+    with residual, final norm.  Unlike oracle.midi_oracle.llama_stack nothing is cast to fp32 on the way.
+
+    sd     : {parameter name: tensor} under cfg.prefix (layers 0 .. cfg.n_layer - 1 and the final norm), upcast here;
+             LoRA runs pass oracle.midi_oracle.lora_effective_sd over fp64 leaves
+    x      : (B, S, H) inputs_embeds
+    cos/sin: RoPE tables [>= S, D/2] indexed by position (the engine's ops.rope_table, upcast)
+    lengths: x is (1, sum(lengths), H) holding consecutive sequences, each run alone from position 0 (packed rows)."""
+    if lengths is not None:
+        parts = torch.split(x, [int(n) for n in lengths], dim=1)
+        return torch.cat([stack64(sd, cfg, t, cos, sin) for t in parts], 1)
+    B, S, H = x.shape
+    nh = cfg.n_head
+    D = H // nh
+    c, s = cos[:S].double(), sin[:S].double()
+    mask = torch.ones(S, S, dtype=torch.bool, device=x.device).triu(1)
+    p = cfg.prefix
+
+    def w(name):
+        return sd[name].double()
+
+    def norm(t, g):
+        return g * (t * torch.rsqrt(t.pow(2).mean(-1, keepdim=True) + cfg.eps))
+
+    def rope(t):
+        t1, t2 = t[..., :D // 2], t[..., D // 2:]
+        return torch.cat((t1 * c - t2 * s, t2 * c + t1 * s), -1)
+
+    x = x.double()
+    for l in range(cfg.n_layer):
+        pre = f"{p}.layers.{l}."
+        n1 = norm(x, w(pre + "input_layernorm.weight"))
+        q, k, v = (torch.nn.functional.linear(n1, w(pre + f"self_attn.{t}_proj.weight")).view(B, S, nh, D).transpose(1, 2)
+                   for t in "qkv")
+        sc = (rope(q) @ rope(k).transpose(-1, -2)) * (1.0 / math.sqrt(D))
+        a = torch.softmax(sc.masked_fill(mask, float("-inf")), -1) @ v
+        x = x + torch.nn.functional.linear(a.transpose(1, 2).reshape(B, S, H), w(pre + "self_attn.o_proj.weight"))
+        n2 = norm(x, w(pre + "post_attention_layernorm.weight"))
+        act = torch.nn.functional.silu(torch.nn.functional.linear(n2, w(pre + "mlp.gate_proj.weight")))
+        x = x + torch.nn.functional.linear(act * torch.nn.functional.linear(n2, w(pre + "mlp.up_proj.weight")),
+                                           w(pre + "mlp.down_proj.weight"))
+    return norm(x, w(f"{p}.norm.weight"))
+
+
+def train_loss64(sd, cfg, batch, rope_net, rope_tok, sample_idx=None):
+    """train.py:168-185 in float64 over stack64: the embedding sum (pad rows contribute nothing), the event-level stack,
+    the token-level input [hidden, embed(y[:, :-1])], the token-level stack, lm_head and the mean cross-entropy over
+    non-pad targets.  cfg: oracle.midi_oracle.ModelCfg; rope_net / rope_tok: (cos, sin) of each stack;
+    sample_idx: train.py --sample-seq's event positions (negative ones count from the end)."""
+    F = torch.nn.functional
+    x, y = batch[:, :-1].long(), batch[:, 1:].long()
+    B, S, T = x.shape
+    e = F.embedding(x, sd["net.embed_tokens.weight"].double(), padding_idx=cfg.pad_id).sum(-2)
+    hidden = stack64(sd, cfg.net, e, *rope_net)
+    if sample_idx is not None:
+        hidden, y = hidden[:, list(sample_idx)], y[:, list(sample_idx)]
+    hidden, y = hidden.reshape(-1, hidden.shape[-1]), y.reshape(-1, T)
+    xe = F.embedding(y[:, :-1], sd["net_token.embed_tokens.weight"].double(), padding_idx=cfg.pad_id)
+    h = stack64(sd, cfg.net_token, torch.cat([hidden[:, None], xe], 1), *rope_tok)
+    logits = F.linear(h, sd["lm_head.weight"].double())
+    return F.cross_entropy(logits.reshape(-1, logits.shape[-1]), y.reshape(-1), ignore_index=cfg.pad_id)
+
+
+def grad_kind(name: str, t: torch.Tensor) -> str:
+    """Which per-block metrics a gradient gets: "dx" (input gradient, per token row), "table" (embedding / lm_head:
+    relative norm only), "lora" (A / B), "qkv" (row blocks are heads), "o" (column blocks are heads), "mlp", "norm"."""
+    if name.startswith("dx"):
+        return "dx"
+    if "embed_tokens" in name or name.startswith("lm_head"):
+        return "table"
+    if ".lora_" in name:
+        return "lora"
+    if any(f".{t}_proj." in name for t in "qkv"):
+        return "qkv"
+    if ".o_proj." in name:
+        return "o"
+    if ".mlp." in name:
+        return "mlp"
+    if t.dim() == 1:
+        return "norm"
+    raise ValueError(f"no gradient kind for {name}")
+
+
+def _rel(a, b):
+    return float((a - b).norm() / b.norm().clamp_min(1e-30))
+
+
+def grad_errors(got: torch.Tensor, ref: torch.Tensor, kind: str, n_head: int) -> dict:
+    """Errors of one gradient against its fp64 reference.
+
+    fro : relative Frobenius error of the whole tensor (every kind)
+    row  : worst relative error of an output row (matrices except tables)
+    dxrow: worst relative error of a token row of dx, with its floor at 1e-3 x the median row norm, as the decode groups
+           score hidden rows
+    head : worst relative error of one head's block -- D rows of dWq / dWk / dWv, D columns of dWo
+    elem : worst |error| of one element of a norm weight's gradient over that vector's norm"""
+    y, r = got.double(), ref.double()
+    out = {"fro": _rel(y, r)}
+    if not torch.isfinite(y).all():
+        out["fro"] = float("inf")
+    if kind == "dx":
+        out["dxrow"] = row_worst(y, r, floor_frac=1e-3)
+    elif kind in ("qkv", "o", "mlp", "lora"):
+        out["row"] = row_worst(y, r)
+    if kind in ("qkv", "o"):
+        blocks = zip(y.chunk(n_head, 0), r.chunk(n_head, 0)) if kind == "qkv" else zip(y.chunk(n_head, 1), r.chunk(n_head, 1))
+        out["head"] = max(_rel(a, b) for a, b in blocks)
+    if kind == "norm":
+        out["elem"] = float((y - r).abs().max() / r.norm().clamp_min(1e-30))
+    return out
+
+
+def grad_report(got: dict, ref: dict, tag: str, n_head=None, floor: dict = None, show=True) -> dict:
+    """Every gradient of `got` ({name: tensor}; "dx..." for input gradients) scored against `ref` (fp64) by
+    grad_errors -> the worst value of each metric over the tensors, as "<metric>_<tag>", and with `floor` (the same
+    gradients from the bf16 eager oracle) the worst ratio of a tensor's error to that tensor's floor error, as
+    "floor_ratio_<metric>_<tag>".  n_head: {name: heads} or one count for every tensor.  Also "min:" counters
+    n_tensors_<tag> and, where heads were scored, n_heads_<tag>.  show: print the worst tensor of every metric."""
+    worst, where = {}, {}
+    n_heads = 0
+    for name, g in got.items():
+        kind = grad_kind(name, g)
+        nh = n_head.get(name) if isinstance(n_head, dict) else n_head
+        e = grad_errors(g, ref[name], kind, nh)
+        vals = dict(e)
+        if floor is not None:
+            f = grad_errors(floor[name], ref[name], kind, nh)
+            vals.update({f"floor_ratio_{k}": v / max(f[k], 1e-30) for k, v in e.items()})
+        n_heads += nh if kind in ("qkv", "o") else 0
+        for k, v in vals.items():
+            if k not in worst or not v <= worst[k]:
+                worst[k], where[k] = v, name
+    if show:
+        for k in worst:
+            print(f"  {tag}: worst {k} = {worst[k]:.3e} at {where[k]}")
+    out = {f"{k}_{tag}": v for k, v in worst.items()}
+    out[f"n_tensors_{tag}"] = float(len(got))
+    if n_heads:
+        out[f"n_heads_{tag}"] = float(n_heads)
+    return out

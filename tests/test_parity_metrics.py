@@ -52,7 +52,7 @@ def test_renamed_metric_of_a_group_fails():
 def _bound_tables():
     for name, g in G.GROUPS.items():
         yield name, g.bounds, g.info
-    for mod in ("test_gpu_ragged", "test_gpu_recompute", "test_gpu_sample_seq"):
+    for mod in ("test_gpu_ragged", "test_gpu_recompute", "test_gpu_sample_seq", "test_gpu_backward"):
         yield mod, importlib.import_module(mod).BOUNDS, ()
 
 
